@@ -1,4 +1,4 @@
-"""auralis_b200 — B200-native XTTSv2 hot path behind the Auralis engine/plugin API.
+"""auralis_b200 — H100-native XTTSv2 hot path behind the Auralis engine/plugin API.
 
 Public surface mirrors the reference (`/root/reference/src/auralis/__init__.py`):
 ``TTS``, ``TTSRequest``, ``TTSOutput``.  Imports are lazy so that ``import auralis_b200``

@@ -1,4 +1,4 @@
-"""Builds libxtts_b200.so in-tree with nvcc for sm_100a (no torch in the link line).
+"""Builds libxtts_b200.so in-tree with nvcc for sm_90a (no torch in the link line).
 
 `python -m auralis_b200.build` or `build_native()`; nvcc cross-compiles without a GPU.
 """
@@ -11,8 +11,9 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libxtts_b200.so")
-SOURCES = ["engine.cu", "gpt_kernels.cu", "gemm_simt.cu", "gemm_tcgen05.cu", "gemm_tcgen05_2cta.cu", "vocoder.cu", "conv1d_tc.cu", "cond.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+SOURCES = ["engine.cu", "gpt_kernels.cu", "gemm_simt.cu", "gemm_wgmma.cu", "gemm_wgmma_wide.cu", "vocoder.cu", "conv1d_tc.cu", "cond.cu"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = [*ARCH, "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-pthread"]
 
 
@@ -51,7 +52,7 @@ def build_native(force: bool = False, verbose: bool = False) -> str:
             raise RuntimeError(f"nvcc failed on {src}")
         if verbose and out:
             print(out.decode())
-    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-Xcompiler", "-pthread", "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-Xcompiler", "-pthread", *ARCH]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)
     if r.returncode != 0:
         sys.stderr.write(r.stdout.decode())

@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels of the XTTSv2 hot path.
+// Shared helpers for the sm_90a kernels of the XTTSv2 hot path.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -93,24 +93,22 @@ struct KernelCtx {
     bool use_pdl = true;
     int voc_sm_cap = 0;           // > 0: persistent tensor-core conv grids take at most this many SMs (set per vocoder batch)
     int attn_ctas_per_sm = 0;     // 0 = uncapped decode-attention grid; > 0: at most this many CTAs per SM
-    int gemm_decode_bn = 0;       // 0 = heuristic; 32/64/128 forces the tile width of decode-shaped tcgen05 GEMMs
-    int conv_epi_groups = 2;      // 1 or 2 epilogue warpgroups in conv1d_tc_kernel
+    int gemm_decode_bn = 0;       // 0 = heuristic; 32/64/128 forces the tile width of decode-shaped tensor-core GEMMs
     int attn_warps = 4;           // warps per (row, head) item of the bf16 decode attention (4, or 8: measured slower, run 7)
     int attn_bulk = 0;            // > 0: 16-bit decode attention streams cache pages with cp.async.bulk, this many CTAs per SM
     int attn_stages = 8;          // ring depth of that kernel (8 KB per stage)
     int attn_l2_pages = 0;        // register-load decode attention: every warp prefetches the page this many of its pages ahead into L2
     int attn_l2_ahead = 1;        // that kernel prefetches the next item's pages into L2 (cp.async.bulk.prefetch.L2)
     int gemm_deep_ring = 0;       // decode-shaped unsplit GEMMs use a ring that fills the SM (BN 32: 10 stages, BN 64: 8) instead of 5 / 4
-    int gemm_l2_prefetch = 0;     // one-tile tcgen05 GEMM: weight tiles beyond the first ring pass are prefetched into L2 before the dependency wait
-    int gemm_2cta = 1;            // large shapes (M >= 256) go to the persistent CTA-pair kernel (gemm_tcgen05_2cta.cu)
+    int gemm_l2_prefetch = 0;     // one-tile GEMM: weight tiles beyond the first ring pass are prefetched into L2 before the dependency wait
+    int gemm_wide = 4;            // large shapes (M >= 256) go to the persistent wide-tile kernel (gemm_wgmma_wide.cu) with this ring depth (2-4); 0: off
 };
 #define g_prof (::xtts::kctx().prof)
 #define g_use_pdl (::xtts::kctx().use_pdl)
 #define g_voc_sm_cap (::xtts::kctx().voc_sm_cap)
 #define g_attn_ctas_per_sm (::xtts::kctx().attn_ctas_per_sm)
 #define g_gemm_decode_bn (::xtts::kctx().gemm_decode_bn)
-#define g_conv_epi_groups (::xtts::kctx().conv_epi_groups)
-#define g_gemm_2cta (::xtts::kctx().gemm_2cta)
+#define g_gemm_wide (::xtts::kctx().gemm_wide)
 #define g_attn_warps (::xtts::kctx().attn_warps)
 #define g_gemm_l2_prefetch (::xtts::kctx().gemm_l2_prefetch)
 #define g_gemm_deep_ring (::xtts::kctx().gemm_deep_ring)
@@ -126,6 +124,20 @@ inline bool first_on_device(bool (&done)[64]) {
     if (dev < 0 || dev >= 64 || done[dev]) return false;
     done[dev] = true;
     return true;
+}
+
+// SM count of the current CUDA device (persistent grids, tile heuristics); cached per device
+inline int sm_count() {
+    static int n[64] = {};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev < 0 || dev >= 64) dev = 0;
+    if (n[dev] <= 0 && cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) {
+        (void)cudaGetLastError();
+        n[dev] = 0;
+        throw CudaError("cudaDevAttrMultiProcessorCount query failed");
+    }
+    return n[dev];
 }
 
 struct ProfScope {
@@ -151,9 +163,9 @@ struct ProfScope {
     }
 };
 inline const char* kernel_family_name(int f) {
-    static const char* n[KF_COUNT] = {"gemm_bf16_tcgen05", "gemm_f32", "attn_decode_paged", "attn_prefill", "layernorm",
+    static const char* n[KF_COUNT] = {"gemm_bf16_wgmma", "gemm_f32", "attn_decode_paged", "attn_prefill", "layernorm",
                                       "sample", "kv_write", "embed", "conv1d", "conv_transpose1d", "conv_post_tanh",
-                                      "interp", "conditioning", "misc", "conv1d_tc_f16_tcgen05", "decode_chain_tcgen05"};
+                                      "interp", "conditioning", "misc", "conv1d_tc_f16_wgmma", "decode_chain_wgmma"};
     return (f >= 0 && f < KF_COUNT) ? n[f] : "?";
 }
 
@@ -183,7 +195,7 @@ __device__ __forceinline__ void trace_pt(int id, int phase) {
 
 // ---- programmatic dependent launch (PDL): the decode step is a chain of ~200 short dependent kernels; with the
 // programmatic-serialization attribute kernel N+1 is launched while kernel N still runs, does its prologue (barrier
-// init, TMEM alloc, weight-tile prefetch) and only blocks at griddepcontrol.wait before touching N's outputs.
+// init, weight-tile prefetch) and only blocks at griddepcontrol.wait before touching N's outputs.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
@@ -198,7 +210,7 @@ struct DepFlag {
     unsigned target = 0;                // its value once every producer CTA has arrived
     unsigned* arrive = nullptr;         // this kernel's own counter (nullptr: nobody polls it)
 };
-__device__ __forceinline__ void dep_wait(const DepFlag& d, int tag) {
+__device__ __forceinline__ void dep_wait(const DepFlag& d) {
     if (d.wait == nullptr) { pdl_wait(); return; }
     const long long t0 = clock64();
     int polls = 0;
@@ -207,10 +219,7 @@ __device__ __forceinline__ void dep_wait(const DepFlag& d, int tag) {
         asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(d.wait) : "memory");
         if (v >= d.target) break;
         __nanosleep(polls < 8 ? 100 : 400);          // hundreds of CTAs poll one line that the producers are also adding to
-        if ((++polls & 255) == 0 && clock64() - t0 > 4000000000LL) {
-            printf("dep_wait watchdog (tag %d, block %d, have %u want %u)\n", tag, blockIdx.x, v, d.target);
-            __trap();
-        }
+        if ((++polls & 255) == 0 && clock64() - t0 > 4000000000LL) __trap();     // watchdog (no printf: see hopper.cuh)
     }
 }
 // every thread that stored results calls this; `leader` (one thread, after a CTA barrier) publishes the CTA's arrival

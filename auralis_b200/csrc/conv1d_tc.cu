@@ -1,140 +1,36 @@
-// Dilated Conv1d ("same" padding) as an implicit GEMM on the 5th-gen tensor cores (fast mode of the vocoder).
+// Dilated Conv1d ("same" padding) as an implicit GEMM on the Hopper tensor cores (fast mode of the vocoder).
 //
 //   y[co][t] = bias[co] + cbias[co] + resid[co][t] + sum_j sum_ci W_j[co][ci] * a[ci][t + (j-c)*d]
 //
 // where `a` is the ALREADY ACTIVATED fp16 input kept in HBM in the tensor-core operand layout
 //   "atoms":  [C/8 plane][PADL + L + PADR time rows][8 channels]   (16-byte atoms, zero pads)
-// which is byte-for-byte the UMMA no-swizzle K-major image (SBO = 128 B => rows linear in time), so
+// which is byte-for-byte the wgmma no-swizzle K-major image (8-row core matrices 128 B apart => rows linear in time), so
 //   * the A tile of a ci-chunk is `CK/8` contiguous cp.async.bulk copies (one per plane), a tap is a start-address
 //     shift of j*d rows inside the staged tile (no im2col, no conversion work in this kernel);
 //   * weights are pre-packed per (ci-chunk, tap) into the same layout: one bulk copy per tile.
-// tcgen05.mma.cta_group::1.kind::f16, fp32 accumulators in TMEM: NACC accumulators (128 time rows each) share every
-// weight tile.  The epilogue (lane = time step) can emit
+// wgmma.mma_async m64nNk16 (f16 x f16 -> f32), accumulators in registers: each of the two consumer warpgroups owns MB
+// blocks of 64 time rows (MB * N / 2 accumulators per thread), so a tile is 128 * MB time rows x N output channels and
+// every staged weight tile feeds all of them.  The consumers' epilogue (straight from the accumulators) can emit
 //   * out32: fp32 channel-major [C][L]  (store or accumulate)  — the residual stream / MRF sum
 //   * out16: lrelu(y, slope_out) as fp16 atoms                 — the next conv's operand, written once, read once.
-// Warp roles: 4*EG epilogue warps (TMEM lane quarter = warp % 4; EG = 1 or 2 warpgroups), then one bulk-copy producer
-// warp and one MMA-issuer warp.
+// Warp roles: warps 0-7 consumer warpgroups (MMA + epilogue), warp 8 bulk-copy producer.  Persistent CTAs walk the tile list.
 //
 // Replaces the cuDNN fp16-autocast Conv1d calls of HifiganGenerator.forward / ResBlock1.forward
 // (hifigan_decoder.py:76-91,241-259; the reference runs them in fp16 under torch.amp.autocast on GPU, App. B.8).
 #include <algorithm>
 #include <vector>
 
+#include "hopper.cuh"
 #include "kernels.h"
 
 namespace xtts {
 namespace {
 
-// warps [0, 4*EG) epilogue (EG warpgroups share a tile's accumulator chunks), warp 4*EG producer, warp 4*EG+1 MMA issuer
-constexpr int threads_tc(int eg) { return (4 * eg + 2) * 32; }
+using namespace hop;
+
+constexpr int kConsumers = 256, kThreadsTc = kConsumers + 32, kConsumerWarps = kConsumers / 32;
 constexpr int SA = 2, SB = 3;          // ring depths (activation chunks, weight tiles)
-
-__device__ __forceinline__ uint32_t s_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void bar_init(uint64_t* b, uint32_t c) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s_u32(b)), "r"(c) : "memory");
-}
-__device__ __forceinline__ void bar_arrive(uint64_t* b) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(s_u32(b)) : "memory");
-}
-__device__ __forceinline__ void bar_expect_tx(uint64_t* b, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(s_u32(b)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool bar_try(uint64_t* b, uint32_t parity) {
-    uint32_t ok;
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(ok) : "r"(s_u32(b)), "r"(parity) : "memory");
-    return ok != 0;
-}
-__device__ __forceinline__ void bar_wait(uint64_t* b, uint32_t parity, int tag) {
-    const long long t0 = clock64();
-    int polls = 0;
-    while (!bar_try(b, parity)) {
-        if ((++polls & 1023) == 0 && clock64() - t0 > 4000000000LL) {
-            printf("conv1d_tc: mbarrier watchdog (tag %d, block %d,%d,%d thread %d)\n", tag, blockIdx.x, blockIdx.y, blockIdx.z,
-                   threadIdx.x);
-            __trap();
-        }
-    }
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(s_u32(dst)), "l"(src), "r"(bytes), "r"(s_u32(bar)) : "memory");
-}
-// no-swizzle K-major descriptor: rows 16 B apart (SBO = 128 B per 8 rows), the two 8-element K halves `lbo` bytes apart
-__device__ __forceinline__ uint64_t desc_nosw(uint32_t addr, uint32_t lbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)(128 >> 4) << 32;
-    d |= (uint64_t)1 << 46;                   // descriptor version (Blackwell); layout_type = 0 (SWIZZLE_NONE)
-    return d;
-}
-__device__ __forceinline__ void mma_f16(uint32_t tmem_d, uint64_t ad, uint64_t bd, uint32_t idesc, uint32_t acc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(tmem_d), "l"(ad), "l"(bd), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void mma_commit(uint64_t* b) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(s_u32(b)) : "memory");
-}
 __device__ __forceinline__ float lrelu_s(float v, float slope) { return v > 0.f ? v : v * slope; }
-
-// Transposed-conv epilogue of one 32-column chunk (co-major GEMM columns: 32/U channels x U phases).  r[c*U + p] is channel
-// co0 + c at output step tb + p.  All register indices are compile-time (no local-memory array).
-template <int U>
-__device__ __forceinline__ void convT_store(const uint32_t (&r)[32], const float* __restrict__ sbc, float* __restrict__ out32,
-                                            uint4* __restrict__ out16, int co0, int tb, int Lout, size_t Ls, int lpad_out,
-                                            float scale16, float slope) {
-    constexpr int CPC = 32 / U;
-    const bool inner = tb >= 0 && tb + U <= Lout;
-    float v[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]) + sbc[i];
-    if (out32) {
-        if (inner) {
-#pragma unroll
-            for (int c = 0; c < CPC; ++c) {
-                float* op = out32 + (size_t)(co0 + c) * Ls + tb;
-                if constexpr (U == 8) {
-                    reinterpret_cast<float4*>(op)[0] = make_float4(v[8 * c], v[8 * c + 1], v[8 * c + 2], v[8 * c + 3]);
-                    reinterpret_cast<float4*>(op)[1] = make_float4(v[8 * c + 4], v[8 * c + 5], v[8 * c + 6], v[8 * c + 7]);
-                } else if constexpr (U == 4) {
-                    reinterpret_cast<float2*>(op)[0] = make_float2(v[4 * c], v[4 * c + 1]);
-                    reinterpret_cast<float2*>(op)[1] = make_float2(v[4 * c + 2], v[4 * c + 3]);
-                } else {
-#pragma unroll
-                    for (int p = 0; p < U; ++p) op[p] = v[U * c + p];
-                }
-            }
-        } else {
-#pragma unroll
-            for (int c = 0; c < CPC; ++c)
-#pragma unroll
-                for (int p = 0; p < U; ++p) {
-                    const int tt = tb + p;
-                    if (tt >= 0 && tt < Lout) out32[(size_t)(co0 + c) * Ls + tt] = v[U * c + p];
-                }
-        }
-    }
-    if (out16) {
-        // atoms [C/8][t][8]: per output step the lane owns CPC consecutive channels; groups of 4 -> 8-byte stores
-        __half* ah = reinterpret_cast<__half*>(out16);
-#pragma unroll
-        for (int p = 0; p < U; ++p) {
-            const int tt = tb + p;
-            if (tt < 0 || tt >= Lout) continue;
-#pragma unroll
-            for (int c4 = 0; c4 < CPC; c4 += 4) {
-                const int co = co0 + c4;
-                __half2 h0 = __floats2half2_rn(lrelu_s(v[(c4 + 0) * U + p] * scale16, slope), lrelu_s(v[(c4 + 1) * U + p] * scale16, slope));
-                __half2 h1 = __floats2half2_rn(lrelu_s(v[(c4 + 2) * U + p] * scale16, slope), lrelu_s(v[(c4 + 3) * U + p] * scale16, slope));
-                uint2 pk;
-                pk.x = *reinterpret_cast<uint32_t*>(&h0); pk.y = *reinterpret_cast<uint32_t*>(&h1);
-                *reinterpret_cast<uint2*>(ah + (((size_t)(co / 8) * lpad_out + (tt + kAtomPadL)) * 8 + (co % 8))) = pk;
-            }
-        }
-    }
-}
 
 struct ConvTcParams {
     const __half* a16;       // input atoms  [batch][Cin/8][lpad][8]
@@ -146,24 +42,22 @@ struct ConvTcParams {
     float slope_out, scale16;   // out16 = lrelu(y * scale16, slope_out)
     int center;              // tap j reads a[t + (j - center) * dil]
     int up;                  // 0: Conv1d.  u > 0: ConvTranspose1d(stride u, kernel 2u, pad u/2) as u two-tap phases:
-                             //    GEMM channel n' = phase * Cr + co, GEMM row s -> output step s*u + phase - u/2
+                             //    GEMM channel n' = co * u + phase, GEMM row s -> output step s*u + phase - u/2
     int Cr, Lout, lpad_out;  // real output channels, output length, padded rows of the output atoms
-    int N;          // output channels per CTA (<= 256, multiple of 32)
     int CK;         // input channels per chunk (<= 64, multiple of 16)
-    int rows;       // time rows staged per chunk = 128*NACC + (K-1)*dil
+    int rows;       // time rows staged per chunk = tile_rows + (K-1)*dil
     int cbias_bs;   // elements between the speaker-bias vectors of consecutive batch items
     int tile_rows, tiles_n, batch; // persistent-CTA tile space: per item ceil(rows_i / tile_rows) x tiles_n tiles
     int item_L[kVocMaxItems];      // ragged batch: input time steps of each item (<= L; buffers are strided by L)
 };
 
-template <int NACC, int EG>
-__global__ void __launch_bounds__(threads_tc(EG), 1)
+// N output channels (GEMM columns) per tile, MB 64-row blocks per consumer warpgroup (tile_rows = 128 * MB)
+template <int N, int MB>
+__global__ void __launch_bounds__(kThreadsTc, 1)
 conv1d_tc_kernel(const ConvTcParams P) {
-    constexpr int kProducerWarp = 4 * EG, kMmaWarp = 4 * EG + 1;
     extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ __align__(8) uint64_t a_full[SA], a_empty[SA], b_full[SB], b_empty[SB], tmem_full[2], tmem_empty[2];
-    __shared__ uint32_t tmem_base_s;
-    __shared__ __align__(16) float sbias[2][256];     // per-tile bias + speaker bias (double buffered across tiles)
+    __shared__ __align__(8) uint64_t a_full[SA], a_empty[SA], b_full[SB], b_empty[SB];
+    __shared__ __align__(16) float sbias[2][N];     // per-tile bias + speaker bias (double buffered across tiles)
     __shared__ int s_cum[kVocMaxItems + 1], s_len[kVocMaxItems];   // ragged batch: first tile / input length of every item
 
     trace_pt(TR_CONV, 0);
@@ -172,16 +66,10 @@ conv1d_tc_kernel(const ConvTcParams P) {
     const int planes = P.CK / 8, ksteps = P.CK / 16, nch = P.Cin / P.CK;
     const uint32_t a_plane = (uint32_t)P.rows * 16u;               // bytes per ci-plane of a staged chunk
     const uint32_t a_stage = a_plane * planes;
-    const uint32_t b_plane = (uint32_t)P.N * 16u;
+    constexpr uint32_t b_plane = (uint32_t)N * 16u;
     const uint32_t b_stage = b_plane * planes;
     uint8_t* sA = smem;
     uint8_t* sB = smem + ((SA * a_stage + 127) & ~127u);
-    // persistent CTA: tiles = (batch item, C_out tile, time tile), strided by the grid; accumulators are double
-    // buffered in TMEM when two sets fit (NACC*N <= 256 columns), so the epilogue of tile i overlaps the MMAs of tile i+1
-    const int acc_cols = NACC * P.N;
-    const int nbuf = (2 * acc_cols <= 512) ? 2 : 1;
-    uint32_t tm_cols = 32;
-    while (tm_cols < (uint32_t)(nbuf * acc_cols)) tm_cols <<= 1;
     const int tiles_n = P.tiles_n;
     const int extra_rows = P.up ? 1 : 0;             // a transposed conv also consumes the zero row x[L]
 
@@ -193,21 +81,13 @@ conv1d_tc_kernel(const ConvTcParams P) {
             c += (Li > 0 ? ceil_div(Li + extra_rows, P.tile_rows) : 0) * tiles_n;
         }
         s_cum[P.batch] = c;
-        for (int i = 0; i < SA; ++i) { bar_init(&a_full[i], 1); bar_init(&a_empty[i], 1); }
-        for (int i = 0; i < SB; ++i) { bar_init(&b_full[i], 1); bar_init(&b_empty[i], 1); }
-        for (int i = 0; i < 2; ++i) { bar_init(&tmem_full[i], 1); bar_init(&tmem_empty[i], 128 * EG); }
+        for (int i = 0; i < SA; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], kConsumerWarps); }
+        for (int i = 0; i < SB; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], kConsumerWarps); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == kMmaWarp) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(&tmem_base_s)), "r"(tm_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = tmem_base_s;
     const int total_tiles = s_cum[P.batch];
-    // tile -> (batch item, C_out tile, time tile); every role walks the same compact tile list
+    // tile -> (batch item, time tile, C_out tile); every role walks the same compact tile list
     auto decode_tile = [&](int tile, int& zi, int& tx, int& ty, int& Li) {
         zi = 0;
         while (zi + 1 < P.batch && tile >= s_cum[zi + 1]) ++zi;
@@ -217,158 +97,7 @@ conv1d_tc_kernel(const ConvTcParams P) {
         tx = local % tt; ty = local / tt;
     };
 
-    if (warp < 4 * EG) {
-        // ------------------------------------------------ epilogue: warp q owns TMEM lanes [32q, 32q+32) = time rows;
-        // the EG warpgroups take alternate 32-column chunks of the tile.  Per tile the per-channel bias (+ speaker bias)
-        // is staged once in shared memory; the residual of the NEXT chunk is requested before the current chunk is
-        // stored (and the first chunk's before the tile's MMAs have finished), so its latency is off the critical path.
-        const int q = warp & 3, grp = warp >> 2, etid = warp * 32 + lane;
-        const int ncn = P.N / 32, nitems = NACC * ncn;
-        const bool has_res = P.resid != nullptr, accum = (P.mode == CONV_ACCUM);
-        const size_t Ls = (size_t)P.Lout;
-        float rs[32];
-        int lt = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
-            int zi, tx, ty, Li;
-            decode_tile(tile, zi, tx, ty, Li);
-            const size_t zo = (size_t)zi;
-            const int row_limit = Li + extra_rows, Lout_i = P.up ? Li * P.up : Li;
-            const int T0 = tx * (128 * NACC), n0 = ty * P.N;
-            float* out32 = P.out32 ? P.out32 + zo * P.Cr * P.Lout : nullptr;
-            const float* resid = has_res ? P.resid + zo * P.Cr * P.Lout : nullptr;
-            const float* cbias = P.cbias ? P.cbias + zo * P.cbias_bs : nullptr;
-            uint4* out16 = P.out16 ? reinterpret_cast<uint4*>(P.out16) + zo * (size_t)(P.Cr / 8) * P.lpad_out : nullptr;
-            float* sb = sbias[lt & 1];
-            for (int j = etid; j < P.N; j += EG * 128) {
-                const int co = P.up ? (n0 + j) / P.up : n0 + j;      // GEMM column -> output channel (transposed conv: co * u + phase)
-                sb[j] = (P.bias ? __ldg(P.bias + co) : 0.f) + (cbias ? __ldg(cbias + co) : 0.f);
-            }
-            // geometry of a 32-column chunk (Conv1d: 32 output channels at the lane's time step)
-            auto geom = [&](int item, int& a, int& nc, int& cb, int& t, bool& valid) {
-                a = item / ncn; nc = item - a * ncn;
-                const int srow = T0 + a * 128 + q * 32 + lane;
-                cb = n0 + nc * 32;
-                t = srow;
-                valid = srow < row_limit && t < Lout_i;
-            };
-            int a, nc, cb, t; bool valid;
-            geom(grp, a, nc, cb, t, valid);
-            if (P.up) {
-                // ---- ConvTranspose1d: GEMM column n' = co * u + phase (co-major), GEMM row s -> output steps
-                // s*u - u/2 + [0, u).  A 32-column chunk is 32/u channels x all u phases: per channel the lane holds u
-                // CONSECUTIVE output steps, stored as whole vectors (whole 32-byte sectors once a warp's neighbouring lanes
-                // have written theirs) instead of one float per phase pass.
-                asm volatile("bar.sync 1, %0;" ::"r"(EG * 128) : "memory");
-                const int ab_ = lt % nbuf;
-                bar_wait(&tmem_full[ab_], (uint32_t)((lt / nbuf) & 1), 4);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const int u = P.up;
-#pragma unroll 1
-                for (int item = grp; item < nitems; item += EG) {
-                    const int a2 = item / ncn, nc2 = item - a2 * ncn;
-                    uint32_t r[32];
-                    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(ab_ * acc_cols + a2 * P.N + nc2 * 32);
-                    asm volatile(
-                        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                        : "r"(taddr) : "memory");
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                    const int srow = T0 + a2 * 128 + q * 32 + lane;
-                    if (srow >= row_limit) continue;
-                    const float* sbc = sb + nc2 * 32;
-                    const int co0 = (n0 + nc2 * 32) / u;
-                    const int tb = srow * u - u / 2;                     // first output step of this lane
-                    if (u == 8) convT_store<8>(r, sbc, out32, out16, co0, tb, Lout_i, Ls, P.lpad_out, P.scale16, P.slope_out);
-                    else if (u == 4) convT_store<4>(r, sbc, out32, out16, co0, tb, Lout_i, Ls, P.lpad_out, P.scale16, P.slope_out);
-                    else convT_store<2>(r, sbc, out32, out16, co0, tb, Lout_i, Ls, P.lpad_out, P.scale16, P.slope_out);
-                }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                bar_arrive(&tmem_empty[ab_]);
-                continue;
-            }
-            if (has_res && valid) {
-                const float* rp = resid + (size_t)cb * Ls + t;
-#pragma unroll
-                for (int i = 0; i < 32; ++i) rs[i] = rp[i * Ls];
-            }
-            asm volatile("bar.sync 1, %0;" ::"r"(EG * 128) : "memory");      // bias table visible to every epilogue warp
-            const int ab = lt % nbuf;
-            bar_wait(&tmem_full[ab], (uint32_t)((lt / nbuf) & 1), 4);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-            for (int item = grp; item < nitems; item += EG) {
-                uint32_t r[32];
-                const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(ab * acc_cols + a * P.N + nc * 32);
-                asm volatile(
-                    "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                    : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                      "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                      "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                      "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                    : "r"(taddr) : "memory");
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                float v[32];
-                const float4* sb4 = reinterpret_cast<const float4*>(sb + nc * 32);
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const float4 b4 = sb4[i];
-                    v[4 * i] = __uint_as_float(r[4 * i]) + b4.x;         v[4 * i + 1] = __uint_as_float(r[4 * i + 1]) + b4.y;
-                    v[4 * i + 2] = __uint_as_float(r[4 * i + 2]) + b4.z; v[4 * i + 3] = __uint_as_float(r[4 * i + 3]) + b4.w;
-                }
-                if (has_res) {
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) v[i] += rs[i];          // (rows outside the signal carry garbage: never stored)
-                }
-                // next chunk: geometry + residual request, in flight while this chunk is stored
-                const bool cur_valid = valid;
-                const int cur_cb = cb, cur_t = t;
-                if (item + EG < nitems) {
-                    geom(item + EG, a, nc, cb, t, valid);
-                    if (has_res && valid) {
-                        const float* rp = resid + (size_t)cb * Ls + t;
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) rs[i] = rp[i * Ls];
-                    }
-                }
-                if (cur_valid) {
-                    if (out32) {
-                        float* op = out32 + (size_t)cur_cb * Ls + cur_t;
-                        if (accum) {
-#pragma unroll
-                            for (int i = 0; i < 32; ++i) v[i] += op[i * Ls];     // all loads before the first store
-                        }
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) op[i * Ls] = v[i];
-                    }
-                    if (out16) {                                     // (after an accumulate: the activated SUM)
-                        uint4* ap = out16 + (size_t)(cur_cb / 8) * P.lpad_out + (cur_t + kAtomPadL);
-#pragma unroll
-                        for (int g = 0; g < 4; ++g) {
-                            float w8[8];
-#pragma unroll
-                            for (int e = 0; e < 8; ++e) w8[e] = lrelu_s(v[8 * g + e] * P.scale16, P.slope_out);
-                            __half2 h0 = __floats2half2_rn(w8[0], w8[1]), h1 = __floats2half2_rn(w8[2], w8[3]);
-                            __half2 h2 = __floats2half2_rn(w8[4], w8[5]), h3 = __floats2half2_rn(w8[6], w8[7]);
-                            uint4 pk;
-                            pk.x = *reinterpret_cast<uint32_t*>(&h0); pk.y = *reinterpret_cast<uint32_t*>(&h1);
-                            pk.z = *reinterpret_cast<uint32_t*>(&h2); pk.w = *reinterpret_cast<uint32_t*>(&h3);
-                            ap[(size_t)g * P.lpad_out] = pk;
-                        }
-                    }
-                }
-            }
-            // this accumulator set is drained: hand it back to the MMA warp
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            bar_arrive(&tmem_empty[ab]);
-        }
-    } else if (warp == kProducerWarp) {
+    if (warp == kConsumerWarps) {
         // ------------------------------------------------ producer: activation planes + weight tiles, all bulk copies
         if (lane == 0) {
             int ita = 0, itb = 0;
@@ -376,69 +105,143 @@ conv1d_tc_kernel(const ConvTcParams P) {
                 int zi, tx, ty, Li;
                 decode_tile(tile, zi, tx, ty, Li);
                 const size_t zo = (size_t)zi;
-                const int T0 = tx * (128 * NACC);
+                const int T0 = tx * P.tile_rows;
                 const __half* wsrc = P.wblob + (size_t)ty * nch * P.K * (b_stage / 2);
                 const __half* asrc = P.a16 + zo * (size_t)(P.Cin / 8) * P.lpad * 8;
                 const int row0 = T0 - halo + kAtomPadL;             // first staged time row inside the padded plane
                 int wt = 0;
                 for (int c = 0; c < nch; ++c, ++ita) {
                     const int sa = ita % SA;
-                    bar_wait(&a_empty[sa], ((ita / SA) & 1) ^ 1, 1);
-                    bar_expect_tx(&a_full[sa], a_stage);
+                    mbar_wait(&a_empty[sa], ((ita / SA) & 1) ^ 1);
+                    mbar_expect_tx(&a_full[sa], a_stage);
                     for (int p = 0; p < planes; ++p)
                         bulk_g2s(sA + (size_t)sa * a_stage + (size_t)p * a_plane,
                                  asrc + ((size_t)(c * planes + p) * P.lpad + row0) * 8, a_plane, &a_full[sa]);
                     for (int j = 0; j < P.K; ++j, ++itb, ++wt) {
                         const int s = itb % SB;
-                        bar_wait(&b_empty[s], ((itb / SB) & 1) ^ 1, 2);
-                        bar_expect_tx(&b_full[s], b_stage);
+                        mbar_wait(&b_empty[s], ((itb / SB) & 1) ^ 1);
+                        mbar_expect_tx(&b_full[s], b_stage);
                         bulk_g2s(sB + (size_t)s * b_stage, wsrc + (size_t)wt * (b_stage / 2), b_stage, &b_full[s]);
                     }
                 }
             }
         }
     } else {
-        // ------------------------------------------------ MMA issuer
-        if (lane == 0) {
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(P.N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);   // f16 x f16 -> f32
-            int ita = 0, itb = 0, lt = 0;
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
-                const int ab = lt % nbuf;
-                bar_wait(&tmem_empty[ab], (uint32_t)(((lt / nbuf) & 1) ^ 1), 6);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t acc0 = tmem_base + (uint32_t)(ab * acc_cols);
-                for (int c = 0; c < nch; ++c, ++ita) {
-                    const int sa = ita % SA;
-                    bar_wait(&a_full[sa], (ita / SA) & 1, 3);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t a_addr = s_u32(sA + (size_t)sa * a_stage);
-                    for (int j = 0; j < P.K; ++j, ++itb) {
-                        const int sb = itb % SB;
-                        bar_wait(&b_full[sb], (itb / SB) & 1, 5);
-                        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                        const uint32_t b_addr = s_u32(sB + (size_t)sb * b_stage);
-                        for (int k = 0; k < ksteps; ++k) {
-                            const uint64_t bd = desc_nosw(b_addr + (uint32_t)(2 * k) * b_plane, b_plane);
-#pragma unroll
-                            for (int a = 0; a < NACC; ++a) {
-                                const uint64_t ad = desc_nosw(a_addr + (uint32_t)(2 * k) * a_plane + (uint32_t)(a * 128 + j * P.dil) * 16u, a_plane);
-                                mma_f16(acc0 + (uint32_t)(a * P.N), ad, bd, idesc, (c | j | k) != 0 ? 1u : 0u);
-                            }
-                        }
-                        mma_commit(&b_empty[sb]);
-                    }
-                    mma_commit(&a_empty[sa]);
-                }
-                mma_commit(&tmem_full[ab]);
+        // ------------------------------------------------ consumer warpgroup wg: time rows [T0 + 64*MB*wg, +64*MB) of a tile.
+        // Weight slots are handed back one tap late (after the next tap's wgmmas are issued), so the tensor cores never
+        // drain between taps; an activation slot is handed back with the last weight slot of its chunk.
+        const int wg = warp >> 2, etid = threadIdx.x;
+        const bool has_res = P.resid != nullptr, accum = (P.mode == CONV_ACCUM);
+        const size_t Ls = (size_t)P.Lout;
+        int ita = 0, itb = 0, lt = 0;
+        float acc[MB][N / 2];
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
+            int zi, tx, ty, Li;
+            decode_tile(tile, zi, tx, ty, Li);
+            const size_t zo = (size_t)zi;
+            const int row_limit = Li + extra_rows, Lout_i = P.up ? Li * P.up : Li;
+            const int T0 = tx * P.tile_rows, n0 = ty * N;
+            const float* cbias = P.cbias ? P.cbias + zo * P.cbias_bs : nullptr;
+            float* sb = sbias[lt & 1];
+            for (int j = etid; j < N; j += kConsumers) {
+                const int co = P.up ? (n0 + j) / P.up : n0 + j;      // GEMM column -> output channel (transposed conv: co * u + phase)
+                sb[j] = (P.bias ? __ldg(P.bias + co) : 0.f) + (cbias ? __ldg(cbias + co) : 0.f);
             }
+#pragma unroll
+            for (int m = 0; m < MB; ++m)
+#pragma unroll
+                for (int i = 0; i < N / 2; ++i) acc[m][i] = 0.f;
+            const uint32_t row_off = (uint32_t)(64 * MB * wg) * 16u;
+            int prev_b = -1, prev_a = -1;
+            auto release = [&] {
+                __syncwarp();
+                if (lane == 0) {
+                    if (prev_b >= 0) mbar_arrive(&b_empty[prev_b]);
+                    if (prev_a >= 0) mbar_arrive(&a_empty[prev_a]);
+                }
+                prev_b = prev_a = -1;
+            };
+            for (int c = 0; c < nch; ++c, ++ita) {
+                const int sa = ita % SA;
+                mbar_wait(&a_full[sa], (ita / SA) & 1);
+                const uint32_t a_addr = smem_u32(sA + (size_t)sa * a_stage) + row_off;
+                for (int j = 0; j < P.K; ++j, ++itb) {
+                    const int sbi = itb % SB;
+                    mbar_wait(&b_full[sbi], (itb / SB) & 1);
+                    const uint32_t b_addr = smem_u32(sB + (size_t)sbi * b_stage);
+                    wgmma_fence();
+                    for (int k = 0; k < ksteps; ++k) {
+                        const uint64_t bd = desc_nosw(b_addr + (uint32_t)(2 * k) * b_plane, b_plane);
+#pragma unroll
+                        for (int m = 0; m < MB; ++m) {
+                            const uint64_t ad = desc_nosw(a_addr + (uint32_t)(2 * k) * a_plane + (uint32_t)(m * 64 + j * P.dil) * 16u, a_plane);
+                            Wgmma<N>::run(acc[m], ad, bd, 1, true);
+                        }
+                    }
+                    wgmma_commit();
+                    wgmma_wait<1>();                             // the previous tap's wgmmas have retired
+#pragma unroll
+                    for (int m = 0; m < MB; ++m) fence_acc(acc[m]);
+                    release();
+                    prev_b = sbi;
+                    if (j == P.K - 1) prev_a = sa;
+                }
+            }
+            wgmma_wait<0>();
+#pragma unroll
+            for (int m = 0; m < MB; ++m) fence_acc(acc[m]);
+            release();
+            asm volatile("bar.sync 1, %0;" ::"r"(kConsumers) : "memory");      // bias table visible to every consumer warp
+
+            // ---- epilogue: a lane holds GEMM columns (col, col+1) of time rows s and s + 8 of each 64-row block
+            float* out32 = P.out32 ? P.out32 + zo * P.Cr * P.Lout : nullptr;
+            const float* resid = has_res ? P.resid + zo * P.Cr * P.Lout : nullptr;
+            __half* out16 = P.out16 ? P.out16 + zo * (size_t)(P.Cr / 8) * P.lpad_out * 8 : nullptr;
+            const int s_base = T0 + 64 * MB * wg + 16 * (warp & 3) + (lane >> 2);
+#pragma unroll
+            for (int m = 0; m < MB; ++m)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int srow = s_base + 64 * m + 8 * h;
+                    if (srow >= row_limit) continue;
+#pragma unroll
+                    for (int i = 0; i < N / 8; ++i) {
+                        const int col = 8 * i + 2 * (lane & 3);
+                        const float v0 = acc[m][4 * i + 2 * h] + sb[col], v1 = acc[m][4 * i + 2 * h + 1] + sb[col + 1];
+                        if (P.up) {
+                            // ---- ConvTranspose1d: column n' = co * u + phase (u even: the pair is one channel, phases p, p + 1)
+                            const int u = P.up, np = n0 + col, co = np / u, p = np - co * u;
+                            const int tt = srow * u - u / 2 + p;
+                            const float w2[2] = {v0, v1};
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                const int t = tt + e;
+                                if (t < 0 || t >= Lout_i) continue;
+                                if (out32) out32[(size_t)co * Ls + t] = w2[e];
+                                if (out16) out16[((size_t)(co / 8) * P.lpad_out + (t + kAtomPadL)) * 8 + (co % 8)] =
+                                               __float2half_rn(lrelu_s(w2[e] * P.scale16, P.slope_out));
+                            }
+                            continue;
+                        }
+                        const int t = srow, co = n0 + col;
+                        if (t >= Lout_i) continue;
+                        float y0 = v0, y1 = v1;
+                        if (has_res) { y0 += resid[(size_t)co * Ls + t]; y1 += resid[(size_t)(co + 1) * Ls + t]; }
+                        if (out32) {
+                            float* op = out32 + (size_t)co * Ls + t;
+                            if (accum) { y0 += op[0]; y1 += op[Ls]; }
+                            op[0] = y0; op[Ls] = y1;
+                        }
+                        if (out16) {                                 // (after an accumulate: the activated SUM)
+                            const __half2 hv = __floats2half2_rn(lrelu_s(y0 * P.scale16, P.slope_out), lrelu_s(y1 * P.scale16, P.slope_out));
+                            *reinterpret_cast<__half2*>(out16 + ((size_t)(co / 8) * P.lpad_out + (t + kAtomPadL)) * 8 + (co % 8)) = hv;
+                        }
+                    }
+                }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
     trace_pt(TR_CONV, 2);
-    if (warp == kMmaWarp) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tm_cols) : "memory");
-    }
 }
 
 // zero the head pad and the rows behind the signal, for every plane of every batch item.  Ragged batches: item i's signal
@@ -470,8 +273,11 @@ ConvTcPlan conv1d_tc_plan(int Cin, int Cout, int K) {
     pl.N = Cout > 256 ? 256 : Cout;
     pl.CK = Cin >= 64 ? 64 : Cin;
     pl.n_tiles = ceil_div(Cout, pl.N);
-    pl.nacc = pl.N >= 128 ? 2 : 4;     // N = 128: two 256-column accumulator sets (double buffered); N = 256: one
-    pl.ok = (Cin % pl.CK == 0) && (pl.CK % 16 == 0) && (pl.N % 32 == 0) && (Cout % pl.N == 0) && K >= 1;
+    // 128-row blocks per tile: MB = nacc 64-row blocks per consumer warpgroup, MB * N / 2 <= 128 accumulator registers
+    // per thread (N = 256: 1, N = 128: 2); narrower tiles stop at 4 (512 rows: the time tiling of atoms_lpad)
+    pl.nacc = pl.N >= 256 ? 1 : (pl.N >= 128 ? 2 : 4);
+    pl.ok = (Cin % pl.CK == 0) && (pl.CK % 16 == 0) && (pl.N == 32 || pl.N == 64 || pl.N == 128 || pl.N == 256) &&
+            (Cout % pl.N == 0) && K >= 1;
     pl.tile_halves = (size_t)(pl.CK / 8) * pl.N * 8;
     pl.blob_halves = (size_t)pl.n_tiles * (Cin / pl.CK) * K * pl.tile_halves;
     return pl;
@@ -496,24 +302,23 @@ void conv1d_tc_pack(const float* w, int Cin, int Cout, int K, const ConvTcPlan& 
 int atoms_lpad(int L) { return kAtomPadL + ceil_div(L + 1, 512) * 512 + kAtomPadR; }
 
 constexpr int kMaxDynTc = 227 * 1024 - 4096;      // opt-in limit minus the kernel's static shared memory
-template <int NACC, int EG>
+template <int N, int MB>
 static void launch_inst(const ConvTcParams& P, dim3 grid, size_t smem, cudaStream_t st) {
     static bool attr[64] = {};
-    if (first_on_device(attr)) CUDA_CHECK(cudaFuncSetAttribute(conv1d_tc_kernel<NACC, EG>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynTc));
-    conv1d_tc_kernel<NACC, EG><<<grid, threads_tc(EG), smem, st>>>(P);
+    if (first_on_device(attr)) CUDA_CHECK(cudaFuncSetAttribute(conv1d_tc_kernel<N, MB>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynTc));
+    conv1d_tc_kernel<N, MB><<<grid, kThreadsTc, smem, st>>>(P);
 }
 
 static void launch_tc_common(ConvTcParams& P, const ConvTcPlan& pl, int rows_to_cover, int batch, const int* item_len,
                              double flops, double bytes, cudaStream_t st) {
     const int tile = 128 * pl.nacc;
-    P.N = pl.N; P.CK = pl.CK;
+    P.CK = pl.CK;
     P.rows = tile + (P.K - 1) * P.dil;
     if (P.lpad < kAtomPadL + ceil_div(rows_to_cover, tile) * tile + (P.K - 1 - P.center) * P.dil || P.center * P.dil > kAtomPadL)
         throw CudaError("conv1d_tc: atom buffer pad too small");
     const size_t a_stage = (size_t)P.rows * 16 * (pl.CK / 8), b_stage = (size_t)pl.N * 16 * (pl.CK / 8);
     const size_t smem = ((SA * a_stage + 127) & ~(size_t)127) + SB * b_stage + 128;
-    constexpr int kMaxDyn = kMaxDynTc;
-    if (smem > (size_t)kMaxDyn) throw CudaError("conv1d_tc: shared memory budget exceeded");
+    if (smem > (size_t)kMaxDynTc) throw CudaError("conv1d_tc: shared memory budget exceeded");
     if (batch > kVocMaxItems) throw CudaError("conv1d_tc: batch exceeds kVocMaxItems");
     P.tile_rows = tile; P.tiles_n = pl.n_tiles; P.batch = batch;
     const int extra = P.up ? 1 : 0;
@@ -525,14 +330,17 @@ static void launch_tc_common(ConvTcParams& P, const ConvTcPlan& pl, int rows_to_
         total_tiles += (Li > 0 ? ceil_div(Li + extra, tile) : 0) * P.tiles_n;
     }
     if (total_tiles == 0) return;
-    static int n_sm = 0;
-    if (n_sm == 0) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev); if (n_sm <= 0) n_sm = 148; }
+    const int n_sm = sm_count();
     const int cap = (g_voc_sm_cap > 0 && g_voc_sm_cap < n_sm) ? g_voc_sm_cap : n_sm;
     dim3 grid(std::min(total_tiles, cap));           // one persistent CTA per SM (of the SMs this launch may take)
     ProfScope ps(KF_CONV1D_TC, st, flops, bytes);
-    const int eg = g_conv_epi_groups >= 2 ? 2 : 1;
-    if (pl.nacc == 2) { if (eg == 2) launch_inst<2, 2>(P, grid, smem, st); else launch_inst<2, 1>(P, grid, smem, st); }
-    else              { if (eg == 2) launch_inst<4, 2>(P, grid, smem, st); else launch_inst<4, 1>(P, grid, smem, st); }
+    switch (pl.N) {
+        case 256: launch_inst<256, 1>(P, grid, smem, st); break;
+        case 128: launch_inst<128, 2>(P, grid, smem, st); break;
+        case 64: launch_inst<64, 4>(P, grid, smem, st); break;
+        case 32: launch_inst<32, 4>(P, grid, smem, st); break;
+        default: throw CudaError("conv1d_tc: tile width must be 32, 64, 128 or 256");
+    }
     COUNT_LAUNCH(); KERNEL_CHECK();
 }
 

@@ -76,7 +76,7 @@ struct Linear {
 
 struct ConvW {
     DBuf<float> wt;               // [Cin][K][Cout]      (CUDA-core path)
-    DBuf<__half> blob;            // tcgen05 tile blob   (fast mode, Conv1d only)
+    DBuf<__half> blob;            // wgmma tile blob     (fast mode, Conv1d only)
     ConvTcPlan plan{};
     bool tc = false;
     DBuf<float> b;                // [Cout]
@@ -183,7 +183,7 @@ private:
     xtts_config cfg;
     int H, L, NH, FF, V, Vpad, B, NSLOT, CAP, MAXP, max_pages, SEENW, S;
     int prefill_rows_cap;
-    bool bf16;                    // 16-bit fast mode (tcgen05 GEMMs, 16-bit KV): bf16 operands, or IEEE fp16 when `f16`
+    bool bf16;                    // 16-bit fast mode (wgmma GEMMs, 16-bit KV): bf16 operands, or IEEE fp16 when `f16`
     bool f16 = false;             // precision fp16: same kernels, fp16 operands (3 more mantissa bits than bf16, range is ample here)
     int gflag = 0;                // GEMM_F16 in fp16 mode
     cudaStream_t st = nullptr;
@@ -391,8 +391,8 @@ Engine::Engine(const xtts_config& c) : cfg(c) {
     CUDA_CHECK(cudaSetDevice(c.device));
     cudaDeviceProp prop{};
     CUDA_CHECK(cudaGetDeviceProperties(&prop, c.device));
-    if (prop.major != 10) {
-        throw std::runtime_error(std::string("libxtts_b200 is built for sm_100a only; found ") + prop.name + " (sm_" +
+    if (prop.major != 9 || prop.minor != 0) {
+        throw std::runtime_error(std::string("libxtts_b200 is built for sm_90a only; found ") + prop.name + " (sm_" +
                                  std::to_string(prop.major) + std::to_string(prop.minor) + ")");
     }
     H = c.hidden; L = c.layers; NH = c.heads; FF = c.ff; V = c.n_audio_tokens;
@@ -1319,7 +1319,7 @@ void Engine::run_vocoder_f32(const VocItem* it, int nb, int Lz, float* wav_dev_o
 }
 
 // Tensor-core vocoder: every Conv1d operand is kept as activated fp16 atoms written by its producer's epilogue
-// (ConvT / previous conv), so the conv kernels are pure bulk-copy + tcgen05; fp32 is kept for the residual stream
+// (ConvT / previous conv), so the conv kernels are pure bulk-copy + wgmma; fp32 is kept for the residual stream
 // (x, r1, r2), the MRF sum and the final waveform.  (speaker biases were gathered into vcb by run_vocoder)
 void Engine::run_vocoder_tc(const VocItem* it, int nb, int Lz, float* wav_dev_out, const char* stage, float* stage_out,
                             int64_t stage_cap) {
@@ -1848,7 +1848,6 @@ void Engine::set_option(const std::string& k, int64_t v) {
     ApiLock lk(this);
     if (k == "d2h_wav") d2h_wav = v != 0;
     else if (k == "tc_vocoder") use_tc_vocoder = v != 0;
-    else if (k == "conv_epi_groups") g_conv_epi_groups = v >= 2 ? 2 : 1;
     else if (k == "attn_ctas_per_sm" || k == "gemm_bn") {
         if (k == "gemm_bn") { if (v != 0 && v != 32 && v != 64 && v != 128) throw std::runtime_error("gemm_bn: 0, 32, 64 or 128"); g_gemm_decode_bn = (int)v; }
         else g_attn_ctas_per_sm = (int)v;                        // < 0: absolute grid size (tests)
@@ -1857,7 +1856,10 @@ void Engine::set_option(const std::string& k, int64_t v) {
     else if (k == "voc_segment") voc_segment = (int)std::max<int64_t>(0, v);
     else if (k == "voc_sms") voc_sms = (int)std::max<int64_t>(0, v);
     else if (k == "voc_batch") voc_max_items = (int)std::max<int64_t>(1, std::min<int64_t>(v, kVocMaxItems));
-    else if (k == "gemm_2cta") g_gemm_2cta = (int)std::max<int64_t>(0, std::min<int64_t>(v, 7));      // 0 off, 1 default, 2-7 ring / epilogue variants
+    else if (k == "gemm_wide") {                                  // 0 off, else the wide kernel's ring depth
+        if (v != 0 && (v < 2 || v > 4)) throw std::runtime_error("gemm_wide: 0 (off) or a ring depth of 2, 3 or 4");
+        g_gemm_wide = (int)v;
+    }
     else if (k == "attn_bulk") { g_attn_bulk = (int)std::max<int64_t>(0, std::min<int64_t>(v, 4)); drop_graphs(); }
     else if (k == "gemm_deep_ring") { g_gemm_deep_ring = v ? 1 : 0; drop_graphs(); }
     else if (k == "gemm_l2_prefetch") { g_gemm_l2_prefetch = v ? 1 : 0; drop_graphs(); }
@@ -2075,18 +2077,24 @@ void Engine::debug_gemm(int mode, const float* A, const float* W, const float* b
     dA.upload(A, (size_t)M * K, st); dW.upload(W, (size_t)N * K, st);
     if (bias) { db.alloc(N); db.upload(bias, N, st); }
     if (resid) { dr.alloc((size_t)M * N); dr.upload(resid, (size_t)M * N, st); }
-    const int flags = (gelu ? GEMM_GELU : 0) | (resid ? GEMM_RESID : 0);
-    DBuf<__nv_bfloat16> hA, hW;
-    if (mode == 1) {
+    if (mode < 0 || mode > 2) throw std::runtime_error("debug_gemm: mode 0 (fp32), 1 (bf16) or 2 (fp16)");
+    const int flags = (gelu ? GEMM_GELU : 0) | (resid ? GEMM_RESID : 0) | (mode == 2 ? GEMM_F16 : 0);
+    DBuf<__nv_bfloat16> hA, hW;                     // 16-bit operands (IEEE fp16 bits in mode 2)
+    if (mode >= 1) {
         std::string err;
         if (!gemm_tc_init(&err)) throw std::runtime_error(err);
         hA.alloc((size_t)M * K); hW.alloc((size_t)N * K);
-        launch_f32_to_bf16(dA.p, hA.p, (size_t)M * K, st); launch_f32_to_bf16(dW.p, hW.p, (size_t)N * K, st);
+        if (mode == 1) {
+            launch_f32_to_bf16(dA.p, hA.p, (size_t)M * K, st); launch_f32_to_bf16(dW.p, hW.p, (size_t)N * K, st);
+        } else {
+            launch_f32_to_f16(dA.p, reinterpret_cast<__half*>(hA.p), (size_t)M * K, st);
+            launch_f32_to_f16(dW.p, reinterpret_cast<__half*>(hW.p), (size_t)N * K, st);
+        }
     }
     cudaEvent_t e0, e1;
     CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
     auto run = [&] {
-        if (mode == 1) launch_gemm_bf16_tc(hA.p, hW.p, db.p, dr.p, dout.p, M, N, K, flags, st);
+        if (mode >= 1) launch_gemm_bf16_tc(hA.p, hW.p, db.p, dr.p, dout.p, M, N, K, flags, st);
         else launch_gemm_f32(dA.p, dW.p, db.p, dr.p, dout.p, M, N, K, flags, st);
     };
     run();
@@ -2156,7 +2164,7 @@ const char* xtts_last_error(void) {
     xtts::t_last_error = xtts::g_last_error;
     return xtts::t_last_error.c_str();
 }
-const char* xtts_version(void) { return "libxtts_b200 0.1 (sm_100a)"; }
+const char* xtts_version(void) { return "libxtts_b200 0.1 (sm_90a)"; }
 
 #define XTTS_TRY_UNBOUND(body)                                          \
     try { body; return XTTS_OK; }                                       \

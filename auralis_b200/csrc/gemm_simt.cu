@@ -1,4 +1,4 @@
-// fp32 CUDA-core GEMM (parity mode and the GPU-side yardstick for the tcgen05 kernel).
+// fp32 CUDA-core GEMM (parity mode and the GPU-side yardstick for the tensor-core kernels).
 //   out[M,N] = epi(A[M,K] . W[N,K]^T + bias)      both operands K-contiguous ("NT")
 // Replaces the cuBLAS calls behind vLLM's QKV/O/MLP linears and the LM head
 // (SURVEY.md §2.4 K4,K6,K7,K9; call sites vllm_mm_gpt.py:759,687).
@@ -133,7 +133,7 @@ void launch_f32_to_f16(const float* in, __half* out, size_t n, cudaStream_t st) 
 void launch_f32_to_bf16(const float* in, __nv_bfloat16* out, size_t n, cudaStream_t st) {
     if (n == 0) return;
     int blocks = (int)((n + 255) / 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > sm_count() * 16) blocks = sm_count() * 16;
     ProfScope ps(KF_MISC, st, 0, 6.0 * n);
     f32_to_bf16_kernel<<<blocks, 256, 0, st>>>(in, out, n);
     COUNT_LAUNCH();

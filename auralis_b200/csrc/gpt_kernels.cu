@@ -111,7 +111,7 @@ layernorm_kernel(const float* __restrict__ X, const float* __restrict__ w, const
                  TOut* __restrict__ Y, int H, float eps, const DepFlag dep) {
     __shared__ float red[32];
     trace_pt(TR_LN, 0); pdl_trigger();
-    if (threadIdx.x == 0) dep_wait(dep, 31);
+    if (threadIdx.x == 0) dep_wait(dep);
     __syncthreads();
     trace_pt(TR_LN, 1);
     const float* x = X + (size_t)blockIdx.x * H;
@@ -148,7 +148,7 @@ residual_reduce_ln_kernel(float* __restrict__ X, const float* __restrict__ P, in
     extern __shared__ float buf[];
     __shared__ float red[32];
     trace_pt(TR_REDUCE_LN, 0); pdl_trigger();
-    if (threadIdx.x == 0) dep_wait(dep, 32);
+    if (threadIdx.x == 0) dep_wait(dep);
     __syncthreads();
     trace_pt(TR_REDUCE_LN, 1);
     float* x = X + (size_t)blockIdx.x * H;
@@ -291,7 +291,7 @@ attn_decode_kernel(const float* __restrict__ QKV, const int* __restrict__ active
     trace_pt(TR_ATTN, 0); pdl_trigger();
     // ncu: 24 resident warps per SM, long-scoreboard stalls dominate: the kernel is bound by the bytes its warps keep in
     // flight against ~1.6 us of HBM latency under load.  Option "attn_l2_pages": cp.async.bulk.prefetch.L2 holds no registers.
-    if (threadIdx.x == 0) dep_wait(dep, 33);
+    if (threadIdx.x == 0) dep_wait(dep);
     __syncthreads();
     trace_pt(TR_ATTN, 1);
     const int H = heads * kHeadDim;
@@ -1198,18 +1198,14 @@ int launch_attn_decode(const float* QKV, const int* active, int M, const int* ct
     const int n_items = M * heads;
     int grid = n_items;
     if (g_attn_ctas_per_sm > 0) {
-        static int n_sm = 0;
-        if (n_sm == 0) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev); if (n_sm <= 0) n_sm = 148; }
-        grid = std::min(n_items, n_sm * g_attn_ctas_per_sm);
+        grid = std::min(n_items, sm_count() * g_attn_ctas_per_sm);
     } else if (g_attn_ctas_per_sm < 0) {
         grid = std::min(n_items, -g_attn_ctas_per_sm);          // test hook: an absolute grid size
     }
     if constexpr (sizeof(TKV) == 2) {
         if (g_attn_bulk > 0 && dep.wait == nullptr && dep.arrive == nullptr) {
             // bulk-copy form: `attn_bulk` persistent CTAs per SM, each with an `attn_stages`-deep ring of 8 KB pages
-            static int n_sm = 0;
-            if (n_sm == 0) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev); if (n_sm <= 0) n_sm = 148; }
-            int g = std::min(n_items, n_sm * g_attn_bulk);
+            int g = std::min(n_items, sm_count() * g_attn_bulk);
             if (g_attn_ctas_per_sm < 0) g = std::min(n_items, -g_attn_ctas_per_sm);          // test hook: an absolute grid size
             g = std::max(g, ceil_div(n_items, kBulkMaxItems));
             // consumer warps per CTA = option "attn_warps" (4 / 8 / 16; same page -> warp assignment and combination order as

@@ -1,6 +1,7 @@
-// Host-side launchers of every sm_100a kernel in the library (one declaration per kernel family).
+// Host-side launchers of every sm_90a kernel in the library (one declaration per kernel family).
 // Each launcher enqueues on `st` and returns; errors surface as xtts::CudaError.
 #pragma once
+#include <cuda.h>
 #include "common.cuh"
 
 namespace xtts {
@@ -13,26 +14,26 @@ namespace xtts {
 // GEMM_OUT_BF16: 16-bit output in the operand format;  GEMM_F16: the 16-bit operands (and that output) are IEEE fp16, not bf16
 enum : int { GEMM_GELU = 1, GEMM_RESID = 2, GEMM_OUT_BF16 = 4, GEMM_F16 = 8, GEMM_NO_L2PF = 16 /* internal: engine option gemm_l2_prefetch = 0 */ };
 
-// fp32 CUDA-core path (parity mode; also the GPU-side reference for the tcgen05 path)
+// fp32 CUDA-core path (parity mode; also the GPU-side reference for the tensor-core path)
 void launch_gemm_f32(const float* A, const float* W, const float* bias, const float* resid, float* out,
                      int M, int N, int K, int flags, cudaStream_t st);
 
-// bf16 tcgen05/TMA path (fast mode).  A [M,K] bf16 row-major, W [N,K] bf16 row-major; fp32 accum in TMEM.
-// out is fp32 unless GEMM_OUT_BF16.  K % 64 == 0, N % 16 == 0 required.
+// bf16 wgmma/TMA path (fast mode).  A [M,K] bf16 row-major, W [N,K] bf16 row-major; fp32 accumulators in registers.
+// out is fp32 unless GEMM_OUT_BF16.  K % 64 == 0, N % 32 == 0 required.
 // `pdl`: launch with the programmatic-dependent-launch attribute (decode chain); every kernel that can be launched
 // that way executes griddepcontrol.wait before touching its predecessor's outputs
 // `dep` (decode chain): wait / arrive counters instead of griddepcontrol.wait (common.cuh).  Returns the number of CTAs
-// launched = the value the kernel's arrive counter reaches (0 when the launch went to the CTA-pair kernel).
+// launched = the value the kernel's arrive counter reaches (0 when the launch went to the wide-tile kernel).
 int launch_gemm_bf16_tc(const __nv_bfloat16* A, const __nv_bfloat16* W, const float* bias, const float* resid,
                         void* out, int M, int N, int K, int flags, cudaStream_t st, bool pdl = false, DepFlag dep = DepFlag());
-// large-shape path (gemm_tcgen05_2cta.cu): persistent CTA pairs (cta_group::2), 256 x 256 tiles, double-buffered TMEM
-bool gemm_2cta_supported(int M, int N, int K);
-void launch_gemm_bf16_2cta(const __nv_bfloat16* A, const __nv_bfloat16* W, const float* bias, const float* resid,
+// large-shape path (gemm_wgmma_wide.cu): persistent CTAs, 128 x 256 tiles
+bool gemm_wide_supported(int M, int N, int K);
+void launch_gemm_bf16_wide(const __nv_bfloat16* A, const __nv_bfloat16* W, const float* bias, const float* resid,
                            void* out, int M, int N, int K, int flags, cudaStream_t st);
 int launch_gemm_bf16_tc_splitk(const __nv_bfloat16* A, const __nv_bfloat16* W, float* partials, int M, int N, int K,
                                int splits, cudaStream_t st, bool pdl = false, DepFlag dep = DepFlag(), int flags = 0);
 
-// Fused decode chain (gemm_tcgen05.cu): one persistent launch runs, for one layer boundary of the decode step,
+// Fused decode chain (gemm_wgmma.cu): one persistent launch runs, for one layer boundary of the decode step,
 //   proj (split-K) -> residual+LN2 -> fc+gelu -> fc2 (split-K) -> residual+LN1(next layer) -> qkv(next layer)
 // with device-wide barriers between the phases.  `phases` selects a contiguous subset (DC_* bits).
 enum { DC_PROJ = 1, DC_LN2 = 2, DC_FC = 4, DC_FC2 = 8, DC_LN1 = 16, DC_QKV = 32 };
@@ -48,6 +49,9 @@ struct DecodeChainArgs {
 bool decode_chain_supported(int M, int H, int FF);
 void launch_decode_chain(const DecodeChainArgs& a, cudaStream_t st, bool pdl);
 bool gemm_tc_init(std::string* err);   // resolves cuTensorMapEncodeTiled; false -> err filled
+// TMA descriptor of a row-major 16-bit matrix [rows, cols]: boxes of 64 columns (128 B, SWIZZLE_128B) x box_rows rows, the
+// operand image the wgmma kernels read (gemm_wgmma.cu, gemm_wgmma_wide.cu); rows past the end are zero-filled
+void tma_encode_bf16_2d(CUtensorMap* tm, const void* ptr, uint64_t rows, uint64_t cols, uint32_t box_rows);
 
 void trace_set_gemm(TraceBuf b);     // per-translation-unit setters of the debug timeline buffer (common.cuh)
 void trace_set_gpt(TraceBuf b);
@@ -162,7 +166,7 @@ void launch_conv1d(const float* x, const float* w_t, const float* bias, const fl
                    float* out, int Cin, int Cout, int L, int K, int dil, float in_scale, float slope, int mode,
                    int batch, int cbias_batch_stride, cudaStream_t st);
 // ---- tensor-core vocoder path (fast mode).  Activations that feed a Conv1d live in HBM as fp16 "atoms":
-//   [C/8 plane][kAtomPadL + L + tail][8 channels], zero pads — the UMMA no-swizzle K-major operand image.
+//   [C/8 plane][kAtomPadL + L + tail][8 channels], zero pads — the wgmma no-swizzle K-major operand image.
 constexpr int kAtomPadL = 64, kAtomPadR = 64;
 int atoms_lpad(int L);                                   // padded rows per plane for a signal of L steps
 struct ConvTcPlan { int N, CK, n_tiles, nacc; bool ok; size_t tile_halves, blob_halves; };
@@ -170,7 +174,7 @@ ConvTcPlan conv1d_tc_plan(int Cin, int Cout, int K);
 void conv1d_tc_pack(const float* w /*[Cout][Cin][K]*/, int Cin, int Cout, int K, const ConvTcPlan& pl, __half* blob);
 // y = bias + cbias + resid + conv(a16);  out32 (fp32 [C][L], store/accumulate) and/or out16 (lrelu(y, slope_out) atoms)
 // out16 = lrelu(y * scale16, slope_out)
-// (engine knobs of the launchers — attention grid cap, decode GEMM tile, conv epilogue groups, vocoder SM cap — live in
+// (engine knobs of the launchers — attention grid cap, decode GEMM tile, vocoder SM cap — live in
 //  the calling engine's KernelCtx, common.cuh)
 void launch_conv1d_tc(const __half* a16, const __half* wblob, const ConvTcPlan& pl, const float* bias, const float* cbias,
                       const float* resid, float* out32, __half* out16, int Cin, int Cout, int L, int lpad, int K, int dil,

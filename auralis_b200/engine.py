@@ -1,5 +1,5 @@
 """XTTSv2Engine — the reference's engine plugin (`/root/reference/src/auralis/models/xttsv2/XTTSv2.py`)
-re-hosted on the native B200 library.  Same public methods, argument meaning and error behaviour:
+re-hosted on the native CUDA library.  Same public methods, argument meaning and error behaviour:
 
 * ``from_pretrained(path, gpt_model=..., max_concurrency=...)``            XTTSv2.py:235-310
 * ``await get_audio_conditioning(speaker_files, ...) -> (cond, g)``         XTTSv2.py:579-615
@@ -95,7 +95,7 @@ class XTTSv2Engine(BaseAsyncTTSEngine):
                  tokenizer_file: Optional[str] = None, early_emit_tokens: int = 0, voc_segment: Optional[int] = None,
                  tune_malloc: bool = False, **_):
         """`devices=[0, 1, ...]`: data parallelism inside the product (north_star: "requests shard data-parallel across the
-        8xB200 box") — one native engine (full weight replica, own scheduler thread, own streams) per listed GPU in THIS
+        8-GPU box") — one native engine (full weight replica, own scheduler thread, own streams) per listed GPU in THIS
         process; every text chunk goes to the engine with the least work in flight, results are re-assembled in request
         order by the façade as before.  `max_concurrency` is per GPU.  Default: the single GPU `device`."""
         prec = {"fp32": native.PRECISION_FP32, "bf16": native.PRECISION_BF16, "fp16": native.PRECISION_FP16}[precision]

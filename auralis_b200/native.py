@@ -1,7 +1,7 @@
 """ctypes binding of ``libxtts_b200.so`` (C ABI: ``include/xtts_b200.h``).
 
 No torch types cross this boundary: numpy arrays in host memory in, numpy arrays out.
-The library is CUDA-only; creating an engine without an sm_100 GPU raises ``NativeError``
+The library is CUDA-only; creating an engine without an sm_90 GPU raises ``NativeError``
 (there is no CPU fallback — parity claims depend on that).
 """
 from __future__ import annotations
@@ -324,8 +324,11 @@ class NativeEngine:
                                                                     launches=int(p.launches[i]))
         return out
 
-    def run_batch(self, jobs, timeout_s: float = 600.0, want_wav: bool = True, want_latents: bool = False):
-        """jobs: iterable of (seq_id, text_ids, speaker_slot, Sampling).  Returns {seq_id: (result, tokens, wav, lat)}."""
+    def run_batch(self, jobs, timeout_s: float = 600.0, want_wav: bool = True, want_latents: bool = False,
+                  defer_fetch: bool = False):
+        """jobs: iterable of (seq_id, text_ids, speaker_slot, Sampling).  Returns {seq_id: (result, tokens, wav, lat)}.
+        defer_fetch: final results stay in the engine (tokens, wav, lat are None) until the caller passes each result to
+        fetch() — e.g. to copy the waveforms out of HBM after a timed region."""
         import time
         n = 0
         # batch submit: the scheduler admits nothing until the whole batch is queued, so admission waves (and with
@@ -352,8 +355,7 @@ class NativeEngine:
                 ptoks, pwav, _ = self.fetch(r, want_wav, False)
                 partials.setdefault(r.seq_id, []).append((r, ptoks, pwav))
                 continue
-            toks, wav, lat = self.fetch(r, want_wav, want_latents)
-            out[r.seq_id] = (r, toks, wav, lat)
+            out[r.seq_id] = (r, None, None, None) if defer_fetch else (r, *self.fetch(r, want_wav, want_latents))
         self.last_partials = partials        # {seq_id: [(result, tokens, wav), ...]} of the batch just run, oldest first
         return out
 

@@ -1,4 +1,4 @@
-"""INTEGRATION.md path B as code: the native B200 engine registered as a plugin of the REFERENCE's own façade.
+"""INTEGRATION.md path B as code: the native engine registered as a plugin of the REFERENCE's own façade.
 
 A maintainer who keeps `auralis.TTS`, its `TwoPhaseScheduler` and its HTTP server installs this package next to the
 reference and adds one line where the reference registers its models (`src/auralis/models/__init__.py`):

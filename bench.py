@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — the hot path's headline metric on N B200s of one node.
+"""bench.py — the hot path's headline metric on N H100s of one node.
 
     python bench.py --gpus N --steps K --warmup W            (N>1: launched by torchrun, one rank per GPU)
     python bench.py --impl reference ...                      (CPU arm: the oracle port on the host cores)
@@ -16,7 +16,9 @@ continuous batching -> latents -> vocoder -> waveforms.
                timed region, waveforms left in HBM).
   * `e2e`    : the same metric through the public API (`TTS.generate_speech_batch(TTSRequest...)`): host text in,
                host float32 waveforms out, tokenisation, H2D and D2H inside the timed region.
-Prints ONE JSON line on rank 0.
+Prints ONE JSON line on rank 0.  `--dump-outputs DIR` (rank 0) also writes what the last timed step of the device-resident
+arm returned to its caller — token ids and waveforms of every chunk, the waveforms as a fixed seeded sample — as DIR/*.npy;
+those results are fetched from the engine after the timed region, so no waveform copy is timed.
 """
 from __future__ import annotations
 
@@ -80,7 +82,7 @@ def synthetic_wav_bytes(seconds: float, f0: float, seed: int, sr: int = 22050) -
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -158,6 +160,33 @@ def cpu_reference_sample(dims, state, n_threads: int, chunks=None, n_chunks: int
             "vocoder_audio_s_per_s": audio_s / max(1e-9, t_all - t_gpt)}
 
 
+def dump_outputs(out_dir: str, res: dict, max_tok: int, n_pick: int = 4096, seed: int = 20240607) -> None:
+    """Writes one step's per-chunk results ({seq_id: (result, tokens, wav, latents)}) as .npy files (< 64 MB in all):
+      tokens.npy      float64 [n_chunks, max_tok]  token ids, -1 past a chunk's end
+      n_samples.npy   float64 [n_chunks]           waveform length of every chunk
+      wav_sample.npy  float32 [n_chunks, n_pick]   every chunk's waveform at n_pick positions drawn by a fixed seed
+                                                   (position = floor(u * n_samples) for the same u in every run)
+      wav_first.npy   float32 [n]                  the whole waveform of chunk 0"""
+    os.makedirs(out_dir, exist_ok=True)
+    ids = sorted(res)
+    toks = np.full((len(ids), max_tok), -1.0, np.float64)
+    n_samp = np.zeros(len(ids), np.float64)
+    u = np.random.RandomState(seed).random_sample(n_pick)
+    wav_s = np.zeros((len(ids), n_pick), np.float32)
+    for i, sid in enumerate(ids):
+        r, t, w, _ = res[sid]
+        toks[i, :min(len(t), max_tok)] = np.asarray(t[:max_tok], np.float64)
+        n = 0 if w is None else int(w.shape[0])
+        n_samp[i] = n
+        if n:
+            wav_s[i] = w[np.minimum((u * n).astype(np.int64), n - 1)]
+    np.save(os.path.join(out_dir, "tokens.npy"), toks)
+    np.save(os.path.join(out_dir, "n_samples.npy"), n_samp)
+    np.save(os.path.join(out_dir, "wav_sample.npy"), wav_s)
+    first = res[ids[0]][2] if ids else None
+    np.save(os.path.join(out_dir, "wav_first.npy"), np.zeros(0, np.float32) if first is None else np.asarray(first, np.float32))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -176,6 +205,8 @@ def main():
     ap.add_argument("--no-extras", action="store_true", help="skip the extra arms (ragged lengths, cfg3 time-to-first-audio, fp32 parity mode, strong scaling)")
     ap.add_argument("--sweep", action="store_true", help="option sweeps only: skip the e2e arm and the CPU baseline (the line says so; not a headline run)")
     ap.add_argument("--small", action="store_true", help="tiny geometry (plumbing check only; not a valid bench number)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step (token ids, seeded waveform sample) to DIR/<name>.npy")
     args = ap.parse_args()
 
     import torch
@@ -224,9 +255,9 @@ def main():
         print(json.dumps(line))
         return
 
-    # ------------------------------------------------------------------------------- B200 arm
+    # ------------------------------------------------------------------------------- GPU arm
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device — the B200 arm has no CPU fallback (use --impl reference)")
+        raise SystemExit("bench.py: no CUDA device — the GPU arm has no CPU fallback (use --impl reference)")
     from auralis_b200 import TTS, TTSRequest, native
     from auralis_b200.engine import XTTSv2Engine, tune_host_allocator
     malloc_tuned = tune_host_allocator()      # output buffers stay on the heap (no page-fault storm per step), see engine.py
@@ -249,8 +280,11 @@ def main():
     n_chunks = sum(len(c) for c in reqs_chunks)
     max_tok = min(args.max_tokens, dims.gpt.max_audio_tokens)
 
-    def device_step(step_idx: int, lengths=None, chunk_lists=None):
-        """lengths: per-chunk max_tokens (the ragged arm); chunk_lists: another request set (the strong-scaling arm)"""
+    last_outputs = {}
+
+    def device_step(step_idx: int, lengths=None, chunk_lists=None, keep=False):
+        """lengths: per-chunk max_tokens (the ragged arm); chunk_lists: another request set (the strong-scaling arm);
+        keep: leave this step's results in the engine and their handles in `last_outputs` (--dump-outputs fetches them later)"""
         jobs, sid = [], 0
         for ri, chunks in enumerate(chunk_lists if chunk_lists is not None else reqs_chunks):
             for ci, ids in enumerate(chunks):
@@ -259,7 +293,10 @@ def main():
                                      stop_token=dims.gpt.stop_audio_token, seed=SEED + step_idx, seq_seed=sid, vocode=True)
                 jobs.append((sid, ids, spk_slots[ri % 4], sp))
                 sid += 1
-        res = eng.run_batch_direct(jobs, timeout_s=900, want_wav=False)
+        res = eng.run_batch_direct(jobs, timeout_s=900, want_wav=False, defer_fetch=keep)
+        if keep:
+            last_outputs.clear()
+            last_outputs.update(res)
         return sum(r.n_samples for (r, _, _, _) in res.values()), sum(r.n_tokens for (r, _, _, _) in res.values())
 
     def e2e_step(step_idx: int):
@@ -336,7 +373,11 @@ def main():
     ne.set_option("reset_stats", 0)
     if sampler:
         sampler.start()
-    dt_dev, wall_dev, acc_dev, span = timed(device_step, 0, args.steps)
+    dump = args.dump_outputs is not None and rank == 0
+    dt_dev, wall_dev, acc_dev, span = timed(lambda i: device_step(i, keep=dump and i == args.steps - 1), 0, args.steps)
+    if dump:          # the last timed step's results, copied out of the engine now that the clock has stopped
+        dump_outputs(args.dump_outputs, {sid: (r, *ne.fetch(r, want_wav=True)) for sid, (r, _, _, _) in last_outputs.items()},
+                     max_tok)
     clocks = sampler.stop(*span) if sampler else None
     st = ne.stats()
     samples_dev = sum(a[0] for a in acc_dev)
@@ -466,9 +507,9 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    tc_peak = float(peaks.get("bf16_tflops_sustained", 1400.0))
-    peak_src = "measured (MEASURED_PEAKS.json)" if peaks else "fallback (B200_PROFILING.md)"
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+    tc_peak = float(peaks.get("bf16_tflops_sustained", 989.0))
+    peak_src = "measured (MEASURED_PEAKS.json)" if peaks else "H100 SXM data sheet (3.35 TB/s HBM3, 989 TFLOP/s dense bf16; not measured)"
     total_ms = sum(v["ms"] for v in prof.values()) or 1.0
     dom_name, dom = max(prof.items(), key=lambda kv: kv[1]["ms"]) if prof else ("none", {"ms": 1, "flops": 0, "bytes": 0, "launches": 1})
     fams = {}
@@ -493,16 +534,6 @@ def main():
                  "fp32_tflops": dom["flops"] / (dom["ms"] * 1e-3) / 1e12 if dom["ms"] else None,
                  "families": fams})
 
-    # DRAM traffic of the dominant family, per launch, from the committed ncu capture (profiles/ncu_traffic.json)
-    try:
-        tr = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json"))).get(dom_name)
-    except Exception:
-        tr = None
-    if tr:
-        roof["traffic"] = tr["dram_bytes_per_launch"]
-        roof["traffic_detail"] = {"unit": "bytes per launch", "algorithmic_bytes_per_launch_at_capture": tr["algorithmic_bytes_per_launch_at_capture"],
-                                  "algorithmic_bytes_per_launch_this_run": dom["bytes"] / max(1, dom["launches"]),
-                                  "shape": tr["shape"], "note": tr["note"], "source": tr["source"]}
 
     cpu = None
     if args.gpus == 1 and not args.sweep:
@@ -517,10 +548,10 @@ def main():
         "config": {"workload": workload, "chunks_per_gpu": n_chunks, "tokens_per_chunk": max_tok,
                    "audio_s_per_step": audio_s_dev / args.steps, "geometry": "small (INVALID as a bench number)" if args.small else "XTTSv2 full: GPT-2 30x1024x16h, HiFi-GAN 512ch, random-init",
                    "parallelism": f"dp{args.gpus} (requests sharded, waveform all-gather only)",
-                   "gpt_compute": (f"{args.precision} tcgen05 GEMM operands + {args.precision} KV, fp32 accumulate/residual/LN/softmax"
+                   "gpt_compute": (f"{args.precision} wgmma GEMM operands + {args.precision} KV, fp32 accumulate/residual/LN/softmax"
                                    if args.precision != "fp32" else "fp32"),
-                   "vocoder_compute": "fp16 tcgen05 implicit-GEMM convs (fp32 accumulate, fp32 residual stream)" if args.precision != "fp32" else "fp32",
-                   "l2": "no explicit flush: per-step working set (0.76 GB weights + >5 GB KV + 0.4 GB vocoder activations) >> 126 MB L2",
+                   "vocoder_compute": "fp16 wgmma implicit-GEMM convs (fp32 accumulate, fp32 residual stream)" if args.precision != "fp32" else "fp32",
+                   "l2": "no explicit flush: per-step working set (0.76 GB weights + >5 GB KV + 0.4 GB vocoder activations) >> 50 MB L2",
                    "timing": "CUDA events on the engine stream (first recorded with the device idle after barrier + synchronize, second "
                              "behind the last step's work); max over ranks; e2e: host wall clock around the public API calls",
                    "host_wall_ms_per_step": 1e3 * wall_dev / args.steps,

@@ -1,4 +1,4 @@
-/* libxtts_b200 — C ABI of the B200-native XTTSv2 hot path.
+/* libxtts_b200 — C ABI of the H100-native (sm_90a) XTTSv2 hot path.
  *
  * The reference (astramind-ai/Auralis) has no FFI of its own: its hot path sits behind two Python
  * surfaces, the `BaseAsyncTTSEngine` plugin API (src/auralis/models/base.py:57-224) and the vLLM
@@ -28,7 +28,7 @@ extern "C" {
 #define XTTS_ERR_CANCELLED -5 /* the chunk was cancelled with xtts_cancel before it finished */
 
 #define XTTS_PRECISION_FP32 0 /* parity mode: fp32 CUDA-core GEMMs, fp32 KV cache            */
-#define XTTS_PRECISION_BF16 1 /* fast mode: bf16 tcgen05 GEMMs (fp32 accumulate), bf16 KV    */
+#define XTTS_PRECISION_BF16 1 /* fast mode: bf16 wgmma GEMMs (fp32 accumulate), bf16 KV      */
 #define XTTS_PRECISION_FP16 2 /* fast mode with IEEE fp16 operands and KV: the same kernels at the same rate, 11 significand
                                  bits instead of 8 — closer to the fp32 parity mode (the reference's GPU vocoder is fp16 too) */
 
@@ -107,7 +107,7 @@ const char* xtts_last_error(void);
 const char* xtts_version(void);
 
 /* XTTSv2Engine.__init__/from_pretrained (XTTSv2.py:53-150,235-310): allocates weights, KV pages,
- * workspaces on `cfg->device`.  Fails loudly (XTTS_ERR_CUDA) if there is no sm_100 GPU. */
+ * workspaces on `cfg->device`.  Fails loudly (XTTS_ERR_CUDA) if there is no sm_90 GPU. */
 int xtts_create(const xtts_config* cfg, xtts_engine** out);
 int xtts_destroy(xtts_engine* e);
 
@@ -144,13 +144,12 @@ int xtts_fetch(xtts_engine* e, uint64_t seq_id, int32_t* tokens, float* wav, flo
  *   "d2h_wav"             0 = leave waveforms in HBM (kernel-only timing), 1 = D2H into pinned memory (default)
  *   "cuda_graphs" / "pdl" / "splitk" / "tc_vocoder"   0/1, fast-mode execution features (all default 1)
  *   "hold_admission"      1 = queue submissions without admitting them, 0 = release (atomic batch submit)
- *   "conv_epi_groups"     1 or 2 epilogue warpgroups in the tensor-core conv kernel (default 2)
  *   "decode_chain"        1 = fused persistent per-layer GEMM/LayerNorm chain kernel in the decode step, 0 = one launch per
  *                         GEMM / LayerNorm with "microbatches" concurrent row branches (default: measured faster)
  *   "microbatches"        1..4 concurrent branches the decode step's rows are split into (default 2)
  *   "microbatch_min_rows" steps with fewer active rows stay single-branch (default 48)
- *   "gemm_2cta"           1 (default) = GEMMs with M >= 256 rows (prefill, conditioning) run on the persistent CTA-pair kernel
- *                         (cta_group::2, 256x256 tiles, double-buffered TMEM), 0 = the one-tile-per-CTA kernel
+ *   "gemm_wide"           4 (default), 3 or 2 = GEMMs with M >= 256 rows (prefill, conditioning) run on the persistent
+ *                         wide-tile kernel (128x256 tiles) with that ring depth, 0 = the one-tile-per-CTA kernel
  *   "voc_segment"         m > 0: a chunk is vocoded in windows of m tokens WHILE it decodes (the vocoder runs on its own
  *                         stream beside the decode step), 0 = one window per chunk when it ends.  Same samples either way.
  *   "voc_sms"             SMs the vocoder's persistent conv kernels may occupy while a decode step is in flight (0 = all)
@@ -194,7 +193,7 @@ int xtts_gpt_prefill(xtts_engine* e, const int32_t* text_ids, int32_t n_text, in
 int xtts_gpt_teacher_forced(xtts_engine* e, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
                             const int32_t* forced_tokens, int32_t n, const xtts_sampling* sp, float* logits_out,
                             float* latents_out, int32_t* sampled_out);
-/* GEMM under test: mode 0 = fp32 CUDA-core, 1 = bf16 tcgen05.  A [M,K], W [N,K], bias [N] or NULL, resid [M,N] or NULL */
+/* GEMM under test: mode 0 = fp32 CUDA-core, 1 = bf16 wgmma, 2 = fp16 wgmma.  A [M,K], W [N,K], bias [N] or NULL, resid [M,N] or NULL */
 int xtts_debug_gemm(xtts_engine* e, int32_t mode, const float* A, const float* W, const float* bias, const float* resid,
                     float* out, int32_t M, int32_t N, int32_t K, int32_t gelu, int32_t iters, float* ms_per_iter);
 /* debug timeline: op 1 arms %globaltimer stamps in the decode / vocoder kernels (first and last CTA: entry, dependency

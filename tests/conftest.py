@@ -21,7 +21,7 @@ torch.set_num_threads(max(1, min(16, os.cpu_count() or 1)))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a)")
     config.addinivalue_line("markers", "slow: long-running")
 
 
@@ -30,11 +30,11 @@ def has_gpu() -> bool:
 
 
 def pytest_collection_modifyitems(config, items):
-    """A box with the library built but no B200: GPU tests are skipped, not errored (the library has no CPU fallback)."""
-    ok = has_gpu() and torch.cuda.get_device_capability(0)[0] == 10
+    """A machine with the library built but no H100: GPU tests are skipped, not errored (the library has no CPU fallback)."""
+    ok = has_gpu() and torch.cuda.get_device_capability(0) == (9, 0)
     if ok:
         return
-    skip = pytest.mark.skip(reason="needs an sm_100 GPU (libxtts_b200 has no CPU fallback)")
+    skip = pytest.mark.skip(reason="needs an sm_90 GPU (libxtts_b200 has no CPU fallback)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

@@ -171,7 +171,7 @@ def test_sampler_full_vocab(engine_full, dims_full, top_k):
 
 
 # ------------------------------------------------------------------------------------------------
-# bf16 / tcgen05 fast mode: same graph, looser tolerance (bf16 operands, fp32 accumulate)
+# bf16 / wgmma fast mode: same graph, looser tolerance (bf16 operands, fp32 accumulate)
 # ------------------------------------------------------------------------------------------------
 def test_bf16_prefill_small(engine_small_bf16, dims_small, state_small, speakers_small):
     orc = _orc(dims_small, state_small)
@@ -377,7 +377,7 @@ def test_kernel_profile_graph_events(engine_small_bf16, dims_small):
     L = g.layers
     att = prof["attn_decode_paged"]
     assert att["launches"] >= 9 * L and att["ms"] > 0 and att["bytes"] > 0, att
-    assert prof["sample"]["launches"] >= 10 and prof["gemm_bf16_tcgen05"]["ms"] > 0
+    assert prof["sample"]["launches"] >= 10 and prof["gemm_bf16_wgmma"]["ms"] > 0
 
 
 def test_device_timer_brackets_a_batch(engine_small, dims_small):
@@ -397,7 +397,7 @@ def test_device_timer_brackets_a_batch(engine_small, dims_small):
 
 
 # ------------------------------------------------------------------------------------------------
-# precision "fp16": the tcgen05 fast path with IEEE fp16 operands / KV instead of bf16 (VERDICT r1 weak 1: a tensor-core mode
+# precision "fp16": the wgmma fast path with IEEE fp16 operands / KV instead of bf16 (VERDICT r1 weak 1: a tensor-core mode
 # closer to the parity mode — kind::f16 takes fp16 at the same rate, 11 significand bits instead of 8)
 # ------------------------------------------------------------------------------------------------
 def test_fp16_operand_mode_small(engine_small_fp16, dims_small, state_small, speakers_small):

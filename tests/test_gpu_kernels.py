@@ -1,4 +1,4 @@
-"""GPU: single-kernel parity through the C ABI — GEMMs (fp32 CUDA-core and bf16 tcgen05) and the fused sampler."""
+"""GPU: single-kernel parity through the C ABI — GEMMs (fp32 CUDA-core and bf16 wgmma) and the fused sampler."""
 import numpy as np
 import pytest
 import torch
@@ -43,9 +43,9 @@ def _bf16(x):
                                    (33, 1056, 1024), (257, 4096, 1024), (256, 256, 64), (1000, 3072, 1024), (513, 288, 192),
                                    (2304, 1056, 1024)])
 def test_gemm_bf16_tcgen05(engine_small, M, N, K):
-    """tcgen05 path vs an fp64 product of the bf16-rounded operands (isolates layout/descriptor bugs from rounding).
-    M >= 256 and N >= 256 shapes run on the persistent CTA-pair kernel (cta_group::2): full and ragged 256 x 256 tiles, more
-    tiles than clusters (the double-buffered accumulators and the stage ring wrap), N tails that are not a multiple of 256."""
+    """Tensor-core path vs an fp64 product of the bf16-rounded operands (isolates layout/descriptor bugs from rounding).
+    M >= 256 and N >= 256 shapes run on the persistent wide-tile kernel: full and ragged 128 x 256 tiles, more tiles than
+    CTAs (the stage ring wraps across tiles), N tails that are not a multiple of 256."""
     rng = np.random.RandomState(M * 13 + N)
     A = rng.randn(M, K).astype(np.float32)
     W = (rng.randn(N, K) * 0.05).astype(np.float32)
@@ -60,12 +60,17 @@ def test_gemm_bf16_tcgen05(engine_small, M, N, K):
                                                           np.unravel_index(np.abs(out - ref).argmax(), out.shape))
 
 
-@pytest.mark.parametrize("variant", [2, 3, 4, 5, 6, 7])
-def test_gemm_2cta_ring_and_epilogue_variants(engine_small, variant):
-    """Engine option "gemm_2cta" = 2..7: ring shapes (stages x k-blocks per stage) and 8 / 16 epilogue warps of the CTA-pair kernel.
-    Every variant, on ragged tiles with more tiles than clusters and on a 16-bit-output... (fp32 here) path, must give the
-    default's result bit for bit (same MMA order per output element)."""
-    outs = {}
+def _f16(x):
+    return x.astype(np.float16).astype(np.float32)
+
+
+@pytest.mark.parametrize("mode", [1, 2], ids=["bf16", "fp16"])
+@pytest.mark.parametrize("depth", [2, 3, 4])
+def test_gemm_wide_ring_depths(engine_small, depth, mode):
+    """Engine option "gemm_wide" = ring depth (2, 3 or 4 stages) of the persistent wide-tile kernel, with bf16 and IEEE fp16
+    operands (the two wgmma instruction types).  Every depth, on ragged tiles with more tiles than CTAs, must give the default
+    depth's result bit for bit (same MMA order per output element)."""
+    rnd = _bf16 if mode == 1 else _f16
     for (M, N, K) in ((1000, 3072, 1024), (513, 288, 192), (2304, 1056, 1024)):
         rng = np.random.RandomState(M + N)
         A = rng.randn(M, K).astype(np.float32)
@@ -73,14 +78,14 @@ def test_gemm_2cta_ring_and_epilogue_variants(engine_small, variant):
         b = rng.randn(N).astype(np.float32)
         r = rng.randn(M, N).astype(np.float32)
         try:
-            engine_small.set_option("gemm_2cta", variant)
-            got, _ = engine_small.debug_gemm(1, A, W, b, r, True)
+            engine_small.set_option("gemm_wide", depth)
+            got, _ = engine_small.debug_gemm(mode, A, W, b, r, True)
         finally:
-            engine_small.set_option("gemm_2cta", 1)
-        ref = _ref_gemm(_bf16(A), _bf16(W), b, r, True)
+            engine_small.set_option("gemm_wide", 4)
+        ref = _ref_gemm(rnd(A), rnd(W), b, r, True)
         assert np.isfinite(got).all()
-        assert np.abs(got - ref).max() < 2e-3 * max(1.0, np.abs(ref).max()), (variant, M, N, K)
-        base, _ = engine_small.debug_gemm(1, A, W, b, r, True)
+        assert np.abs(got - ref).max() < 2e-3 * max(1.0, np.abs(ref).max()), (depth, mode, M, N, K)
+        base, _ = engine_small.debug_gemm(mode, A, W, b, r, True)
         np.testing.assert_array_equal(got, base)
 
 
@@ -94,9 +99,9 @@ def test_gemm_tcgen05_speed_report(engine_small):
             _, ms = engine_small.debug_gemm(mode, A, W, None, None, False, iters=20)
             print(f"gemm mode={mode} M={M} N={N} K={K}: {ms * 1e3:.1f} us  {2.0 * M * N * K / ms / 1e9:.2f} TFLOP/s")
         if M >= 256:
-            engine_small.set_option("gemm_2cta", 0)
+            engine_small.set_option("gemm_wide", 0)
             _, ms = engine_small.debug_gemm(1, A, W, None, None, False, iters=20)
-            engine_small.set_option("gemm_2cta", 1)
+            engine_small.set_option("gemm_wide", 4)
             print(f"gemm one-tile-per-CTA kernel M={M} N={N} K={K}: {ms * 1e3:.1f} us  {2.0 * M * N * K / ms / 1e9:.2f} TFLOP/s")
 
 

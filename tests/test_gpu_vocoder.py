@@ -69,7 +69,7 @@ def test_vocoder_max_length_shape(engine_full, dims_full):
 
 
 # ------------------------------------------------------------------------------------------------
-# fast mode: Conv1d on the tensor cores (tcgen05, fp16 operands, fp32 accumulate) — the precision the
+# fast mode: Conv1d on the tensor cores (wgmma, fp16 operands, fp32 accumulate) — the precision the
 # reference itself runs the vocoder at on GPU (torch.amp.autocast fp16, hifigan_decoder.py:241-242)
 # ------------------------------------------------------------------------------------------------
 TOL_FP16 = 2e-2

@@ -135,29 +135,15 @@ def test_topk_topp_mask_matches_installed_vllm_sampler():
         assert torch.equal(got[~torch.isinf(got)], want[~torch.isinf(want)])
 
 
-def _reference_penalizer():
-    """`LogitsRepetitionPenalizer` lifted by source out of the reference's hijack.py (the module itself imports vLLM 0.6.4)."""
-    import ast
-    from oracle import ref_import
-    path = os.path.join(ref_import.REF_SRC, "auralis", "models", "xttsv2", "components", "vllm", "hijack.py")
-    if not os.path.exists(path):
-        return None
-    tree = ast.parse(open(path).read())
-    cls = [n for n in tree.body if isinstance(n, ast.ClassDef) and n.name == "LogitsRepetitionPenalizer"]
-    from typing import List
-    ns = {"torch": torch, "List": List}
-    exec(compile(ast.Module(body=cls, type_ignores=[]), path, "exec"), ns)
-    return ns["LogitsRepetitionPenalizer"]
+PENALIZER_GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "penalizer_reference.npz")
 
 
-def test_repetition_penalty_matches_the_reference_class(dims_small):
-    """hijack.py:49-88 — the reference's OWN penaliser, run as-is on the prompt the reference builds
-    (`[1]*(32+Lt)+[start]`, vllm_mm_gpt.py:325) plus a generated history with repeats."""
-    Pen = _reference_penalizer()
-    if Pen is None:
-        pytest.skip("reference tree not mounted")
-    g = dims_small.gpt
+def penalizer_trials(dims):
+    """20 (logits, prompt ids, generated ids, penalty) cases: the prompt the reference builds (`[1]*(32+Lt)+[start]`,
+    vllm_mm_gpt.py:325) plus a generated history with repeats"""
+    g = dims.gpt
     rng = np.random.RandomState(4)
+    out = []
     for trial in range(20):
         V = g.n_audio_tokens
         z = torch.from_numpy(rng.randn(V).astype(np.float32) * 3)
@@ -165,11 +151,19 @@ def test_repetition_penalty_matches_the_reference_class(dims_small):
         prompt = [1] * (g.n_cond_latents + n_text) + [g.start_audio_token]
         gen = rng.randint(0, V, size=int(rng.randint(0, 30))).tolist()
         gen = gen + gen[:3]                                              # repeats must be penalised once
-        p = [5.0, 1.0, 2.5, 0.5][trial % 4]
-        want = Pen(p)(prompt, gen, z.clone())
-        seen = O.prompt_seen_set(g) | set(gen)
-        got = O.apply_repetition_penalty(z.clone(), seen, p)
-        assert torch.equal(got, want), (trial, p)
+        out.append((z, prompt, gen, [5.0, 1.0, 2.5, 0.5][trial % 4]))
+    return out
+
+
+def test_repetition_penalty_matches_the_reference_class(dims_small):
+    """hijack.py:49-88 — the reference's OWN penaliser (`LogitsRepetitionPenalizer`), run as-is on penalizer_trials; its
+    outputs are stored in tests/golden/penalizer_reference.npz (tests/golden/make_penalizer_golden.py)."""
+    g = dims_small.gpt
+    with np.load(PENALIZER_GOLDEN) as want:
+        for trial, (z, prompt, gen, p) in enumerate(penalizer_trials(dims_small)):
+            seen = O.prompt_seen_set(g) | set(gen)
+            got = O.apply_repetition_penalty(z.clone(), seen, p)
+            assert torch.equal(got, torch.from_numpy(want[f"trial{trial}"])), (trial, p)
 
 
 def test_batched_decode_equals_per_sequence_decode():

@@ -1,235 +1,133 @@
-"""CPU, container only (needs /root/reference): the oracle restatement against the REFERENCE's own modules, imported
-unmodified (oracle/ref_import.py), on inputs OTHER than the committed golden vectors — ragged lengths, a one-frame
-chunk, several speakers, reference audio that is cut into more than one conditioning chunk.  The golden files
-(tests/golden/*.npz) carry the same pin to machines without the reference tree."""
-import importlib.util
+"""CPU: the oracle restatement against the REFERENCE's own modules on inputs OTHER than tests/golden/{vocoder,conditioning}_*.npz
+— ragged lengths, a one-frame chunk, several speakers, reference audio that is cut into more than one conditioning chunk,
+prompt construction and the GPT wrapper's embedding splice.  What the reference computed on these inputs is stored in
+tests/golden/oracle_live.npz (made by tests/golden/make_oracle_live_golden.py, which imports the reference modules
+unmodified through oracle/ref_import.py or lifts their source where the module itself imports vLLM)."""
 import os
 
 import numpy as np
 import pytest
 import torch
 
-from auralis_b200.config import XTTSDims
-from oracle import ref_import
 from oracle import xtts_oracle as O
 
-pytestmark = pytest.mark.skipif(not ref_import.available(), reason="reference tree not mounted")
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "oracle_live.npz")
+VOCODER_LENGTHS = [1, 2, 7, 33]
+CONDITIONING_CASES = [(0.4, 95.0), (1.3, 180.0)]
+SPEAKER_CASES = [(0.35, 110.0), (0.9, 210.0)]
+CHUNKING_CASES = [(2.6, 30, 1), (2.6, 2, 1), (1.2, 30, 4), (2.2, 30, 1)]     # 2.2 s / 1 s: last piece 0.2 s is dropped
+PROMPT_CASES = [(1, 0), (3, 1)]
+PLACEHOLDER_TEXT_LENS = [3, 17]
+WRAPPER_IDS = [0, 17, 5, 44, 9, 1]
 
 
-def _golden_tools():
-    spec = importlib.util.spec_from_file_location(
-        "make_golden", os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "make_golden.py"))
-    m = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(m)
-    return m
+def WRAPPER_DECODE(g):
+    return [(3, 1), (g.start_audio_token - 1, 7), (60, g.max_audio_tokens)]
+
+
+def vocoder_inputs(dims, T):
+    """(latents [T, in_dim], unit d-vector) of two speakers for a chunk of T frames"""
+    g = torch.Generator().manual_seed(1000 + T)
+    out = []
+    for _ in range(2):
+        lat = torch.randn(T, dims.voc.in_dim, generator=g)
+        gv = torch.nn.functional.normalize(torch.randn(dims.voc.d_vector, generator=g), dim=0)
+        out.append((lat, gv))
+    return out
+
+
+def prompt_chunks(dims, n_chunks, seed):
+    rng = np.random.RandomState(seed)
+    g = dims.gpt
+    return [rng.randint(2, g.n_text_tokens, size=int(rng.randint(1, g.max_text_tokens - 1))).tolist() for _ in range(n_chunks)]
 
 
 @pytest.fixture(scope="module")
-def ref():
-    return ref_import.load()
+def want():
+    with np.load(GOLDEN) as z:
+        return {k: z[k] for k in z.files}
 
 
-@pytest.mark.parametrize("T", [1, 2, 7, 33])
-def test_vocoder_live(ref, dims_small, state_small, T):
-    mg = _golden_tools()
-    hd = mg.ref_vocoder(ref, dims_small, state_small[1])
-    g = torch.Generator().manual_seed(1000 + T)
-    for spk in range(2):
-        lat = torch.randn(T, dims_small.voc.in_dim, generator=g)
-        gv = torch.nn.functional.normalize(torch.randn(dims_small.voc.d_vector, generator=g), dim=0)
-        with torch.no_grad():
-            want = ref.HifiDecoder.forward(hd, lat[None], g=gv.reshape(1, -1, 1)).reshape(-1)
+@pytest.mark.parametrize("T", VOCODER_LENGTHS)
+def test_vocoder_live(want, dims_small, state_small, T):
+    for spk, (lat, gv) in enumerate(vocoder_inputs(dims_small, T)):
+        ref = want[f"voc_T{T}_s{spk}"]
         got = O.vocoder(lat, gv, state_small[1], dims_small)
-        assert got.shape == want.shape == (dims_small.voc.n_samples(T),)
-        np.testing.assert_allclose(got.numpy(), want.numpy(), atol=2e-6, rtol=0)
+        assert got.shape == ref.shape == (dims_small.voc.n_samples(T),)
+        np.testing.assert_allclose(got.numpy(), ref, atol=2e-6, rtol=0)
 
 
-@pytest.mark.parametrize("seconds,f0", [(0.4, 95.0), (1.3, 180.0)])
-def test_conditioning_live(ref, dims_small, state_small, seconds, f0):
+@pytest.mark.parametrize("seconds,f0", CONDITIONING_CASES)
+def test_conditioning_live(want, dims_small, state_small, seconds, f0):
     cs, dims = state_small[1], dims_small
+    case = CONDITIONING_CASES.index((seconds, f0))
     wav22 = O.synthetic_reference_wav(seconds, 22050, f0, 21)
-    mel = ref.wav_to_mel_cloning(wav22[None], mel_norms=cs["mel_stats"], n_fft=2048, hop_length=256, win_length=1024, power=2,
-                                 normalized=False, sample_rate=22050, f_min=0, f_max=8000, n_mels=80)
-    np.testing.assert_allclose(O.mel_cloning(wav22, cs["mel_stats"], dims.cond.n_mels).numpy(), mel[0].numpy(), atol=2e-5, rtol=0)
-    ce = ref.ConditioningEncoder(dims.cond.n_mels, dims.gpt.hidden, attn_blocks=dims.cond.cond_blocks, num_attn_heads=dims.gpt.heads)
-    ce.load_state_dict({k[len("conditioning_encoder."):]: t for k, t in cs.items() if k.startswith("conditioning_encoder.")})
-    pr = ref.PerceiverResampler(dim=dims.gpt.hidden, depth=dims.cond.perceiver_depth, dim_context=dims.gpt.hidden,
-                                num_latents=dims.gpt.n_cond_latents, dim_head=dims.cond.perceiver_dim_head,
-                                heads=dims.cond.perceiver_heads, ff_mult=dims.cond.perceiver_ff_mult, use_flash_attn=False)
-    pr.load_state_dict({k[len("conditioning_perceiver."):]: t for k, t in cs.items() if k.startswith("conditioning_perceiver.")})
-    with torch.no_grad():
-        h = ce(mel)
-        want = pr(h.permute(0, 2, 1))[0]
-    got_h = O.cond_encoder(mel[0], cs, dims)
-    np.testing.assert_allclose(got_h.numpy(), h[0].numpy(), atol=2e-5, rtol=0)
-    np.testing.assert_allclose(O.perceiver(got_h.t(), cs, dims).numpy(), want.numpy(), atol=5e-5, rtol=0)
+    mel = want[f"cond{case}_mel"]
+    np.testing.assert_allclose(O.mel_cloning(wav22, cs["mel_stats"], dims.cond.n_mels).numpy(), mel, atol=2e-5, rtol=0)
+    got_h = O.cond_encoder(torch.from_numpy(mel), cs, dims)
+    np.testing.assert_allclose(got_h.numpy(), want[f"cond{case}_h"], atol=2e-5, rtol=0)
+    np.testing.assert_allclose(O.perceiver(got_h.t(), cs, dims).numpy(), want[f"cond{case}_latents"], atol=5e-5, rtol=0)
 
 
-def test_speaker_encoder_live(ref, dims_small, state_small):
+def test_speaker_encoder_live(want, dims_small, state_small):
     cs, dims = state_small[1], dims_small
-    se = ref.ResNetSpeakerEncoder(input_dim=dims.cond.spk_mels, proj_dim=dims.cond.spk_proj, layers=list(dims.cond.spk_layers),
-                                  num_filters=list(dims.cond.spk_filters), log_input=True, use_torch_spec=True,
-                                  audio_config={"fft_size": 512, "win_length": 400, "hop_length": 160, "sample_rate": 16000,
-                                                "preemphasis": 0.97, "num_mels": 64})
-    pre = "hifigan_decoder.speaker_encoder."
-    se.load_state_dict({k[len(pre):]: t for k, t in cs.items() if k.startswith(pre)})
-    se.eval()
-    for seconds, f0 in ((0.35, 110.0), (0.9, 210.0)):
+    for i, (seconds, f0) in enumerate(SPEAKER_CASES):
         wav16 = O.synthetic_reference_wav(seconds, 16000, f0, 5)
-        with torch.no_grad():
-            want = se.forward(wav16[None].clone(), l2_norm=True)[0]
-        np.testing.assert_allclose(O.speaker_embedding(wav16, cs, dims).numpy(), want.numpy(), atol=2e-6, rtol=0)
+        np.testing.assert_allclose(O.speaker_embedding(wav16, cs, dims).numpy(), want[f"spk{i}"], atol=2e-6, rtol=0)
 
 
-def _lift_methods(path, cls_name, names):
-    """Methods of a reference class lifted by source into plain functions (the module itself imports vLLM 0.6.4)."""
-    import ast
-    tree = ast.parse(open(path).read())
-    cls = next(n for n in tree.body if isinstance(n, ast.ClassDef) and n.name == cls_name)
-    fns = [n for n in cls.body if isinstance(n, (ast.FunctionDef, ast.AsyncFunctionDef)) and n.name in names]
-    assert len(fns) == len(names)
-    return fns
-
-
-def test_gpt_cond_latents_chunking_live(ref, dims_small, state_small):
+def test_gpt_cond_latents_chunking_live(want, dims_small, state_small):
     """XTTSv2Engine.get_gpt_cond_latents (XTTSv2.py:349-407) run AS WRITTEN — truncation to `length` seconds, `chunk_length`
     pieces, pieces under 0.33 s dropped, mean over pieces — on the reference's own encoder modules, against the oracle."""
-    import ast
-    import types
-    from typing import Optional
-    import torchaudio
     cs, dims = state_small[1], dims_small
-    path = os.path.join(ref_import.REF_SRC, "auralis", "models", "xttsv2", "XTTSv2.py")
-    fns = _lift_methods(path, "XTTSv2Engine", ("get_gpt_cond_latents", "get_style_emb"))
-    ns = {"torch": torch, "torchaudio": torchaudio, "wav_to_mel_cloning": ref.wav_to_mel_cloning, "Optional": Optional}
-    exec(compile(ast.Module(body=fns, type_ignores=[]), path, "exec"), ns)
-    ce = ref.ConditioningEncoder(dims.cond.n_mels, dims.gpt.hidden, attn_blocks=dims.cond.cond_blocks, num_attn_heads=dims.gpt.heads)
-    ce.load_state_dict({k[len("conditioning_encoder."):]: t for k, t in cs.items() if k.startswith("conditioning_encoder.")})
-    pr = ref.PerceiverResampler(dim=dims.gpt.hidden, depth=dims.cond.perceiver_depth, dim_context=dims.gpt.hidden,
-                                num_latents=dims.gpt.n_cond_latents, dim_head=dims.cond.perceiver_dim_head,
-                                heads=dims.cond.perceiver_heads, ff_mult=dims.cond.perceiver_ff_mult, use_flash_attn=False)
-    pr.load_state_dict({k[len("conditioning_perceiver."):]: t for k, t in cs.items() if k.startswith("conditioning_perceiver.")})
-    me = types.SimpleNamespace(gpt_config=types.SimpleNamespace(use_perceiver_resampler=True), mel_stats=cs["mel_stats"],
-                               device=torch.device("cpu"), conditioning_encoder=ce, conditioning_perceiver=pr)
-    me.get_style_emb = lambda mel, rl=False: ns["get_style_emb"](me, mel, rl)
-    for seconds, length, chunk in ((2.6, 30, 1), (2.6, 2, 1), (1.2, 30, 4), (2.2, 30, 1)):     # 2.2 s / 1 s: last piece 0.2 s is dropped
+    for i, (seconds, length, chunk) in enumerate(CHUNKING_CASES):
         wav = O.synthetic_reference_wav(seconds, 22050, 140.0, 31)
-        with torch.no_grad():
-            want = ns["get_gpt_cond_latents"](me, wav[None], 22050, length=length, chunk_length=chunk)[0]      # [32, H]
         got = O.gpt_cond_latents(wav, cs, dims, length=length, chunk_length=chunk)
-        assert got.shape == want.shape == (dims.gpt.n_cond_latents, dims.gpt.hidden)
-        np.testing.assert_allclose(got.numpy(), want.numpy(), atol=5e-5, rtol=0)
+        ref = want[f"gcl{i}"]
+        assert got.shape == ref.shape == (dims.gpt.n_cond_latents, dims.gpt.hidden)
+        np.testing.assert_allclose(got.numpy(), ref, atol=5e-5, rtol=0)
 
 
-def test_prompt_construction_live(dims_small, state_small, speakers_small):
+def test_prompt_construction_live(want, dims_small, state_small, speakers_small):
     """Rows a1-a2 of the hot path: XTTSv2Engine.prepare_text_tokens_async + _merge_conditioning (XTTSv2.py:506-543,330-347)
-    and LearnedPositionEmbeddings (vllm_mm_gpt.py:165-214), lifted by source and executed as written with the synthetic
-    embedding tables, against the oracle's prompt rows ([cond latents ; text_emb + text_pos] — the audio-bos row is added by
-    the GPT wrapper, vllm_mm_gpt.py:806-813)."""
-    import ast
-    import asyncio
-    import logging
-    import random
-    import types
-    from typing import List, Tuple, Union
+    and LearnedPositionEmbeddings (vllm_mm_gpt.py:165-214), executed as written with the synthetic embedding tables, against
+    the oracle's prompt rows ([cond latents ; text_emb + text_pos] — the audio-bos row is added by the GPT wrapper,
+    vllm_mm_gpt.py:806-813)."""
     gs, cs = state_small
     g = dims_small.gpt
-    base = os.path.join(ref_import.REF_SRC, "auralis", "models", "xttsv2")
-    fns = _lift_methods(os.path.join(base, "XTTSv2.py"), "XTTSv2Engine", ("prepare_text_tokens_async", "_merge_conditioning"))
-    tree = ast.parse(open(os.path.join(base, "components", "vllm_mm_gpt.py")).read())
-    lpe = [n for n in tree.body if isinstance(n, ast.ClassDef) and n.name == "LearnedPositionEmbeddings"]
-    ns = {"torch": torch, "nn": torch.nn, "random": random, "List": List, "Tuple": Tuple, "Union": Union}
-    exec(compile(ast.Module(body=lpe + fns, type_ignores=[]), "lifted", "exec"), ns)
-    text_emb = torch.nn.Embedding(g.n_text_tokens, g.hidden)
-    text_emb.weight.data.copy_(cs["text_embedding.weight"])
-    text_pos = ns["LearnedPositionEmbeddings"](g.max_text_tokens + 2, g.hidden)
-    text_pos.emb.weight.data.copy_(cs["text_pos_embedding.emb.weight"])
     orc = O.GPTOracle(gs, cs, dims_small)
-    for n_chunks, seed in ((1, 0), (3, 1)):
-        rng = np.random.RandomState(seed)
-        chunks = [rng.randint(2, g.n_text_tokens, size=int(rng.randint(1, g.max_text_tokens - 1))).tolist() for _ in range(n_chunks)]
-        tok = types.SimpleNamespace(bos_token_id=0, eos_token_id=1,
-                                    batch_encode_with_split=lambda text, lang, _c=chunks: [list(c) for c in _c])
-        me = types.SimpleNamespace(tokenizer=tok, text_embedding=text_emb, text_pos_embedding=text_pos, logger=logging.getLogger("x"),
-                                   llm_engine=types.SimpleNamespace(engine=types.SimpleNamespace(model_config=types.SimpleNamespace(dtype=torch.float32))))
-        cond = speakers_small[0][0]                                        # [32, H]
-
-        async def go():
-            fake, embeds = await ns["prepare_text_tokens_async"](me, "ignored", "en", split_text=True)
-            merged = await ns["_merge_conditioning"](me, embeds, cond[None])
-            return fake, merged
-        with torch.no_grad():
-            fake, merged = asyncio.new_event_loop().run_until_complete(go())
-        assert [len(f) for f in fake] == [len(c) + 2 for c in chunks]       # placeholder ids [1]*(L+2) (App. A.2)
-        for c, m in zip(chunks, merged):
+    cond = speakers_small[0][0]                                        # [32, H]
+    for n_chunks, seed in PROMPT_CASES:
+        chunks = prompt_chunks(dims_small, n_chunks, seed)
+        assert want[f"prompt{n_chunks}_fake_lens"].tolist() == [len(c) + 2 for c in chunks]   # placeholder ids [1]*(L+2) (App. A.2)
+        for j, c in enumerate(chunks):
             ids = [0] + c + [1]
             rows = orc.prompt_rows(cond, ids)
             assert rows.shape[0] == g.n_cond_latents + len(ids) + 1
-            np.testing.assert_allclose(rows[:-1].numpy(), m.numpy(), atol=1e-6, rtol=0)
+            np.testing.assert_allclose(rows[:-1].numpy(), want[f"prompt{n_chunks}_{j}"], atol=1e-6, rtol=0)
 
 
-def test_gpt_wrapper_embedding_and_splice_live(dims_small, state_small, speakers_small):
-    """Row a5: the embedding / conditioning-splice part of the reference's GPT2Model.forward (vllm_mm_gpt.py:768-833) lifted by
-    source and executed as written with zero transformer layers: prefill rows = [prefix ; wte[start] + wpe[0]], decode row k =
-    wte[t_k] + wpe[k], and a mixed prefill + decode batch — against the oracle's prompt_rows / audio_row."""
-    import __future__
-    import ast
-    import random
-    import types
+def test_gpt_wrapper_embedding_and_splice_live(want, dims_small, state_small, speakers_small):
+    """Row a5: the embedding / conditioning-splice part of the reference's GPT2Model.forward (vllm_mm_gpt.py:768-833) executed
+    as written with zero transformer layers: prefill rows = [prefix ; wte[start] + wpe[0]], decode row k = wte[t_k] + wpe[k],
+    and a mixed prefill + decode batch — against the oracle's prompt_rows / audio_row."""
     gs, cs = state_small
     g = dims_small.gpt
-    path = os.path.join(ref_import.REF_SRC, "auralis", "models", "xttsv2", "components", "vllm_mm_gpt.py")
-    tree = ast.parse(open(path).read())
-    lpe = [n for n in tree.body if isinstance(n, ast.ClassDef) and n.name == "LearnedPositionEmbeddings"]
-    fns = _lift_methods(path, "GPT2Model", ("forward", "_insert_conditioning_into_hidden_states"))
-    for f in fns:
-        f.decorator_list = []
-    ns = {"torch": torch, "nn": torch.nn, "random": random,
-          "get_pp_group": lambda: types.SimpleNamespace(is_first_rank=True, is_last_rank=True)}
-    exec(compile(ast.Module(body=lpe + fns, type_ignores=[]), "lifted", "exec", flags=__future__.annotations.compiler_flag), ns)
-    wte = torch.nn.Embedding(g.n_audio_tokens, g.hidden)
-    wte.weight.data.copy_(gs["gpt.wte.weight"])
-    wpe = ns["LearnedPositionEmbeddings"](g.max_audio_tokens + 3, g.hidden)
-    wpe.emb.weight.data.copy_(gs["gpt.wpe.emb.weight"])
-    me = types.SimpleNamespace(wte=wte, wpe=wpe, audio_start_generation_token=g.start_audio_token, embed_dim=g.hidden,
-                               start_layer=0, end_layer=0, h=[], ln_f=lambda x: x,
-                               _insert_conditioning_into_hidden_states=ns["_insert_conditioning_into_hidden_states"])
     orc = O.GPTOracle(gs, cs, dims_small)
-    cond = speakers_small[1][0]
-    ids = [0, 17, 5, 44, 9, 1]
-    rows = orc.prompt_rows(cond, ids)
-    prefix = rows[:-1]                                                         # what _merge_conditioning hands to vLLM
-    empty = torch.empty(0, dtype=torch.long)
-    with torch.no_grad():
-        got = ns["forward"](me, empty, empty, [], None, None, input_embeds=[prefix[None]], starting_sequence_start_ids=[0],
-                            is_logit_only=torch.tensor([False]))
-        np.testing.assert_allclose(got.numpy(), rows.numpy(), atol=1e-6, rtol=0)
-        for tok, k in ((3, 1), (g.start_audio_token - 1, 7), (60, g.max_audio_tokens)):
-            got = ns["forward"](me, torch.tensor([tok]), torch.tensor([k]), [], None, None)
-            np.testing.assert_allclose(got[0].numpy(), orc.audio_row(tok, k).numpy(), atol=1e-6, rtol=0)
-        # one sequence decoding (row first), another one starting in the same step (spliced after it)
-        got = ns["forward"](me, torch.tensor([9]), torch.tensor([4]), [], None, None, input_embeds=[prefix[None]],
-                            starting_sequence_start_ids=[1], is_logit_only=torch.tensor([False]))
-        want = torch.cat([orc.audio_row(9, 4)[None], rows], dim=0)
-        np.testing.assert_allclose(got.numpy(), want.numpy(), atol=1e-6, rtol=0)
+    rows = orc.prompt_rows(speakers_small[1][0], WRAPPER_IDS)
+    np.testing.assert_allclose(want["wrapper_prefill"], rows.numpy(), atol=1e-6, rtol=0)
+    for i, (tok, k) in enumerate(WRAPPER_DECODE(g)):
+        np.testing.assert_allclose(want[f"wrapper_decode{i}"], orc.audio_row(tok, k).numpy(), atol=1e-6, rtol=0)
+    # one sequence decoding (row first), another one starting in the same step (spliced after it)
+    np.testing.assert_allclose(want["wrapper_mixed"], torch.cat([orc.audio_row(9, 4)[None], rows], dim=0).numpy(), atol=1e-6, rtol=0)
 
 
-def test_placeholder_prompt_and_penalty_seed_live(dims_small):
+def test_placeholder_prompt_and_penalty_seed_live(want, dims_small):
     """Row a3: input_processor_for_xtts2_gpt (vllm_mm_gpt.py:296-334) executed as written — the prompt vLLM sees is
     [1]*(32+Lt) + [start_audio_token], so the repetition penaliser's prompt set is {1, start} (App. B.7), which is what the
     oracle and the CUDA sampler seed their 'seen' set with."""
-    import __future__
-    import ast
-    import types
-    path = os.path.join(ref_import.REF_SRC, "auralis", "models", "xttsv2", "components", "vllm_mm_gpt.py")
-    tree = ast.parse(open(path).read())
-    fn = [n for n in tree.body if isinstance(n, ast.FunctionDef) and n.name == "input_processor_for_xtts2_gpt"]
-    ns = {"token_inputs": lambda **kw: kw, "PlaceholderRange": lambda **kw: kw}
-    exec(compile(ast.Module(body=fn, type_ignores=[]), "lifted", "exec", flags=__future__.annotations.compiler_flag), ns)
     g = dims_small.gpt
-    ctx = types.SimpleNamespace(model_config=types.SimpleNamespace(hf_config=types.SimpleNamespace(start_audio_token=g.start_audio_token)))
-    for n_text in (3, 17):
-        embeds = torch.zeros(g.n_cond_latents + n_text, g.hidden)
-        out = ns["input_processor_for_xtts2_gpt"](ctx, {"multi_modal_data": {"audio": {"embeds": embeds}}, "prompt_token_ids": [1] * n_text})
-        assert out["prompt_token_ids"] == [1] * (g.n_cond_latents + n_text) + [g.start_audio_token]
-        assert set(out["prompt_token_ids"]) == O.prompt_seen_set(g)
+    for n_text in PLACEHOLDER_TEXT_LENS:
+        ids = want[f"placeholder{n_text}"].tolist()
+        assert ids == [1] * (g.n_cond_latents + n_text) + [g.start_audio_token]
+        assert set(ids) == O.prompt_seen_set(g)

@@ -1,16 +1,15 @@
 """CPU: the Chinese normaliser (auralis_b200/zh_textnorm.py) against the reference's own `zh_num2words` — golden records
-everywhere, live fuzz when /root/reference is mounted."""
+(tests/golden/zh_textnorm.json) and fuzzed sentences (tests/golden/text_live_reference.json.gz)."""
+import gzip
 import json
 import os
 
-import pytest
-
 from auralis_b200 import textnorm as T
 from auralis_b200 import zh_textnorm as Z
-from oracle import ref_import
-from zh_fixture import load_reference_zh, sentences
+from zh_fixture import sentences
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "zh_textnorm.json")
+LIVE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "text_live_reference.json.gz")
 
 
 def test_golden_records_from_the_reference():
@@ -32,18 +31,14 @@ def test_examples():
     assert T.multilingual_cleaners("价格 5£ 和 3°, 共12个!", "zh") == "价格 五 英镑 和 三 度 , 共十二个,"
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree not mounted")
 def test_live_fuzz_against_the_reference_module():
-    z = load_reference_zh()
-    norm = z.TextNorm()
-    for s in sentences(3000, 99):
-        assert Z.normalize(s) == norm(s), s
-    ref_tok = None
-    try:
-        from oracle import ref_text
-        ref_tok = ref_text.load()
-    except Exception:
-        pass
-    if ref_tok is not None:                       # the whole zh cleaner chain of the reference tokenizer
-        for s in sentences(300, 7):
-            assert T.multilingual_cleaners(s, "zh") == ref_tok.multilingual_cleaners(s, "zh"), s
+    """3 000 fuzzed sentences through zh_num2words.TextNorm and 300 through the reference tokenizer's whole zh cleaner chain
+    (tests/zh_fixture.py generates them; the reference's outputs are in tests/golden/text_live_reference.json.gz)."""
+    with gzip.open(LIVE, "rt", encoding="utf-8") as f:
+        rec = json.load(f)
+    assert len(rec["zh_normalize"]) >= 3000 and len(rec["zh_cleaners"]) >= 300
+    assert [s for s, _ in rec["zh_normalize"]] == sentences(3000, 99)        # the stored inputs are the fixture's
+    for s, want in rec["zh_normalize"]:
+        assert Z.normalize(s) == want, s
+    for s, want in rec["zh_cleaners"]:
+        assert T.multilingual_cleaners(s, "zh") == want, s

@@ -1,5 +1,5 @@
 // cp.async.bulk streaming rate per SM as a function of copy size, ring depth and issuing threads (one CTA per SM, consumers
-// only hand the slot back).   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o bulk_probe bulk_probe.cu && ./bulk_probe
+// only hand the slot back).   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o bulk_probe bulk_probe.cu && ./bulk_probe
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

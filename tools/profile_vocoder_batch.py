@@ -1,5 +1,5 @@
 """8 full-length chunks through the engine so that the vocoder runs exactly as in the bench (batch of 8 x 605 latents).
-    ncu --metrics gpu__time_duration.sum -k regex:'conv1d_tc|conv_post|interp|atoms_zero' --csv ... python tools/profile_vocoder_batch.py
+    python tools/profile_vocoder_batch.py [tokens]   (run under a profiler, e.g. torch.profiler or a CUDA-event wrapper)
 """
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -13,7 +13,6 @@ g = torch.Generator().manual_seed(500)
 cond = torch.randn(32, 1024, generator=g); dv = torch.nn.functional.normalize(torch.randn(512, generator=g), dim=0)
 eng = native.NativeEngine(dims, precision=1, max_batch=8, max_speakers=2)
 eng.load_state(gs, cs); eng.set_speaker(0, cond.numpy(), dv.numpy())
-if len(sys.argv) > 2: eng.set_option("conv_epi_groups", int(sys.argv[2]))
 rng = np.random.RandomState(1)
 nt = int(sys.argv[1]) if len(sys.argv) > 1 else 605
 jobs = [(i, [0] + rng.randint(2, 6000, size=78).tolist() + [1], 0,

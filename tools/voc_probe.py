@@ -1,5 +1,5 @@
-"""Vocoder A/B: 8 full-length chunks finish together (batch submit) -> one batch-of-8 vocoder pass; engine vocoder_ms per
-option setting.   python tools/voc_probe.py [tokens]"""
+"""Vocoder timing: 16 full-length chunks finish together (batch submit) -> batched vocoder passes; engine vocoder_ms and
+the tensor-core conv family's profile.   python tools/voc_probe.py [tokens]"""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -20,17 +20,14 @@ def jobs():
              native.Sampling(temperature=0.75, top_p=0.85, top_k=50, max_tokens=nt, seed=1, seq_seed=i, vocode=True, stop_token=-1)) for i in range(NB)]
 eng.set_option("d2h_wav", 0)
 eng.run_batch(jobs(), timeout_s=600, want_wav=False)
-for eg in (1, 2, 1, 2):
-    eng.set_option("conv_epi_groups", eg)
+for rep in range(2):
     eng.set_option("reset_stats", 0)
     res = eng.run_batch(jobs(), timeout_s=600, want_wav=False)
     st = eng.stats()
     audio = sum(r.n_samples for (r, _, _, _) in res.values()) / 24000.0
-    print(f"conv_epi_groups={eg}: vocoder {st.vocoder_ms:8.2f} ms for {NB} chunks ({st.vocoder_ms / NB:.3f} ms/chunk, {audio / (st.vocoder_ms / 1e3):.0f} audio-s/s vocoder-only); gpt {st.gpt_ms:.0f} ms", flush=True)
-for eg in (1, 2):
-    eng.set_option("conv_epi_groups", eg)
-    eng.set_option("profile", 1)
-    eng.run_batch(jobs(), timeout_s=600, want_wav=False)
-    prof = eng.kernel_profile(); eng.set_option("profile", 0)
-    v = prof.get("conv1d_tc_f16_tcgen05")
-    print(f"  profile eg={eg}: conv1d_tc {v['ms']:.2f} ms, {v['launches']} launches, {v['flops'] / v['ms'] / 1e9:.1f} TFLOP/s, {v['bytes'] / v['ms'] / 1e6:.0f} GB/s")
+    print(f"run {rep}: vocoder {st.vocoder_ms:8.2f} ms for {NB} chunks ({st.vocoder_ms / NB:.3f} ms/chunk, {audio / (st.vocoder_ms / 1e3):.0f} audio-s/s vocoder-only); gpt {st.gpt_ms:.0f} ms", flush=True)
+eng.set_option("profile", 1)
+eng.run_batch(jobs(), timeout_s=600, want_wav=False)
+prof = eng.kernel_profile(); eng.set_option("profile", 0)
+v = prof.get("conv1d_tc_f16_wgmma")
+print(f"  profile: conv1d_tc {v['ms']:.2f} ms, {v['launches']} launches, {v['flops'] / v['ms'] / 1e9:.1f} TFLOP/s, {v['bytes'] / v['ms'] / 1e6:.0f} GB/s")
