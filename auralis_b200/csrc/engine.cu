@@ -176,6 +176,15 @@ public:
                     int N, int K, int gelu, int iters, float* ms);
     void debug_sample(const float* logits, const uint8_t* seen, int B, int V, const xtts_sampling& sp, int step,
                       int32_t* out);
+    void debug_attn_decode(int kv_type, int heads, int M, const int32_t* active, int n_slots, const int32_t* ctx_len,
+                           const int32_t* block_tables, int max_pages, int n_pages, void* kpool, void* vpool,
+                           const float* qkv, float* out);
+    void debug_attn_prefill(int out_type, int heads, const int32_t* seqs, int nseq, int causal, float scale,
+                            const float* q, int64_t q_len, int q_row_stride, int q_head_stride,
+                            const float* kv, int64_t kv_len, int kv_row_stride, int kv_head_stride, int64_t k_off,
+                            int64_t v_off, float* out, int out_rows);
+    void debug_splitk_ln(int mode, int M, int N, int K, int splits, const float* A, const float* W, const float* bias,
+                         float* X, const float* ln_w, const float* ln_b, float* Y);
 
 private:
     KernelCtx kctx_;
@@ -2142,6 +2151,161 @@ void Engine::debug_sample(const float* logits, const uint8_t* seen, int Bn, int 
     CUDA_CHECK(cudaStreamSynchronize(st));
 }
 
+// 16-bit device values -> fp32 on the host (exact)
+static void widen16(const std::vector<uint16_t>& in, bool f16, float* out) {
+    for (size_t i = 0; i < in.size(); ++i) {
+        if (f16) { __half_raw r; r.x = in[i]; out[i] = __half2float(__half(r)); }
+        else { const uint32_t u = (uint32_t)in[i] << 16; std::memcpy(&out[i], &u, 4); }
+    }
+}
+
+// One launch of the paged decode attention (launch_attn_decode) on private buffers, under the engine's current attention
+// options.  The pools are raw cache-typed arrays in the device layout (kernels.h); they come back with the appended tokens.
+void Engine::debug_attn_decode(int kv_type, int heads, int M, const int32_t* active, int n_slots, const int32_t* ctx_len,
+                               const int32_t* block_tables, int mp, int n_pages, void* kpool, void* vpool,
+                               const float* qkv, float* out) {
+    ApiLock lk(this);
+    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
+    if (kv_type < 0 || kv_type > 2) throw std::runtime_error("debug_attn_decode: kv_type 0 (fp32), 1 (bf16) or 2 (fp16)");
+    if (heads < 1 || M < 1 || n_slots < 1 || mp < 1 || n_pages < 1) throw std::runtime_error("debug_attn_decode: empty problem");
+    // the kernels' contract: distinct active slots, the new token's page inside the block table, page ids inside the pool
+    std::vector<char> used(n_slots, 0);
+    for (int i = 0; i < M; ++i) {
+        const int s = active[i];
+        if (s < 0 || s >= n_slots || used[s]) throw std::runtime_error("debug_attn_decode: active slots must be distinct and < n_slots");
+        used[s] = 1;
+        if (ctx_len[s] < 0 || ctx_len[s] / kPageTokens >= mp) throw std::runtime_error("debug_attn_decode: ctx_len outside the block table");
+        for (int p = 0; p <= ctx_len[s] / kPageTokens; ++p) {
+            const int id = block_tables[(size_t)s * mp + p];
+            if (id < 0 || id >= n_pages) throw std::runtime_error("debug_attn_decode: page id outside the pool");
+        }
+    }
+    CUDA_CHECK(cudaSetDevice(cfg.device));
+    const size_t esz = kv_type == 0 ? 4 : 2;
+    const size_t pool = (size_t)n_pages * heads * kPageTokens * kHeadDim, Hq = (size_t)heads * kHeadDim;
+    DBuf<int> dact, dctx, dbt;
+    DBuf<float> dqkv;
+    DBuf<uint8_t> dk, dv, dout;
+    dact.alloc(M); dctx.alloc(n_slots); dbt.alloc((size_t)n_slots * mp); dqkv.alloc((size_t)M * 3 * Hq);
+    dk.alloc(pool * esz); dv.alloc(pool * esz); dout.alloc((size_t)M * Hq * esz);
+    dact.upload(active, M, st); dctx.upload(ctx_len, n_slots, st); dbt.upload(block_tables, (size_t)n_slots * mp, st);
+    dqkv.upload(qkv, (size_t)M * 3 * Hq, st);
+    dk.upload(static_cast<const uint8_t*>(kpool), pool * esz, st); dv.upload(static_cast<const uint8_t*>(vpool), pool * esz, st);
+    double ctx_sum = 0;
+    for (int i = 0; i < M; ++i) ctx_sum += ctx_len[active[i]];
+    if (kv_type == 0)
+        launch_attn_decode<float, float>(dqkv.p, dact.p, M, dctx.p, dbt.p, mp, reinterpret_cast<float*>(dk.p),
+                                         reinterpret_cast<float*>(dv.p), reinterpret_cast<float*>(dout.p), heads, st, ctx_sum);
+    else if (kv_type == 1)
+        launch_attn_decode<__nv_bfloat16, __nv_bfloat16>(dqkv.p, dact.p, M, dctx.p, dbt.p, mp, reinterpret_cast<__nv_bfloat16*>(dk.p),
+                                                         reinterpret_cast<__nv_bfloat16*>(dv.p),
+                                                         reinterpret_cast<__nv_bfloat16*>(dout.p), heads, st, ctx_sum);
+    else
+        launch_attn_decode<__half, __half>(dqkv.p, dact.p, M, dctx.p, dbt.p, mp, reinterpret_cast<__half*>(dk.p),
+                                           reinterpret_cast<__half*>(dv.p), reinterpret_cast<__half*>(dout.p), heads, st, ctx_sum);
+    dk.download(static_cast<uint8_t*>(kpool), pool * esz, st); dv.download(static_cast<uint8_t*>(vpool), pool * esz, st);
+    if (kv_type == 0) {
+        dout.download(reinterpret_cast<uint8_t*>(out), (size_t)M * Hq * 4, st);
+        CUDA_CHECK(cudaStreamSynchronize(st));
+    } else {
+        std::vector<uint16_t> o((size_t)M * Hq);
+        dout.download(reinterpret_cast<uint8_t*>(o.data()), o.size() * 2, st);
+        CUDA_CHECK(cudaStreamSynchronize(st));
+        widen16(o, kv_type == 2, out);
+    }
+}
+
+// One launch of the prefill / encoder attention (launch_attn_generic).  q rows and k / v rows are addressed with the given
+// strides (k at kv + k_off, v at kv + v_off); out is [out_rows][heads * 64], rows no sequence covers keep their NaN fill.
+void Engine::debug_attn_prefill(int out_type, int heads, const int32_t* seqs, int nseq, int causal, float scale,
+                                const float* q, int64_t q_len, int q_row_stride, int q_head_stride,
+                                const float* kv, int64_t kv_len, int kv_row_stride, int kv_head_stride, int64_t k_off,
+                                int64_t v_off, float* out, int out_rows) {
+    ApiLock lk(this);
+    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
+    if (out_type < 0 || out_type > 2) throw std::runtime_error("debug_attn_prefill: out_type 0 (fp32), 1 (bf16) or 2 (fp16)");
+    if (heads < 1 || nseq < 1 || out_rows < 1 || q_len < 1 || kv_len < 1) throw std::runtime_error("debug_attn_prefill: empty problem");
+    const int Hq = heads * kHeadDim;
+    int max_nq = 0;
+    auto last = [&](int64_t row, int64_t rs, int64_t hs) { return row * rs + (int64_t)(heads - 1) * hs + kHeadDim - 1; };
+    for (int i = 0; i < nseq; ++i) {
+        const int32_t* s = seqs + 4 * i;        // q_start, nq, kv_start, nk
+        if (s[0] < 0 || s[1] < 1 || s[2] < 0 || s[3] < 1 || s[0] + s[1] > out_rows)
+            throw std::runtime_error("debug_attn_prefill: sequence outside the output rows");
+        if (causal && s[3] < s[1]) throw std::runtime_error("debug_attn_prefill: causal attention needs nk >= nq");
+        if (last(s[0] + s[1] - 1, q_row_stride, q_head_stride) >= q_len ||
+            std::max(k_off, v_off) + last(s[2] + s[3] - 1, kv_row_stride, kv_head_stride) >= kv_len || std::min(k_off, v_off) < 0)
+            throw std::runtime_error("debug_attn_prefill: sequence outside the q / kv buffers");
+        max_nq = std::max(max_nq, (int)s[1]);
+    }
+    CUDA_CHECK(cudaSetDevice(cfg.device));
+    const size_t esz = out_type == 0 ? 4 : 2, n_out = (size_t)out_rows * Hq;
+    DBuf<float> dq, dkv;
+    DBuf<AttnSeq> dseq;
+    DBuf<uint8_t> dout;
+    dq.alloc(q_len); dkv.alloc(kv_len); dseq.alloc(nseq); dout.alloc(n_out * esz);
+    dq.upload(q, q_len, st); dkv.upload(kv, kv_len, st);
+    dseq.upload(reinterpret_cast<const AttnSeq*>(seqs), nseq, st);
+    CUDA_CHECK(cudaMemsetAsync(dout.p, 0xFF, n_out * esz, st));        // NaN in every output type
+    AttnLayout A;
+    A.q = dq.p; A.k = dkv.p + k_off; A.v = dkv.p + v_off;
+    A.q_row_stride = q_row_stride; A.kv_row_stride = kv_row_stride; A.q_head_stride = q_head_stride; A.kv_head_stride = kv_head_stride;
+    A.heads = heads; A.scale = scale; A.causal = causal ? 1 : 0;
+    if (out_type == 0) launch_attn_generic<float>(A, dseq.p, nseq, max_nq, reinterpret_cast<float*>(dout.p), Hq, st);
+    else if (out_type == 1) launch_attn_generic<__nv_bfloat16>(A, dseq.p, nseq, max_nq, reinterpret_cast<__nv_bfloat16*>(dout.p), Hq, st);
+    else launch_attn_generic<__half>(A, dseq.p, nseq, max_nq, reinterpret_cast<__half*>(dout.p), Hq, st);
+    if (out_type == 0) {
+        dout.download(reinterpret_cast<uint8_t*>(out), n_out * 4, st);
+        CUDA_CHECK(cudaStreamSynchronize(st));
+    } else {
+        std::vector<uint16_t> o(n_out);
+        dout.download(reinterpret_cast<uint8_t*>(o.data()), n_out * 2, st);
+        CUDA_CHECK(cudaStreamSynchronize(st));
+        widen16(o, out_type == 2, out);
+    }
+}
+
+// The decode step's split-K projection + residual / LayerNorm pair, as layers_forward runs it: the 16-bit GEMM into fp32
+// partials, then X += bias + sum of the partials and Y = LN(X) (Y skipped without ln_w / ln_b: the last layer's form).
+void Engine::debug_splitk_ln(int mode, int M, int N, int K, int splits, const float* A, const float* W, const float* bias,
+                             float* X, const float* ln_w, const float* ln_b, float* Y) {
+    ApiLock lk(this);
+    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
+    if (mode != 1 && mode != 2) throw std::runtime_error("debug_splitk_ln: mode 1 (bf16) or 2 (fp16)");
+    if (M < 1 || N < 32 || N % 32 != 0 || N > 8192 || K < 64 || K % 64 != 0 || splits < 1 || splits > 8 || (K / 64) % splits != 0)
+        throw std::runtime_error("debug_splitk_ln: need N % 32 == 0 (<= 8192), K % 64 == 0, 1 <= splits <= 8 dividing K / 64");
+    if (!bias || (ln_w == nullptr) != (ln_b == nullptr) || (ln_w && !Y)) throw std::runtime_error("debug_splitk_ln: bias, and ln_w / ln_b / Y together");
+    CUDA_CHECK(cudaSetDevice(cfg.device));
+    std::string err;
+    if (!gemm_tc_init(&err)) throw std::runtime_error(err);
+    DBuf<float> dA, dW, db, dX, dlw, dlb, dpart;
+    DBuf<__nv_bfloat16> hA, hW, dY;                 // 16-bit operands / output (IEEE fp16 bits in mode 2)
+    dA.alloc((size_t)M * K); dW.alloc((size_t)N * K); db.alloc(N); dX.alloc((size_t)M * N); dpart.alloc((size_t)splits * M * N);
+    hA.alloc((size_t)M * K); hW.alloc((size_t)N * K);
+    dA.upload(A, (size_t)M * K, st); dW.upload(W, (size_t)N * K, st); db.upload(bias, N, st); dX.upload(X, (size_t)M * N, st);
+    if (ln_w) {
+        dlw.alloc(N); dlb.alloc(N); dY.alloc((size_t)M * N);
+        dlw.upload(ln_w, N, st); dlb.upload(ln_b, N, st);
+    }
+    if (mode == 1) {
+        launch_f32_to_bf16(dA.p, hA.p, (size_t)M * K, st); launch_f32_to_bf16(dW.p, hW.p, (size_t)N * K, st);
+    } else {
+        launch_f32_to_f16(dA.p, reinterpret_cast<__half*>(hA.p), (size_t)M * K, st);
+        launch_f32_to_f16(dW.p, reinterpret_cast<__half*>(hW.p), (size_t)N * K, st);
+    }
+    launch_gemm_bf16_tc_splitk(hA.p, hW.p, dpart.p, M, N, K, splits, st, false, DepFlag(), mode == 2 ? GEMM_F16 : 0);
+    if (mode == 2)
+        launch_residual_reduce_layernorm<__half>(dX.p, dpart.p, splits, db.p, dlw.p, dlb.p, reinterpret_cast<__half*>(dY.p), M, N,
+                                                 cfg.ln_eps, st);
+    else
+        launch_residual_reduce_layernorm<__nv_bfloat16>(dX.p, dpart.p, splits, db.p, dlw.p, dlb.p, dY.p, M, N, cfg.ln_eps, st);
+    dX.download(X, (size_t)M * N, st);
+    std::vector<uint16_t> y(ln_w ? (size_t)M * N : 0);
+    if (ln_w) dY.download(reinterpret_cast<__nv_bfloat16*>(y.data()), y.size(), st);
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    if (ln_w) widen16(y, mode == 2, Y);
+}
+
 }  // namespace xtts
 
 // ================================================================================================
@@ -2234,6 +2398,23 @@ int xtts_debug_gemm(xtts_engine* e, int32_t mode, const float* A, const float* W
 int xtts_debug_sample(xtts_engine* e, const float* logits, const uint8_t* seen, int32_t B, int32_t V,
                       const xtts_sampling* sp, int32_t step, int32_t* out_tokens) {
     XTTS_TRY(e->impl->debug_sample(logits, seen, B, V, *sp, step, out_tokens))
+}
+int xtts_debug_attn_decode(xtts_engine* e, int32_t kv_type, int32_t heads, int32_t M, const int32_t* active, int32_t n_slots,
+                           const int32_t* ctx_len, const int32_t* block_tables, int32_t max_pages, int32_t n_pages,
+                           void* kpool, void* vpool, const float* qkv, float* out) {
+    XTTS_TRY(e->impl->debug_attn_decode(kv_type, heads, M, active, n_slots, ctx_len, block_tables, max_pages, n_pages, kpool, vpool,
+                                        qkv, out))
+}
+int xtts_debug_attn_prefill(xtts_engine* e, int32_t out_type, int32_t heads, const int32_t* seqs, int32_t nseq, int32_t causal,
+                            float scale, const float* q, int64_t q_len, int32_t q_row_stride, int32_t q_head_stride,
+                            const float* kv, int64_t kv_len, int32_t kv_row_stride, int32_t kv_head_stride, int64_t k_off,
+                            int64_t v_off, float* out, int32_t out_rows) {
+    XTTS_TRY(e->impl->debug_attn_prefill(out_type, heads, seqs, nseq, causal, scale, q, q_len, q_row_stride, q_head_stride, kv,
+                                         kv_len, kv_row_stride, kv_head_stride, k_off, v_off, out, out_rows))
+}
+int xtts_debug_splitk_ln(xtts_engine* e, int32_t mode, int32_t M, int32_t N, int32_t K, int32_t splits, const float* A,
+                         const float* W, const float* bias, float* X, const float* ln_w, const float* ln_b, float* Y) {
+    XTTS_TRY(e->impl->debug_splitk_ln(mode, M, N, K, splits, A, W, bias, X, ln_w, ln_b, Y))
 }
 
 }  // extern "C"

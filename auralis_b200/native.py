@@ -77,6 +77,7 @@ ABI_SYMBOLS = [
     "xtts_set_speaker", "xtts_get_speaker", "xtts_condition", "xtts_submit", "xtts_cancel", "xtts_poll", "xtts_fetch",
     "xtts_set_option", "xtts_get_stats", "xtts_sync", "xtts_get_kernel_profile", "xtts_device_timer", "xtts_vocode", "xtts_vocode_window", "xtts_gpt_prefill", "xtts_gpt_teacher_forced",
     "xtts_debug_gemm", "xtts_debug_sample", "xtts_debug_trace",
+    "xtts_debug_attn_decode", "xtts_debug_attn_prefill", "xtts_debug_splitk_ln",
 ]
 
 _lib = None
@@ -117,6 +118,10 @@ def load_library(path: Optional[str] = None):
     lib.xtts_debug_gemm.argtypes = [vp, i32, f32p, f32p, f32p, f32p, f32p, i32, i32, i32, i32, i32, f32p]
     lib.xtts_debug_sample.argtypes = [vp, f32p, C.POINTER(C.c_uint8), i32, i32, C.POINTER(XttsSampling), i32, i32p]
     lib.xtts_debug_trace.argtypes = [vp, i32, C.POINTER(C.c_uint64), i32]
+    lib.xtts_debug_attn_decode.argtypes = [vp, i32, i32, i32, i32p, i32, i32p, i32p, i32, i32, vp, vp, f32p, f32p]
+    lib.xtts_debug_attn_prefill.argtypes = [vp, i32, i32, i32p, i32, i32, C.c_float, f32p, i64, i32, i32, f32p, i64, i32, i32,
+                                            i64, i64, f32p, i32]
+    lib.xtts_debug_splitk_ln.argtypes = [vp, i32, i32, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, f32p, f32p]
     for s in ABI_SYMBOLS:
         if s not in ("xtts_last_error", "xtts_version"):
             getattr(lib, s).restype = C.c_int
@@ -425,3 +430,48 @@ class NativeEngine:
         self._chk(self.lib.xtts_debug_sample(self.h, _fp(lg), sn.ctypes.data_as(C.POINTER(C.c_uint8)) if sn is not None else None,
                                              Bn, V, C.byref(cs), step, _ip(out)), "debug_sample")
         return out
+
+    # KV type code of xtts_debug_attn_decode -> numpy dtype of the raw pool elements (bf16 as its uint16 bit pattern)
+    KV_DTYPES = {0: np.float32, 1: np.uint16, 2: np.float16}
+
+    def debug_attn_decode(self, kv_type: int, heads: int, qkv, active, ctx_len, block_tables, kpool, vpool):
+        """One decode-attention launch under the current options.  kpool / vpool: [n_pages, heads, 32 * 64] raw cache
+        elements in the device layout (include/xtts_b200.h), dtype KV_DTYPES[kv_type].  -> (out [M, heads*64] fp32,
+        kpool after, vpool after)."""
+        q, act, ctx, bt = _f32(qkv), _i32(active), _i32(ctx_len), _i32(block_tables)
+        dt = self.KV_DTYPES[kv_type]
+        k = np.ascontiguousarray(kpool, dtype=dt).copy()
+        v = np.ascontiguousarray(vpool, dtype=dt).copy()
+        assert k.shape == v.shape and k.shape[1] == heads and bt.ndim == 2 and bt.shape[0] == ctx.size
+        M = act.size
+        out = np.empty((M, heads * 64), np.float32)
+        self._chk(self.lib.xtts_debug_attn_decode(self.h, kv_type, heads, M, _ip(act), ctx.size, _ip(ctx), _ip(bt), bt.shape[1],
+                                                  k.shape[0], k.ctypes.data, v.ctypes.data, _fp(q), _fp(out)),
+                  "debug_attn_decode")
+        return out, k, v
+
+    def debug_attn_prefill(self, out_type: int, heads: int, seqs, causal: bool, scale: float, q, q_row_stride: int,
+                           q_head_stride: int, kv, kv_row_stride: int, kv_head_stride: int, k_off: int, v_off: int,
+                           out_rows: int):
+        """One prefill-attention launch.  seqs: [(q_start, nq, kv_start, nk)]; q / kv: flat fp32 buffers addressed with the
+        strides (include/xtts_b200.h).  -> out [out_rows, heads*64] fp32 (NaN where no sequence writes)."""
+        s, qq, kk = _i32(seqs).reshape(-1, 4), _f32(q).reshape(-1), _f32(kv).reshape(-1)
+        out = np.empty((out_rows, heads * 64), np.float32)
+        self._chk(self.lib.xtts_debug_attn_prefill(self.h, out_type, heads, _ip(s), s.shape[0], 1 if causal else 0, scale,
+                                                   _fp(qq), qq.size, q_row_stride, q_head_stride, _fp(kk), kk.size,
+                                                   kv_row_stride, kv_head_stride, k_off, v_off, _fp(out), out_rows),
+                  "debug_attn_prefill")
+        return out
+
+    def debug_splitk_ln(self, mode: int, A, W, bias, X, splits: int, ln_w=None, ln_b=None):
+        """Split-K 16-bit GEMM + fused residual / LayerNorm (mode 1 bf16, 2 fp16).  -> (X + bias + A.W^T, LN of it or None)."""
+        A, W, b = _f32(A), _f32(W), _f32(bias)
+        x = _f32(X).copy()
+        M, K = A.shape
+        N = W.shape[0]
+        lw = _f32(ln_w) if ln_w is not None else None
+        lb = _f32(ln_b) if ln_b is not None else None
+        y = np.empty((M, N), np.float32) if lw is not None else None
+        self._chk(self.lib.xtts_debug_splitk_ln(self.h, mode, M, N, K, splits, _fp(A), _fp(W), _fp(b), _fp(x), _fp(lw),
+                                                _fp(lb), _fp(y)), "debug_splitk_ln")
+        return x, y

@@ -203,6 +203,28 @@ int xtts_debug_trace(xtts_engine* e, int32_t op, uint64_t* out, int32_t cap);
 /* sampler under test: logits [B,V]; seen [B,V] (0/1) ; out tokens [B] */
 int xtts_debug_sample(xtts_engine* e, const float* logits, const uint8_t* seen, int32_t B, int32_t V,
                       const xtts_sampling* sp, int32_t step, int32_t* out_tokens);
+/* Single-kernel entry points below: an idle engine, private device buffers, the engine's current kernel options
+ * (xtts_set_option), no engine state touched. */
+/* paged decode attention (one launch, appends each row's k / v): kv_type 0 fp32, 1 bf16, 2 fp16 (the output has the cache
+ * type, returned as fp32).  active [M] (distinct slots < n_slots), ctx_len [n_slots], block_tables [n_slots][max_pages];
+ * kpool / vpool: n_pages pages of raw cache-typed elements in the device layout (K [page][head][64/X][32 tok][X], X = 16 bytes
+ * per element group; V [page][head][32 tok][64]), updated in place; qkv [M][3 * heads * 64]; out [M][heads * 64] */
+int xtts_debug_attn_decode(xtts_engine* e, int32_t kv_type, int32_t heads, int32_t M, const int32_t* active, int32_t n_slots,
+                           const int32_t* ctx_len, const int32_t* block_tables, int32_t max_pages, int32_t n_pages,
+                           void* kpool, void* vpool, const float* qkv, float* out);
+/* prefill / encoder attention (head dim 64): out_type 0 fp32, 1 bf16, 2 fp16 (returned as fp32); seqs [nseq][4] =
+ * (q_start, nq, kv_start, nk); q element (row r, head h, dim d) at q[r * q_row_stride + h * q_head_stride + d], k / v at
+ * kv[k_off | v_off + r * kv_row_stride + h * kv_head_stride + d]; causal: key j visible to query i iff j <= i + nk - nq;
+ * out [out_rows][heads * 64], rows outside every sequence are NaN */
+int xtts_debug_attn_prefill(xtts_engine* e, int32_t out_type, int32_t heads, const int32_t* seqs, int32_t nseq, int32_t causal,
+                            float scale, const float* q, int64_t q_len, int32_t q_row_stride, int32_t q_head_stride,
+                            const float* kv, int64_t kv_len, int32_t kv_row_stride, int32_t kv_head_stride, int64_t k_off,
+                            int64_t v_off, float* out, int32_t out_rows);
+/* decode projection as in fast mode: mode 1 bf16 / 2 fp16 operands, partials = split-K GEMM of A [M,K] . W [N,K]^T in `splits`
+ * K ranges, then X [M,N] += bias + sum of partials (in place) and Y = LayerNorm(X; ln_w, ln_b, the engine's eps) in the
+ * 16-bit type (returned as fp32); ln_w = ln_b = NULL: X only (the last layer) */
+int xtts_debug_splitk_ln(xtts_engine* e, int32_t mode, int32_t M, int32_t N, int32_t K, int32_t splits, const float* A,
+                         const float* W, const float* bias, float* X, const float* ln_w, const float* ln_b, float* Y);
 
 #ifdef __cplusplus
 }
