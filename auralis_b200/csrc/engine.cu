@@ -185,6 +185,9 @@ public:
                             int64_t v_off, float* out, int out_rows);
     void debug_splitk_ln(int mode, int M, int N, int K, int splits, const float* A, const float* W, const float* bias,
                          float* X, const float* ln_w, const float* ln_b, float* Y);
+    void debug_conv_tc(int up, int Cin, int Cout, int K, int dil, int batch, int L, const int32_t* item_len, const float* w,
+                       const float* bias, const float* cbias, int cbias_stride, const float* x, const float* resid, int mode,
+                       float slope_out, float scale16, int max_ctas, float* out32, float* out16);
 
 private:
     KernelCtx kctx_;
@@ -2306,6 +2309,82 @@ void Engine::debug_splitk_ln(int mode, int M, int N, int K, int splits, const fl
     if (ln_w) widen16(y, mode == 2, Y);
 }
 
+// One launch of the fast-mode vocoder convolution (launch_conv1d_tc, or launch_convT_tc for up > 0) with the weights
+// packed and planned as make_conv does.  The input atom image is NaN except each item's signal rows; the production pad
+// routine then clears what it claims the kernel reads, so any other read reaches a stored output as NaN.  out32 / out16
+// are in/out: their incoming contents are the accumulate base and the sentinels of every row the kernel must not write.
+void Engine::debug_conv_tc(int up, int Cin, int Cout, int K, int dil, int batch, int L, const int32_t* item_len,
+                           const float* w, const float* bias, const float* cbias, int cbias_stride, const float* x,
+                           const float* resid, int mode, float slope_out, float scale16, int max_ctas, float* out32,
+                           float* out16) {
+    ApiLock lk(this);
+    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
+    if (up != 0 && up != 2 && up != 4 && up != 8) throw std::runtime_error("debug_conv_tc: up 0 (Conv1d) or 2, 4, 8 (ConvTranspose1d)");
+    if (up == 0 && (K < 1 || K % 2 == 0 || dil < 1)) throw std::runtime_error("debug_conv_tc: Conv1d needs an odd K and dil >= 1");
+    if (up > 0 && (K != 2 * up || dil != 1)) throw std::runtime_error("debug_conv_tc: ConvTranspose1d needs K = 2 * up and dil = 1");
+    if (up > 0 && (resid || mode != CONV_STORE || scale16 != 1.0f))
+        throw std::runtime_error("debug_conv_tc: ConvTranspose1d takes no resid, mode STORE and scale16 1");
+    if (mode != CONV_STORE && mode != CONV_ACCUM) throw std::runtime_error("debug_conv_tc: mode 0 (store) or 1 (accumulate)");
+    if (mode == CONV_ACCUM && !out32) throw std::runtime_error("debug_conv_tc: accumulate mode needs out32");
+    if (up == 0 && (K - 1) / 2 * dil > kAtomPadL) throw std::runtime_error("debug_conv_tc: halo (K-1)/2*dil exceeds the atom head pad");
+    if (batch < 1 || batch > kVocMaxItems) throw std::runtime_error("debug_conv_tc: batch must be 1..32");
+    if (L < 1) throw std::runtime_error("debug_conv_tc: L must be >= 1");
+    if (!w) throw std::runtime_error("debug_conv_tc: w is required");
+    if (!x) throw std::runtime_error("debug_conv_tc: x is required");
+    std::vector<int> lens(batch, L);
+    for (int i = 0; i < batch && item_len; ++i) {
+        if (item_len[i] < 0 || item_len[i] > L) throw std::runtime_error("debug_conv_tc: item_len must lie in [0, L]");
+        lens[i] = item_len[i];
+    }
+    if (Cin < 1 || Cout < 1) throw std::runtime_error("debug_conv_tc: empty channel count");
+    const ConvTcPlan pl = up ? conv1d_tc_plan(Cin, up * Cout, 2) : conv1d_tc_plan(Cin, Cout, K);
+    if (!pl.ok) throw std::runtime_error("debug_conv_tc: no tensor-core plan for these channel counts");
+    if (up > 0 && Cout % 32 != 0) throw std::runtime_error("debug_conv_tc: ConvTranspose1d needs Cout % 32 == 0");
+    if (out16 && Cout % 8 != 0) throw std::runtime_error("debug_conv_tc: out16 needs Cout % 8 == 0");
+    if (cbias && cbias_stride < Cout) throw std::runtime_error("debug_conv_tc: cbias_stride < Cout");
+    if (max_ctas < 0) throw std::runtime_error("debug_conv_tc: max_ctas must be >= 0");
+    CUDA_CHECK(cudaSetDevice(cfg.device));
+    const int Lout = up ? L * up : L, lpad = atoms_lpad(L), lpad_out = atoms_lpad(Lout);
+    std::vector<__half> blob(pl.blob_halves);
+    if (up) convT_tc_pack(w, Cin, Cout, up, pl, blob.data());
+    else conv1d_tc_pack(w, Cin, Cout, K, pl, blob.data());
+    __half_raw nan_raw; nan_raw.x = 0x7e00;
+    const size_t n_in = (size_t)batch * Cin * lpad, n32 = (size_t)batch * Cout * Lout, n16 = (size_t)batch * Cout * lpad_out;
+    std::vector<__half> a(n_in, __half(nan_raw));
+    for (int b = 0; b < batch; ++b)
+        for (int c = 0; c < Cin; ++c)
+            for (int t = 0; t < lens[b]; ++t)
+                a[(((size_t)b * (Cin / 8) + c / 8) * lpad + kAtomPadL + t) * 8 + c % 8] = __float2half_rn(x[((size_t)b * Cin + c) * L + t]);
+    DBuf<__half> da, dblob, do16;
+    DBuf<float> dbias, dcb, dres, do32;
+    da.alloc(n_in); dblob.alloc(blob.size());
+    da.upload(a.data(), n_in, st); dblob.upload(blob.data(), blob.size(), st);
+    if (bias) { dbias.alloc(Cout); dbias.upload(bias, Cout, st); }
+    if (cbias) { dcb.alloc((size_t)batch * cbias_stride); dcb.upload(cbias, (size_t)batch * cbias_stride, st); }
+    if (resid) { dres.alloc(n32); dres.upload(resid, n32, st); }
+    if (out32) { do32.alloc(n32); do32.upload(out32, n32, st); }
+    std::vector<__half> o16(out16 ? n16 : 0);
+    if (out16) {
+        for (size_t i = 0; i < n16; ++i) o16[i] = __float2half_rn(out16[i]);
+        do16.alloc(n16); do16.upload(o16.data(), n16, st);
+    }
+    launch_atoms_zero_pads(da.p, batch * Cin / 8, lpad, L, st, batch, lens.data());
+    const int* il = item_len ? lens.data() : nullptr;
+    struct CapRestore { int& cap; int prev; ~CapRestore() { cap = prev; } } restore{g_voc_sm_cap, g_voc_sm_cap};
+    g_voc_sm_cap = max_ctas;
+    if (up)
+        launch_convT_tc(da.p, dblob.p, pl, dbias.p, dcb.p, do32.p, do16.p, Cin, Cout, L, lpad, lpad_out, up, slope_out, batch,
+                        cbias_stride, st, il);
+    else
+        launch_conv1d_tc(da.p, dblob.p, pl, dbias.p, dcb.p, dres.p, do32.p, do16.p, Cin, Cout, L, lpad, K, dil, slope_out,
+                         scale16, mode, batch, cbias_stride, st, il);
+    if (out32) do32.download(out32, n32, st);
+    std::vector<uint16_t> r16(out16 ? n16 : 0);
+    if (out16) do16.download(reinterpret_cast<__half*>(r16.data()), n16, st);
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    if (out16) widen16(r16, true, out16);
+}
+
 }  // namespace xtts
 
 // ================================================================================================
@@ -2415,6 +2494,13 @@ int xtts_debug_attn_prefill(xtts_engine* e, int32_t out_type, int32_t heads, con
 int xtts_debug_splitk_ln(xtts_engine* e, int32_t mode, int32_t M, int32_t N, int32_t K, int32_t splits, const float* A,
                          const float* W, const float* bias, float* X, const float* ln_w, const float* ln_b, float* Y) {
     XTTS_TRY(e->impl->debug_splitk_ln(mode, M, N, K, splits, A, W, bias, X, ln_w, ln_b, Y))
+}
+int xtts_debug_conv_tc(xtts_engine* e, int32_t up, int32_t Cin, int32_t Cout, int32_t K, int32_t dil, int32_t batch, int32_t L,
+                       const int32_t* item_len, const float* w, const float* bias, const float* cbias, int32_t cbias_stride,
+                       const float* x, const float* resid, int32_t mode, float slope_out, float scale16, int32_t max_ctas,
+                       float* out32, float* out16) {
+    XTTS_TRY(e->impl->debug_conv_tc(up, Cin, Cout, K, dil, batch, L, item_len, w, bias, cbias, cbias_stride, x, resid, mode,
+                                    slope_out, scale16, max_ctas, out32, out16))
 }
 
 }  // extern "C"

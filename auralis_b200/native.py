@@ -77,7 +77,7 @@ ABI_SYMBOLS = [
     "xtts_set_speaker", "xtts_get_speaker", "xtts_condition", "xtts_submit", "xtts_cancel", "xtts_poll", "xtts_fetch",
     "xtts_set_option", "xtts_get_stats", "xtts_sync", "xtts_get_kernel_profile", "xtts_device_timer", "xtts_vocode", "xtts_vocode_window", "xtts_gpt_prefill", "xtts_gpt_teacher_forced",
     "xtts_debug_gemm", "xtts_debug_sample", "xtts_debug_trace",
-    "xtts_debug_attn_decode", "xtts_debug_attn_prefill", "xtts_debug_splitk_ln",
+    "xtts_debug_attn_decode", "xtts_debug_attn_prefill", "xtts_debug_splitk_ln", "xtts_debug_conv_tc",
 ]
 
 _lib = None
@@ -122,6 +122,8 @@ def load_library(path: Optional[str] = None):
     lib.xtts_debug_attn_prefill.argtypes = [vp, i32, i32, i32p, i32, i32, C.c_float, f32p, i64, i32, i32, f32p, i64, i32, i32,
                                             i64, i64, f32p, i32]
     lib.xtts_debug_splitk_ln.argtypes = [vp, i32, i32, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, f32p, f32p]
+    lib.xtts_debug_conv_tc.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, i32p, f32p, f32p, f32p, i32, f32p, f32p, i32,
+                                       C.c_float, C.c_float, i32, f32p, f32p]
     for s in ABI_SYMBOLS:
         if s not in ("xtts_last_error", "xtts_version"):
             getattr(lib, s).restype = C.c_int
@@ -135,6 +137,12 @@ def _f32(a) -> np.ndarray:
 
 def _i32(a) -> np.ndarray:
     return np.ascontiguousarray(np.asarray(a, dtype=np.int32))
+
+
+def atoms_lpad(L: int) -> int:
+    """Rows per plane of an fp16 atom image holding a signal of L steps (atoms_lpad in csrc/conv1d_tc.cu): a 64-row head
+    pad, the signal plus at least one zero row rounded up to 512, a 64-row tail pad."""
+    return 64 + -(-(L + 1) // 512) * 512 + 64
 
 
 def _fp(a: Optional[np.ndarray]):
@@ -475,3 +483,35 @@ class NativeEngine:
         self._chk(self.lib.xtts_debug_splitk_ln(self.h, mode, M, N, K, splits, _fp(A), _fp(W), _fp(b), _fp(x), _fp(lw),
                                                 _fp(lb), _fp(y)), "debug_splitk_ln")
         return x, y
+
+    CONV_STORE, CONV_ACCUM = 0, 1
+
+    def debug_conv_tc(self, x, w, up: int = 0, dil: int = 1, item_len=None, bias=None, cbias=None, resid=None,
+                      mode: int = 0, slope_out: float = 0.1, scale16: float = 1.0, max_ctas: int = 0, out32=None,
+                      out16=None):
+        """One launch of the fast-mode vocoder convolution (include/xtts_b200.h).  x [batch, Cin, L]; w [Cout, Cin, K]
+        (up 0, Conv1d) or [Cin, Cout, 2 * up] (ConvTranspose1d); cbias [batch, stride].  out32 [batch, Cout, Lout] and
+        out16 [batch, Cout / 8, atoms_lpad(Lout), 8] are the incoming contents (accumulate base, sentinels); None = not
+        produced.  -> (out32, out16) after the launch."""
+        x, w = _f32(x), _f32(w)
+        B, Cin, L = x.shape
+        Cout, K = (w.shape[1], w.shape[2]) if up else (w.shape[0], w.shape[2])
+        if w.shape[0 if up else 1] != Cin:
+            raise ValueError(f"weight {w.shape} does not take {Cin} input channels")
+        Lout = L * up if up else L
+        il = _i32(item_len) if item_len is not None else None
+        cb = _f32(cbias) if cbias is not None else None
+        r = _f32(resid) if resid is not None else None
+        b = _f32(bias) if bias is not None else None
+        o32 = _f32(out32).copy() if out32 is not None else None
+        o16 = _f32(out16).copy() if out16 is not None else None
+        for name, a, n in [("item_len", il, B), ("bias", b, Cout), ("resid", r, B * Cout * Lout),
+                           ("out32", o32, B * Cout * Lout), ("out16", o16, B * Cout * atoms_lpad(Lout))]:
+            if a is not None and a.size != n:
+                raise ValueError(f"{name} has {a.size} elements, expected {n}")
+        if cb is not None and (cb.ndim != 2 or cb.shape[0] != B):
+            raise ValueError(f"cbias must be [batch, stride], got {cb.shape}")
+        self._chk(self.lib.xtts_debug_conv_tc(self.h, up, Cin, Cout, K, dil, B, L, _ip(il), _fp(w), _fp(b), _fp(cb),
+                                              cb.shape[1] if cb is not None else 0, _fp(x), _fp(r), mode, slope_out,
+                                              scale16, max_ctas, _fp(o32), _fp(o16)), "debug_conv_tc")
+        return o32, o16

@@ -225,6 +225,23 @@ int xtts_debug_attn_prefill(xtts_engine* e, int32_t out_type, int32_t heads, con
  * 16-bit type (returned as fp32); ln_w = ln_b = NULL: X only (the last layer) */
 int xtts_debug_splitk_ln(xtts_engine* e, int32_t mode, int32_t M, int32_t N, int32_t K, int32_t splits, const float* A,
                          const float* W, const float* bias, float* X, const float* ln_w, const float* ln_b, float* Y);
+/* fast-mode vocoder convolution on the tensor cores (fp16 operands, fp32 accumulate), weights packed as the engine packs
+ * them.  up 0: Conv1d(Cin -> Cout, odd K, dilation dil, "same" padding), w [Cout][Cin][K]; up u in {2, 4, 8}:
+ * ConvTranspose1d(Cin -> Cout, kernel K = 2u, stride u, padding u/2), w [Cin][Cout][2u], dil 1, no resid, mode 0,
+ * scale16 1.  x [batch][Cin][L]: the already-activated input, rounded to fp16; item_len [batch] (0 <= L_i <= L) or NULL
+ * (all L).  Lout = L * u (up > 0) or L.  bias [Cout], cbias [batch][cbias_stride], resid [batch][Cout][Lout]: each
+ * optional.  Per item i and output step t < Lout_i:
+ *   y = conv(x_i) + bias + cbias_i + resid_i;  out32 = y (mode 0) or out32 + y (mode 1, needs out32);
+ *   out16 = fp16(lrelu(out32 value * scale16, slope_out))   (with mode 1: the activated sum)
+ * out32 [batch][Cout][Lout] fp32 and out16 [batch][Cout/8][lpad(Lout)][8] (the raw output atom image, uploaded as fp16 and
+ * returned as fp32, lpad(n) = 64 + ceil((n + 1) / 512) * 512 + 64, signal at rows 64 .. 64 + Lout_i) are in/out, NULL = not
+ * produced; rows the kernel does not write keep their contents.  max_ctas > 0 caps the persistent grid for this call
+ * (0: one CTA per SM).  Rejected before any launch: a geometry without a tensor-core plan, an even Conv1d K,
+ * (K-1)/2*dil > 64, batch outside 1..32, L_i > L. */
+int xtts_debug_conv_tc(xtts_engine* e, int32_t up, int32_t Cin, int32_t Cout, int32_t K, int32_t dil, int32_t batch, int32_t L,
+                       const int32_t* item_len, const float* w, const float* bias, const float* cbias, int32_t cbias_stride,
+                       const float* x, const float* resid, int32_t mode, float slope_out, float scale16, int32_t max_ctas,
+                       float* out32, float* out16);
 
 #ifdef __cplusplus
 }

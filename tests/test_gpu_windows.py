@@ -30,34 +30,49 @@ def _jobs(dims, n_seq, max_tokens, early=0, temperature=0.0, base=100):
                                                 ("engine_full_bf16", "dims_full", 605), ("engine_full", "dims_full", 60)])
 def test_window_interior_equals_whole_chunk(request, which, dims_name, T):
     """xtts_vocode_window: samples further than the receptive field (16 z-frames) from an inner window edge are the whole
-    chunk's, bit for bit (same arithmetic on the same inputs, in fp32 and in the fp16 tensor-core path); window edges that
-    coincide with the chunk's edges need no margin."""
+    chunk's, bit for bit (same arithmetic on the same inputs); window edges that coincide with the chunk's edges need no
+    margin.  engine_full_bf16 runs the fp16 tensor-core convs; the others run the fp32 convs (the small geometry has no
+    tensor-core plan, so engine_small_bf16 falls back to them)."""
     eng, dims = request.getfixturevalue(which), request.getfixturevalue(dims_name)
     hop, HZ = dims.voc.hop, 16
     lat = torch.randn(T, dims.voc.in_dim, generator=torch.Generator().manual_seed(77)).numpy()
-    full = eng.vocode(lat, 0)
-    Tz = dims.voc.z_frames(T)
-    assert full.shape[0] == Tz * hop
-    for z0, z1 in [(0, Tz // 2), (Tz // 3, Tz - 5), (Tz // 2, Tz), (0, Tz), (max(0, Tz - 40), Tz)]:
-        if z1 - z0 <= 2 * HZ:
-            continue
-        w = eng.vocode_window(lat, 0, z0, z1 - z0)
-        a = 0 if z0 == 0 else HZ
-        b = (z1 - z0) if z1 == Tz else (z1 - z0 - HZ)
-        np.testing.assert_array_equal(w[a * hop: b * hop], full[(z0 + a) * hop: (z0 + b) * hop])
+    eng.set_option("profile", 1)
+    try:
+        full = eng.vocode(lat, 0)
+        Tz = dims.voc.z_frames(T)
+        assert full.shape[0] == Tz * hop
+        for z0, z1 in [(0, Tz // 2), (Tz // 3, Tz - 5), (Tz // 2, Tz), (0, Tz), (max(0, Tz - 40), Tz)]:
+            if z1 - z0 <= 2 * HZ:
+                continue
+            w = eng.vocode_window(lat, 0, z0, z1 - z0)
+            a = 0 if z0 == 0 else HZ
+            b = (z1 - z0) if z1 == Tz else (z1 - z0 - HZ)
+            np.testing.assert_array_equal(w[a * hop: b * hop], full[(z0 + a) * hop: (z0 + b) * hop])
+        n_tc = eng.kernel_profile().get("conv1d_tc_f16_wgmma", {}).get("launches", 0)
+    finally:
+        eng.set_option("profile", 0)
+    assert (n_tc > 0) == (which == "engine_full_bf16"), n_tc
 
 
-@pytest.mark.parametrize("which", ["engine_small", "engine_small_bf16", "engine_small_fp16"])
-def test_ragged_batch_equals_single_chunks(request, dims_small, which):
+@pytest.mark.parametrize("which", ["engine_small", "engine_small_bf16", "engine_small_fp16", "engine_full_bf16"])
+def test_ragged_batch_equals_single_chunks(request, which):
     """chunks of different lengths finish at different steps and share vocoder launches (per-item lengths): tokens and
-    waveform of each equal what the same chunk gives alone; the waveform also equals xtts_vocode of its own latents."""
+    waveform of each equal what the same chunk gives alone; the waveform also equals xtts_vocode of its own latents.
+    engine_full_bf16 vocodes these ragged batches with the tensor-core convs."""
     eng = request.getfixturevalue(which)
+    dims = eng.dims
     lens = [5, 33, 12, 40, 7, 26, 40, 19]
-    jobs = _jobs(dims_small, len(lens), lens)
-    res = eng.run_batch(jobs, timeout_s=120, want_latents=True)
+    jobs = _jobs(dims, len(lens), lens)
+    eng.set_option("profile", 1)
+    try:
+        res = eng.run_batch(jobs, timeout_s=120, want_latents=True)
+        n_tc = eng.kernel_profile().get("conv1d_tc_f16_wgmma", {}).get("launches", 0)
+    finally:
+        eng.set_option("profile", 0)
+    assert (n_tc > 0) == (which == "engine_full_bf16"), n_tc
     for (sid, ids, spk, sp), n in zip(jobs, lens):
         r, toks, wav, lat = res[sid]
-        assert r.n_tokens == n and r.n_samples == dims_small.voc.n_samples(n) == wav.shape[0]
+        assert r.n_tokens == n and r.n_samples == dims.voc.n_samples(n) == wav.shape[0]
         alone = eng.run_batch([(sid, ids, spk, sp)], timeout_s=60)[sid]
         np.testing.assert_array_equal(toks, alone[1])
         np.testing.assert_array_equal(wav, alone[2])
