@@ -174,8 +174,10 @@ public:
                                  const xtts_sampling& sp, float* logits_out, float* latents_out, int32_t* sampled_out);
     void debug_gemm(int mode, const float* A, const float* W, const float* bias, const float* resid, float* out, int M,
                     int N, int K, int gelu, int iters, float* ms);
-    void debug_sample(const float* logits, const uint8_t* seen, int B, int V, const xtts_sampling& sp, int step,
-                      int32_t* out);
+    void debug_sample_slots(int V, int M, const int32_t* active, int n_slots, const float* logits, int ld,
+                            const xtts_sampling* sp, int cap, int advance_ctx, const int32_t* forced, int32_t* n_gen,
+                            int32_t* ctx_len, int32_t* finished, int32_t* last_tok, uint8_t* seen, int32_t* tokens,
+                            int32_t* sampled);
     void debug_attn_decode(int kv_type, int heads, int M, const int32_t* active, int n_slots, const int32_t* ctx_len,
                            const int32_t* block_tables, int max_pages, int n_pages, void* kpool, void* vpool,
                            const float* qkv, float* out);
@@ -2124,34 +2126,77 @@ void Engine::debug_gemm(int mode, const float* A, const float* W, const float* b
     cudaEventDestroy(e0); cudaEventDestroy(e1);
 }
 
-void Engine::debug_sample(const float* logits, const uint8_t* seen, int Bn, int Vn, const xtts_sampling& sp, int step,
-                          int32_t* out) {
+// One launch of the fused sampler (launch_sample) on private per-slot arrays: row r of logits samples for slot active[r]
+// with that slot's parameters, and every state array comes back as the kernel left it.  seen crosses as one byte per id
+// and is packed into ceil(V / 32) bitmap words per slot, as the engine keeps it.
+void Engine::debug_sample_slots(int Vn, int M, const int32_t* active, int n_slots, const float* logits, int ld,
+                                const xtts_sampling* sp, int cap, int advance_ctx, const int32_t* forced, int32_t* n_gen,
+                                int32_t* ctx_len, int32_t* finished, int32_t* last_tok, uint8_t* seen, int32_t* tokens,
+                                int32_t* sampled) {
     ApiLock lk(this);
     if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
-    if (Bn < 1 || Bn > B || Vn != V) throw std::runtime_error("debug_sample: bad batch or vocabulary size");
-    CUDA_CHECK(cudaSetDevice(cfg.device));
-    std::vector<float> lg((size_t)Bn * Vpad, 0.f);
-    for (int b = 0; b < Bn; ++b) std::memcpy(&lg[(size_t)b * Vpad], logits + (size_t)b * V, V * sizeof(float));
-    wLOG.upload(lg.data(), lg.size(), st);
-    std::vector<int> slots(Bn), ngen(Bn, step), zeros(Bn, 0), tk(Bn, sp.top_k), mt(Bn, CAP), stp(Bn, sp.stop_token), ss(Bn);
-    std::vector<float> T(Bn, sp.temperature), tp(Bn, sp.top_p), pen(Bn, sp.repetition_penalty);
-    std::vector<unsigned long long> seed(Bn, sp.seed);
-    std::vector<unsigned> sb((size_t)Bn * SEENW, 0u);
-    for (int b = 0; b < Bn; ++b) {
-        slots[b] = b; ss[b] = sp.seq_seed + b;
-        if (seen) for (int v = 0; v < V; ++v) if (seen[(size_t)b * V + v]) sb[(size_t)b * SEENW + (v >> 5)] |= 1u << (v & 31);
+    if (Vn < 1 || Vn > 2048) throw std::runtime_error("debug_sample_slots: V must be 1..2048");
+    if (n_slots < 1 || M < 1 || M > n_slots) throw std::runtime_error("debug_sample_slots: M must be 1..n_slots");
+    if (ld < Vn) throw std::runtime_error("debug_sample_slots: ld < V");
+    if (cap < 1) throw std::runtime_error("debug_sample_slots: cap must be >= 1");
+    if (!active || !logits || !sp || !n_gen || !ctx_len || !finished || !last_tok || !seen || !tokens || !sampled)
+        throw std::runtime_error("debug_sample_slots: only forced may be NULL");
+    std::vector<char> used(n_slots, 0);
+    for (int i = 0; i < M; ++i) {
+        const int s = active[i];
+        if (s < 0 || s >= n_slots || used[s]) throw std::runtime_error("debug_sample_slots: active slots must be distinct and < n_slots");
+        used[s] = 1;
+        // the kernel reads forced[slot][n_gen] without a bound check and sets the forced id's seen bit
+        if (n_gen[s] < 0) throw std::runtime_error("debug_sample_slots: n_gen must be >= 0");
+        if (forced && n_gen[s] >= cap) throw std::runtime_error("debug_sample_slots: with forced, n_gen must be < cap");
+        if (forced && forced[(size_t)s * cap + n_gen[s]] >= Vn) throw std::runtime_error("debug_sample_slots: forced id >= V");
     }
-    d_active.upload(slots.data(), Bn, st); d_n_gen.upload(ngen.data(), Bn, st); d_finished.upload(zeros.data(), Bn, st);
-    d_top_k.upload(tk.data(), Bn, st); d_max_tokens.upload(mt.data(), Bn, st); d_stop.upload(stp.data(), Bn, st);
-    d_seq_seed.upload(ss.data(), Bn, st); d_temp.upload(T.data(), Bn, st); d_top_p.upload(tp.data(), Bn, st);
-    d_pen.upload(pen.data(), Bn, st); d_seed.upload(seed.data(), Bn, st); d_seen.upload(sb.data(), sb.size(), st);
-    launch_sample(wLOG.p, Vpad, d_active.p, Bn, V, sample_state(), 0, st);
-    std::vector<int> res(Bn);
-    d_last_tok.download(res.data(), Bn, st);
+    CUDA_CHECK(cudaSetDevice(cfg.device));
+    const int sw = (Vn + 31) / 32;
+    const size_t nt = (size_t)n_slots * cap;
+    std::vector<unsigned> sb((size_t)n_slots * sw, 0u);
+    for (int s = 0; s < n_slots; ++s)
+        for (int v = 0; v < Vn; ++v)
+            if (seen[(size_t)s * Vn + v]) sb[(size_t)s * sw + (v >> 5)] |= 1u << (v & 31);
+    std::vector<float> T(n_slots), tp(n_slots), pen(n_slots);
+    std::vector<int> tk(n_slots), mt(n_slots), stp(n_slots), ss(n_slots);
+    std::vector<unsigned long long> seed(n_slots);
+    for (int s = 0; s < n_slots; ++s) {
+        T[s] = sp[s].temperature; tp[s] = sp[s].top_p; pen[s] = sp[s].repetition_penalty; tk[s] = sp[s].top_k;
+        mt[s] = sp[s].max_tokens; stp[s] = sp[s].stop_token; ss[s] = sp[s].seq_seed; seed[s] = sp[s].seed;
+    }
+    DBuf<float> dlg, dT, dtp, dpen;
+    DBuf<int> dact, dng, dctx, dfin, dlast, dtok, dsmp, dfor, dtk, dmt, dstp, dss;
+    DBuf<unsigned> dseen;
+    DBuf<unsigned long long> dseed;
+    dlg.alloc((size_t)M * ld); dact.alloc(M);
+    for (auto* b : {&dng, &dctx, &dfin, &dlast, &dtk, &dmt, &dstp, &dss}) b->alloc(n_slots);
+    for (auto* b : {&dT, &dtp, &dpen}) b->alloc(n_slots);
+    dtok.alloc(nt); dsmp.alloc(nt); dseen.alloc(sb.size()); dseed.alloc(n_slots);
+    dlg.upload(logits, (size_t)M * ld, st); dact.upload(active, M, st);
+    dng.upload(n_gen, n_slots, st); dctx.upload(ctx_len, n_slots, st); dfin.upload(finished, n_slots, st);
+    dlast.upload(last_tok, n_slots, st); dtok.upload(tokens, nt, st); dsmp.upload(sampled, nt, st);
+    dseen.upload(sb.data(), sb.size(), st);
+    dT.upload(T.data(), n_slots, st); dtp.upload(tp.data(), n_slots, st); dpen.upload(pen.data(), n_slots, st);
+    dtk.upload(tk.data(), n_slots, st); dmt.upload(mt.data(), n_slots, st); dstp.upload(stp.data(), n_slots, st);
+    dss.upload(ss.data(), n_slots, st); dseed.upload(seed.data(), n_slots, st);
+    if (forced) { dfor.alloc(nt); dfor.upload(forced, nt, st); }
+    SampleState S;
+    S.last_tok = dlast.p; S.n_gen = dng.p; S.ctx_len = dctx.p; S.finished = dfin.p;
+    S.tokens = dtok.p; S.sampled = dsmp.p; S.forced = forced ? dfor.p : nullptr;
+    S.seen = dseen.p; S.temperature = dT.p; S.top_p = dtp.p; S.top_k = dtk.p; S.penalty = dpen.p;
+    S.max_tokens = dmt.p; S.stop_token = dstp.p; S.seed = dseed.p; S.seq_seed = dss.p;
+    S.tokens_cap = cap; S.seen_words = sw;
+    launch_sample(dlg.p, ld, dact.p, M, Vn, S, advance_ctx, st);
+    dng.download(n_gen, n_slots, st); dctx.download(ctx_len, n_slots, st); dfin.download(finished, n_slots, st);
+    dlast.download(last_tok, n_slots, st); dtok.download(tokens, nt, st); dsmp.download(sampled, nt, st);
+    dseen.download(sb.data(), sb.size(), st);
     CUDA_CHECK(cudaStreamSynchronize(st));
-    for (int b = 0; b < Bn; ++b) out[b] = res[b];
-    d_n_gen.upload(zeros.data(), Bn, st); d_finished.upload(zeros.data(), Bn, st);
-    CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int s = 0; s < n_slots; ++s) {
+        for (int v = 0; v < Vn; ++v) seen[(size_t)s * Vn + v] = (uint8_t)((sb[(size_t)s * sw + (v >> 5)] >> (v & 31)) & 1u);
+        if (Vn % 32 && (sb[(size_t)s * sw + sw - 1] >> (Vn % 32)))
+            throw std::runtime_error("debug_sample_slots: the kernel set a seen bit at an id >= V");
+    }
 }
 
 // 16-bit device values -> fp32 on the host (exact)
@@ -2474,9 +2519,12 @@ int xtts_debug_gemm(xtts_engine* e, int32_t mode, const float* A, const float* W
                     float* out, int32_t M, int32_t N, int32_t K, int32_t gelu, int32_t iters, float* ms_per_iter) {
     XTTS_TRY(e->impl->debug_gemm(mode, A, W, bias, resid, out, M, N, K, gelu, iters, ms_per_iter))
 }
-int xtts_debug_sample(xtts_engine* e, const float* logits, const uint8_t* seen, int32_t B, int32_t V,
-                      const xtts_sampling* sp, int32_t step, int32_t* out_tokens) {
-    XTTS_TRY(e->impl->debug_sample(logits, seen, B, V, *sp, step, out_tokens))
+int xtts_debug_sample_slots(xtts_engine* e, int32_t V, int32_t M, const int32_t* active, int32_t n_slots, const float* logits,
+                            int32_t ld, const xtts_sampling* sp, int32_t cap, int32_t advance_ctx, const int32_t* forced,
+                            int32_t* n_gen, int32_t* ctx_len, int32_t* finished, int32_t* last_tok, uint8_t* seen,
+                            int32_t* tokens, int32_t* sampled) {
+    XTTS_TRY(e->impl->debug_sample_slots(V, M, active, n_slots, logits, ld, sp, cap, advance_ctx, forced, n_gen, ctx_len,
+                                         finished, last_tok, seen, tokens, sampled))
 }
 int xtts_debug_attn_decode(xtts_engine* e, int32_t kv_type, int32_t heads, int32_t M, const int32_t* active, int32_t n_slots,
                            const int32_t* ctx_len, const int32_t* block_tables, int32_t max_pages, int32_t n_pages,

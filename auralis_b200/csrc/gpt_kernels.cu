@@ -846,7 +846,12 @@ sample_kernel(const float* __restrict__ logits, int ld, const int* __restrict__ 
         __shared__ float cv[128];
         __shared__ short ci[128];
         __shared__ float cum[128];
-        auto fkey = [](float x) { unsigned b = __float_as_uint(x); return (b & 0x80000000u) ? ~b : (b | 0x80000000u); };
+        // order-preserving key; -0.0 maps to +0.0's key, since the full sort's float compare treats the two as equal
+        auto fkey = [](float x) {
+            unsigned b = __float_as_uint(x);
+            if (b == 0x80000000u) b = 0u;
+            return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+        };
         if (tid == 0) { sel_prefix = 0u; sel_k = (unsigned)tk_fast; ncand = 0u; }
         for (int pass = 3; pass >= 0; --pass) {
             hist[tid] = 0u;

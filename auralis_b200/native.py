@@ -76,7 +76,7 @@ ABI_SYMBOLS = [
     "xtts_last_error", "xtts_version", "xtts_create", "xtts_destroy", "xtts_load_weight", "xtts_finalize_weights",
     "xtts_set_speaker", "xtts_get_speaker", "xtts_condition", "xtts_submit", "xtts_cancel", "xtts_poll", "xtts_fetch",
     "xtts_set_option", "xtts_get_stats", "xtts_sync", "xtts_get_kernel_profile", "xtts_device_timer", "xtts_vocode", "xtts_vocode_window", "xtts_gpt_prefill", "xtts_gpt_teacher_forced",
-    "xtts_debug_gemm", "xtts_debug_sample", "xtts_debug_trace",
+    "xtts_debug_gemm", "xtts_debug_sample_slots", "xtts_debug_trace",
     "xtts_debug_attn_decode", "xtts_debug_attn_prefill", "xtts_debug_splitk_ln", "xtts_debug_conv_tc",
 ]
 
@@ -116,7 +116,8 @@ def load_library(path: Optional[str] = None):
     lib.xtts_gpt_prefill.argtypes = [vp, i32p, i32, i32, i32p, i32, f32p, f32p, f32p]
     lib.xtts_gpt_teacher_forced.argtypes = [vp, i32p, i32, i32, i32p, i32, C.POINTER(XttsSampling), f32p, f32p, i32p]
     lib.xtts_debug_gemm.argtypes = [vp, i32, f32p, f32p, f32p, f32p, f32p, i32, i32, i32, i32, i32, f32p]
-    lib.xtts_debug_sample.argtypes = [vp, f32p, C.POINTER(C.c_uint8), i32, i32, C.POINTER(XttsSampling), i32, i32p]
+    lib.xtts_debug_sample_slots.argtypes = [vp, i32, i32, i32p, i32, f32p, i32, C.POINTER(XttsSampling), i32, i32, i32p,
+                                            i32p, i32p, i32p, i32p, C.POINTER(C.c_uint8), i32p, i32p]
     lib.xtts_debug_trace.argtypes = [vp, i32, C.POINTER(C.c_uint64), i32]
     lib.xtts_debug_attn_decode.argtypes = [vp, i32, i32, i32, i32p, i32, i32p, i32p, i32, i32, vp, vp, f32p, f32p]
     lib.xtts_debug_attn_prefill.argtypes = [vp, i32, i32, i32p, i32, i32, C.c_float, f32p, i64, i32, i32, f32p, i64, i32, i32,
@@ -430,14 +431,45 @@ class NativeEngine:
         return out, ms.value
 
     def debug_sample(self, logits, seen, sp: Sampling, step: int = 0):
+        """Row b of logits [B, V] sampled as slot b with sp and seq_seed sp.seq_seed + b at step `step`; seen [B, V] (0/1)
+        or None.  -> the drawn tokens [B]."""
         lg = _f32(logits)
         Bn, V = lg.shape
-        sn = np.ascontiguousarray(np.asarray(seen, dtype=np.uint8)) if seen is not None else None
-        out = np.empty((Bn,), np.int32)
-        cs = sp.c()
-        self._chk(self.lib.xtts_debug_sample(self.h, _fp(lg), sn.ctypes.data_as(C.POINTER(C.c_uint8)) if sn is not None else None,
-                                             Bn, V, C.byref(cs), step, _ip(out)), "debug_sample")
-        return out
+        sps = [Sampling(**{**sp.__dict__, "seq_seed": sp.seq_seed + b}) for b in range(Bn)]
+        st = self.debug_sample_slots(V, lg, np.arange(Bn), sps, n_gen=np.full(Bn, step), cap=step + 1,
+                                     seen=np.zeros((Bn, V), np.uint8) if seen is None else seen)
+        return st["last_tok"]
+
+    SAMPLE_STATE = ("n_gen", "ctx_len", "finished", "last_tok", "seen", "tokens", "sampled")
+
+    def debug_sample_slots(self, V: int, logits, active, sps, n_gen=None, ctx_len=None, finished=None, last_tok=None,
+                           seen=None, tokens=None, sampled=None, cap: Optional[int] = None, advance_ctx: int = 0,
+                           forced=None):
+        """One launch of the fused sampler (include/xtts_b200.h).  logits [M, ld]; active [M]; sps: one Sampling per slot.
+        State arrays default to zeros (tokens / sampled to -1, with `cap` columns); n_slots = len(sps).
+        -> {name: array after the launch} for every name in SAMPLE_STATE."""
+        lg, act = _f32(logits), _i32(active)
+        n = len(sps)
+        if cap is None:
+            cap = tokens.shape[1] if tokens is not None else 1
+        z = lambda a, fill=0: _i32(a).copy() if a is not None else np.full(n, fill, np.int32)
+        st = dict(n_gen=z(n_gen), ctx_len=z(ctx_len), finished=z(finished), last_tok=z(last_tok, -1))
+        st["seen"] = (np.ascontiguousarray(seen, dtype=np.uint8).copy() if seen is not None
+                      else np.zeros((n, V), np.uint8))
+        for k, a in (("tokens", tokens), ("sampled", sampled)):
+            st[k] = _i32(a).copy() if a is not None else np.full((n, max(cap, 0)), -1, np.int32)
+        f = _i32(forced) if forced is not None else None
+        for k, a in [("seen", st["seen"]), ("tokens", st["tokens"]), ("sampled", st["sampled"]), ("forced", f)]:
+            if a is not None and a.size != n * (V if k == "seen" else max(cap, 0)):
+                raise ValueError(f"{k} has {a.size} elements for {n} slots")
+        cs = (XttsSampling * max(n, 1))(*[s.c() for s in sps])
+        M = act.size
+        ld = lg.shape[1] if lg.ndim == 2 else V
+        self._chk(self.lib.xtts_debug_sample_slots(self.h, V, M, _ip(act), n, _fp(lg), ld, cs, cap, advance_ctx, _ip(f),
+                                                   _ip(st["n_gen"]), _ip(st["ctx_len"]), _ip(st["finished"]),
+                                                   _ip(st["last_tok"]), st["seen"].ctypes.data_as(C.POINTER(C.c_uint8)),
+                                                   _ip(st["tokens"]), _ip(st["sampled"])), "debug_sample_slots")
+        return st
 
     # KV type code of xtts_debug_attn_decode -> numpy dtype of the raw pool elements (bf16 as its uint16 bit pattern)
     KV_DTYPES = {0: np.float32, 1: np.uint16, 2: np.float16}

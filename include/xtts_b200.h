@@ -200,11 +200,20 @@ int xtts_debug_gemm(xtts_engine* e, int32_t mode, const float* A, const float* W
  * resolved, exit), op 0 disarms and copies up to `cap` records [n][2] u64 = (ns, id<<32 | grid<<40 | last<<8 | phase) into
  * `out`; returns the count (>= 0) or a negative error.  Nothing is serialised: shows the step as it really runs. */
 int xtts_debug_trace(xtts_engine* e, int32_t op, uint64_t* out, int32_t cap);
-/* sampler under test: logits [B,V]; seen [B,V] (0/1) ; out tokens [B] */
-int xtts_debug_sample(xtts_engine* e, const float* logits, const uint8_t* seen, int32_t B, int32_t V,
-                      const xtts_sampling* sp, int32_t step, int32_t* out_tokens);
 /* Single-kernel entry points below: an idle engine, private device buffers, the engine's current kernel options
  * (xtts_set_option), no engine state touched. */
+/* fused sampler (one launch): row r of logits [M][ld] samples for slot active[r] (M distinct slots < n_slots) over ids
+ * 0 .. V-1 (1 <= V <= 2048, ld >= V) with the slot's parameters sp[slot] (temperature, top_p, repetition_penalty, top_k,
+ * max_tokens, stop_token, seed, seq_seed; the other fields are ignored).  Per-slot state, in/out, as the kernel leaves
+ * it for active and inactive slots alike: n_gen, ctx_len, finished, last_tok [n_slots]; seen [n_slots][V] (0/1, the
+ * penalty set); tokens, sampled [n_slots][cap].  forced [n_slots][cap] or NULL: an entry >= 0 at [slot][n_gen] replaces
+ * the drawn id in tokens / last_tok / seen.  advance_ctx 1 adds one to ctx_len of every active slot.  Rejected before
+ * any launch: V, M, ld or cap out of range, duplicate or out-of-range active slots, a negative n_gen, NULL (except
+ * forced), and with forced an n_gen >= cap or a forced id >= V. */
+int xtts_debug_sample_slots(xtts_engine* e, int32_t V, int32_t M, const int32_t* active, int32_t n_slots, const float* logits,
+                            int32_t ld, const xtts_sampling* sp, int32_t cap, int32_t advance_ctx, const int32_t* forced,
+                            int32_t* n_gen, int32_t* ctx_len, int32_t* finished, int32_t* last_tok, uint8_t* seen,
+                            int32_t* tokens, int32_t* sampled);
 /* paged decode attention (one launch, appends each row's k / v): kv_type 0 fp32, 1 bf16, 2 fp16 (the output has the cache
  * type, returned as fp32).  active [M] (distinct slots < n_slots), ctx_len [n_slots], block_tables [n_slots][max_pages];
  * kpool / vpool: n_pages pages of raw cache-typed elements in the device layout (K [page][head][64/X][32 tok][X], X = 16 bytes

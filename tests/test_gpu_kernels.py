@@ -5,6 +5,7 @@ import torch
 
 from auralis_b200.native import Sampling
 from oracle import xtts_oracle as O
+from test_gpu_sampler import reference
 
 pytestmark = pytest.mark.gpu
 
@@ -115,6 +116,12 @@ def _oracle_tokens(logits, seen, sp, step):
     return np.array(out)
 
 
+def _exact_tokens(logits, seen, sp, step):
+    B = logits.shape[0]
+    return reference(logits, seen, [sp.temperature] * B, [sp.top_k] * B, [sp.top_p] * B, [sp.repetition_penalty] * B,
+                     [sp.seed] * B, sp.seq_seed + np.arange(B), [step] * B)
+
+
 def test_sampler_greedy_with_penalty(engine_small, dims_small):
     V = dims_small.gpt.n_audio_tokens
     rng = np.random.RandomState(3)
@@ -127,11 +134,12 @@ def test_sampler_greedy_with_penalty(engine_small, dims_small):
 
 @pytest.mark.parametrize("top_k,quantised", [(50, False), (0, False), (100, False), (50, True)])
 def test_sampler_topk_topp_seeded(engine_small, dims_small, top_k, quantised):
-    """Same Philox stream, same kept set -> same token (a few near-ties may flip on exp/log ulps).
+    """Same Philox stream, same kept set -> the same token as the exact reference on every decisive row (one whose
+    top-p compares and winning ratio clear the kernel's fp32 error bound, tests/test_gpu_sampler.py).
     top_k=50 takes the radix-select fast path; 0 / 100 and the heavily tied (quantised) logits take the full sort."""
     V = dims_small.gpt.n_audio_tokens
     rng = np.random.RandomState(5)
-    agree = total = 0
+    decisive = total = 0
     for step in range(6):
         logits = (rng.randn(8, V) * 2.0).astype(np.float32)
         if quantised:
@@ -140,9 +148,12 @@ def test_sampler_topk_topp_seeded(engine_small, dims_small, top_k, quantised):
         sp = Sampling(temperature=0.75, top_p=0.85, top_k=top_k, repetition_penalty=5.0, seed=1234 + step, seq_seed=7,
                       stop_token=dims_small.gpt.stop_audio_token)
         got = engine_small.debug_sample(logits, seen, sp, step=step)
-        exp = _oracle_tokens(logits, seen, sp, step)
-        agree += int((got == exp).sum()); total += got.size
-    assert agree >= total - 1, (agree, total)
+        ref = _exact_tokens(logits, seen, sp, step)
+        d = ref.decisive
+        np.testing.assert_array_equal(got[d], ref.token[d])
+        np.testing.assert_array_equal(ref.token[d], _oracle_tokens(logits, seen, sp, step)[d])
+        decisive += int(d.sum()); total += got.size
+    assert decisive >= 0.9 * total, (decisive, total)
 
 
 def test_sampler_distribution(engine_small, dims_small):
