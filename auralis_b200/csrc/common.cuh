@@ -92,6 +92,7 @@ struct KernelCtx {
     KernelProfiler prof;
     bool use_pdl = true;
     int voc_sm_cap = 0;           // > 0: persistent tensor-core conv grids take at most this many SMs (set per vocoder batch)
+    int conv_tc_epilogue = 1;     // tensor-core Conv1d epilogue: 1 staged through shared memory + bulk copies, 0 direct
     int attn_ctas_per_sm = 0;     // 0 = uncapped decode-attention grid; > 0: at most this many CTAs per SM
     int gemm_decode_bn = 0;       // 0 = heuristic; 32/64/128 forces the tile width of decode-shaped tensor-core GEMMs
     int attn_warps = 4;           // warps per (row, head) item of the bf16 decode attention (4, or 8: measured slower, run 7)
@@ -106,6 +107,7 @@ struct KernelCtx {
 #define g_prof (::xtts::kctx().prof)
 #define g_use_pdl (::xtts::kctx().use_pdl)
 #define g_voc_sm_cap (::xtts::kctx().voc_sm_cap)
+#define g_conv_tc_epilogue (::xtts::kctx().conv_tc_epilogue)
 #define g_attn_ctas_per_sm (::xtts::kctx().attn_ctas_per_sm)
 #define g_gemm_decode_bn (::xtts::kctx().gemm_decode_bn)
 #define g_gemm_wide (::xtts::kctx().gemm_wide)

@@ -49,14 +49,37 @@ struct ConvTcParams {
     int cbias_bs;   // elements between the speaker-bias vectors of consecutive batch items
     int tile_rows, tiles_n, batch; // persistent-CTA tile space: per item ceil(rows_i / tile_rows) x tiles_n tiles
     int item_L[kVocMaxItems];      // ragged batch: input time steps of each item (<= L; buffers are strided by L)
+    int epi_nf;                    // staged epilogue: fp32 buffers per slab (0, 1, or 2 = residual + accumulate base)
+    uint32_t epi_off, epi_slab;    // staged epilogue: byte offset of the slab ring in dynamic shared memory, bytes per slab
 };
 
-// N output channels (GEMM columns) per tile, MB 64-row blocks per consumer warpgroup (tile_rows = 128 * MB)
-template <int N, int MB>
-__global__ void __launch_bounds__(kThreadsTc, 1)
+// Staged epilogue (Conv1d only): the tile's GEMM columns are processed in slabs of EpiSlab<N>::SN columns x tile_rows
+// rows, through a ring of kES slabs behind the A/B rings.  Per slab:
+//   fp32 [SN][tile_rows + 4]       residual (or the accumulate base), prefetched by the loader warp; y is written over it
+//   fp32 [SN][tile_rows + 4]       accumulate base, when the conv has both a residual and an accumulated out32
+//   fp16 [SN/8][tile_rows][8]      lrelu(y * scale16) as output atoms
+// then bulk shared->global copies drain it while the consumers go on.  The +4-float row pad makes the epilogue's
+// (8 rows x 4 column pairs) per-warp access conflict-free and keeps every row 16-byte aligned.  SN is the widest that
+// fits two slabs (with both fp32 buffers) beside the worst-case A/B rings (K = 11, dil = 5) of each instantiation:
+//   N = 256 (128 rows, CK 64): A/B 144000 B + 2 x 41984 B = 227968 B    (limit kMaxDynTc = 228352 B)
+//   N = 128 (256 rows, CK 64): A/B 127616 B + 2 x 41472 B = 210560 B
+//   N =  64 (512 rows, CK 64): A/B 168576 B + 2 x 41216 B = 251008 B    over: only with a single fp32 buffer (2 x 24704)
+//   N =  32 (512 rows, CK 32): A/B  78208 B + 2 x 41216 B = 160640 B
+// launch_tc_common computes the exact figure per launch and keeps the direct epilogue where it does not fit.
+constexpr int kES = 2;
+template <int N> struct EpiSlab { static constexpr int SN = N >= 256 ? 32 : (N >= 128 ? 16 : 8); };
+constexpr int kEpiRowPad = 4;
+inline size_t epi_slab_bytes(int SN, int tile_rows, int nf) {
+    return ((size_t)nf * SN * (tile_rows + kEpiRowPad) * 4 + (size_t)(SN / 8) * tile_rows * 16 + 127) & ~(size_t)127;
+}
+
+// N output channels (GEMM columns) per tile, MB 64-row blocks per consumer warpgroup (tile_rows = 128 * MB).
+// STAGED: one more warp (the epilogue loader) and the staged epilogue above; otherwise the direct epilogue.
+template <int N, int MB, bool STAGED>
+__global__ void __launch_bounds__(kThreadsTc + (STAGED ? 32 : 0), 1)
 conv1d_tc_kernel(const ConvTcParams P) {
     extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ __align__(8) uint64_t a_full[SA], a_empty[SA], b_full[SB], b_empty[SB];
+    __shared__ __align__(8) uint64_t a_full[SA], a_empty[SA], b_full[SB], b_empty[SB], e_full[kES], e_empty[kES];
     __shared__ __align__(16) float sbias[2][N];     // per-tile bias + speaker bias (double buffered across tiles)
     __shared__ int s_cum[kVocMaxItems + 1], s_len[kVocMaxItems];   // ragged batch: first tile / input length of every item
 
@@ -83,6 +106,7 @@ conv1d_tc_kernel(const ConvTcParams P) {
         s_cum[P.batch] = c;
         for (int i = 0; i < SA; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], kConsumerWarps); }
         for (int i = 0; i < SB; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], kConsumerWarps); }
+        for (int i = 0; i < kES; ++i) { mbar_init(&e_full[i], 1); mbar_init(&e_empty[i], 1); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -126,6 +150,39 @@ conv1d_tc_kernel(const ConvTcParams P) {
                 }
             }
         }
+    } else if (STAGED && warp == kConsumerWarps + 1) {
+        // ------------------------------------------------ epilogue loader: residual / accumulate-base rows of every slab.
+        // Runs ahead of the consumers by the ring depth, so a tile's first slabs land while its MMAs are still running.
+        // Every slab is announced on e_full (with 0 bytes when it has no input): that is also the consumers' "slot free".
+        constexpr int SN = EpiSlab<N>::SN, TR = 128 * MB, LDR = TR + kEpiRowPad;
+        const bool accum32 = P.mode == CONV_ACCUM && P.out32 != nullptr;
+        const float* in0 = P.resid ? P.resid : (accum32 ? P.out32 : nullptr);
+        const float* in1 = (P.resid && accum32) ? P.out32 : nullptr;
+        const uint32_t nin = (in0 ? 1u : 0u) + (in1 ? 1u : 0u);
+        const size_t Ls = (size_t)P.Lout;
+        int ie = 0;
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+            int zi, tx, ty, Li;
+            decode_tile(tile, zi, tx, ty, Li);
+            const int T0 = tx * P.tile_rows, n0 = ty * N;
+            const int nr = min(TR, Li - T0);
+            const uint32_t rb = (uint32_t)((nr + 3) & ~3) * 4u;     // whole 16-byte units: Lout % 4 == 0 keeps this inside the row
+            const size_t item = (size_t)zi * P.Cr * Ls;
+            for (int g = 0; g < N / SN; ++g, ++ie) {
+                const int slot = ie % kES;
+                float* f = reinterpret_cast<float*>(smem + P.epi_off + (size_t)slot * P.epi_slab);
+                if (lane == 0) {
+                    mbar_wait(&e_empty[slot], ((ie / kES) & 1) ^ 1);
+                    mbar_expect_tx(&e_full[slot], nin * SN * rb);
+                }
+                __syncwarp();
+                if (lane < SN) {
+                    const size_t go = item + (size_t)(n0 + g * SN + lane) * Ls + T0;
+                    if (in0) bulk_g2s(f + lane * LDR, in0 + go, rb, &e_full[slot]);
+                    if (in1) bulk_g2s(f + (SN + lane) * LDR, in1 + go, rb, &e_full[slot]);
+                }
+            }
+        }
     } else {
         // ------------------------------------------------ consumer warpgroup wg: time rows [T0 + 64*MB*wg, +64*MB) of a tile.
         // Weight slots are handed back one tap late (after the next tap's wgmmas are issued), so the tensor cores never
@@ -133,7 +190,7 @@ conv1d_tc_kernel(const ConvTcParams P) {
         const int wg = warp >> 2, etid = threadIdx.x;
         const bool has_res = P.resid != nullptr, accum = (P.mode == CONV_ACCUM);
         const size_t Ls = (size_t)P.Lout;
-        int ita = 0, itb = 0, lt = 0;
+        int ita = 0, itb = 0, lt = 0, ie = 0;
         float acc[MB][N / 2];
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
             int zi, tx, ty, Li;
@@ -193,6 +250,65 @@ conv1d_tc_kernel(const ConvTcParams P) {
             release();
             asm volatile("bar.sync 1, %0;" ::"r"(kConsumers) : "memory");      // bias table visible to every consumer warp
 
+            if constexpr (STAGED) {
+                // ---- staged epilogue, slab by slab; same arithmetic, in the same order, as the direct epilogue below
+                constexpr int SN = EpiSlab<N>::SN, TR = 128 * MB, LDR = TR + kEpiRowPad;
+                const int nr = min(TR, Li - T0), nr4 = nr & ~3;      // rows of this item in the tile; bulk-copied part of them
+                float* out32 = P.out32 ? P.out32 + zo * P.Cr * Ls : nullptr;
+                __half* out16 = P.out16 ? P.out16 + zo * (size_t)(P.Cr / 8) * P.lpad_out * 8 : nullptr;
+                const int r_base = 64 * MB * wg + 16 * (warp & 3) + (lane >> 2);
+#pragma unroll
+                for (int g = 0; g < N / SN; ++g, ++ie) {
+                    const int slot = ie % kES;
+                    uint8_t* sl = smem + P.epi_off + (size_t)slot * P.epi_slab;
+                    float* f0 = reinterpret_cast<float*>(sl);
+                    const float* fb = has_res ? f0 + SN * LDR : f0;         // accumulate base: second buffer behind a residual
+                    uint8_t* h16 = sl + (size_t)P.epi_nf * SN * LDR * 4;
+                    mbar_wait(&e_full[slot], (ie / kES) & 1);
+#pragma unroll
+                    for (int ii = 0; ii < SN / 8; ++ii) {
+                        const int i = g * (SN / 8) + ii, c = 8 * ii + 2 * (lane & 3);   // accumulator group, slab column
+#pragma unroll
+                        for (int m = 0; m < MB; ++m)
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) {
+                                const int r = r_base + 64 * m + 8 * h;
+                                float y[2];
+#pragma unroll
+                                for (int e = 0; e < 2; ++e) {
+                                    y[e] = acc[m][4 * i + 2 * h + e] + sb[g * SN + c + e];
+                                    const int o = (c + e) * LDR + r;
+                                    if (has_res) y[e] += f0[o];
+                                    if (out32) {
+                                        if (accum) y[e] += fb[o];
+                                        f0[o] = y[e];
+                                        if (r >= nr4 && r < nr) out32[(size_t)(n0 + g * SN + c + e) * Ls + T0 + r] = y[e];   // row tail
+                                    }
+                                }
+                                if (out16)
+                                    *reinterpret_cast<__half2*>(h16 + ((size_t)ii * TR + r) * 16 + 4 * (lane & 3)) =
+                                        __floats2half2_rn(lrelu_s(y[0] * P.scale16, P.slope_out), lrelu_s(y[1] * P.scale16, P.slope_out));
+                            }
+                    }
+                    fence_proxy_async_smem();
+                    asm volatile("bar.sync 1, %0;" ::"r"(kConsumers) : "memory");
+                    if (warp == 0) {
+                        // lane l: fp32 row of slab column l, and (l < SN/8) atom plane l; then the slot goes back to the
+                        // loader as soon as these copies have read it
+                        if (lane < SN && out32 && nr4 > 0)
+                            bulk_s2g(out32 + (size_t)(n0 + g * SN + lane) * Ls + T0, f0 + lane * LDR, (uint32_t)nr4 * 4u);
+                        if (lane < SN / 8 && out16)
+                            bulk_s2g(out16 + ((size_t)((n0 + g * SN) / 8 + lane) * P.lpad_out + T0 + kAtomPadL) * 8,
+                                     h16 + (size_t)lane * TR * 16, (uint32_t)nr * 16u);
+                        bulk_commit();
+                        bulk_wait_read<0>();
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(&e_empty[slot]);
+                    }
+                }
+                continue;
+            }
+
             // ---- epilogue: a lane holds GEMM columns (col, col+1) of time rows s and s + 8 of each 64-row block
             float* out32 = P.out32 ? P.out32 + zo * P.Cr * P.Lout : nullptr;
             const float* resid = has_res ? P.resid + zo * P.Cr * P.Lout : nullptr;
@@ -239,6 +355,7 @@ conv1d_tc_kernel(const ConvTcParams P) {
                     }
                 }
         }
+        if (STAGED && warp == 0) bulk_wait_all<0>();         // the last slabs' global writes have landed
     }
     __syncthreads();
     trace_pt(TR_CONV, 2);
@@ -302,11 +419,33 @@ void conv1d_tc_pack(const float* w, int Cin, int Cout, int K, const ConvTcPlan& 
 int atoms_lpad(int L) { return kAtomPadL + ceil_div(L + 1, 512) * 512 + kAtomPadR; }
 
 constexpr int kMaxDynTc = 227 * 1024 - 4096;      // opt-in limit minus the kernel's static shared memory
-template <int N, int MB>
+template <int N, int MB, bool STAGED>
 static void launch_inst(const ConvTcParams& P, dim3 grid, size_t smem, cudaStream_t st) {
     static bool attr[64] = {};
-    if (first_on_device(attr)) CUDA_CHECK(cudaFuncSetAttribute(conv1d_tc_kernel<N, MB>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynTc));
-    conv1d_tc_kernel<N, MB><<<grid, kThreadsTc, smem, st>>>(P);
+    if (first_on_device(attr))
+        CUDA_CHECK(cudaFuncSetAttribute(conv1d_tc_kernel<N, MB, STAGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynTc));
+    conv1d_tc_kernel<N, MB, STAGED><<<grid, kThreadsTc + (STAGED ? 32 : 0), smem, st>>>(P);
+}
+template <int N, int MB>
+static void launch_inst(const ConvTcParams& P, bool staged, dim3 grid, size_t smem, cudaStream_t st) {
+    if (staged) launch_inst<N, MB, true>(P, grid, smem, st);
+    else launch_inst<N, MB, false>(P, grid, smem, st);
+}
+
+// Shared memory of a launch: the A/B rings and, for the staged epilogue, its slab ring behind them (0 when the staged
+// epilogue cannot be used: a transposed conv, or the slabs do not fit).  nf: fp32 buffers per slab.
+ConvTcSmem conv1d_tc_smem(const ConvTcPlan& pl, int K, int dil, int up, int nf) {
+    ConvTcSmem s{};
+    const int tile = 128 * pl.nacc;
+    const size_t a_stage = (size_t)(tile + (K - 1) * dil) * 16 * (pl.CK / 8), b_stage = (size_t)pl.N * 16 * (pl.CK / 8);
+    const size_t ab = ((SA * a_stage + 127) & ~(size_t)127) + SB * b_stage;
+    s.direct = ab + 128;
+    s.slab_cols = pl.N >= 256 ? EpiSlab<256>::SN : (pl.N >= 128 ? EpiSlab<128>::SN : EpiSlab<64>::SN);
+    s.slab_bytes = epi_slab_bytes(s.slab_cols, tile, nf);
+    s.epi_off = (ab + 127) & ~(size_t)127;
+    const size_t staged = s.epi_off + kES * s.slab_bytes + 128;
+    s.staged = (up == 0 && staged <= (size_t)kMaxDynTc) ? staged : 0;
+    return s;
 }
 
 static void launch_tc_common(ConvTcParams& P, const ConvTcPlan& pl, int rows_to_cover, int batch, const int* item_len,
@@ -316,9 +455,16 @@ static void launch_tc_common(ConvTcParams& P, const ConvTcPlan& pl, int rows_to_
     P.rows = tile + (P.K - 1) * P.dil;
     if (P.lpad < kAtomPadL + ceil_div(rows_to_cover, tile) * tile + (P.K - 1 - P.center) * P.dil || P.center * P.dil > kAtomPadL)
         throw CudaError("conv1d_tc: atom buffer pad too small");
-    const size_t a_stage = (size_t)P.rows * 16 * (pl.CK / 8), b_stage = (size_t)pl.N * 16 * (pl.CK / 8);
-    const size_t smem = ((SA * a_stage + 127) & ~(size_t)127) + SB * b_stage + 128;
-    if (smem > (size_t)kMaxDynTc) throw CudaError("conv1d_tc: shared memory budget exceeded");
+    const bool accum32 = P.mode == CONV_ACCUM && P.out32 != nullptr;
+    const int nf = (P.resid || P.out32) ? ((P.resid && accum32) ? 2 : 1) : 0;
+    const ConvTcSmem sm = conv1d_tc_smem(pl, P.K, P.dil, P.up, nf);
+    if (sm.direct > (size_t)kMaxDynTc) throw CudaError("conv1d_tc: shared memory budget exceeded");
+    // the staged epilogue moves whole 16-byte units: fp32 rows (stride Lout) and atom planes must start 16-byte aligned
+    auto al16 = [](const void* p) { return ((uintptr_t)p & 15) == 0; };
+    const bool staged = g_conv_tc_epilogue != 0 && sm.staged != 0 && (nf == 0 || P.Lout % 4 == 0) && al16(P.resid) &&
+                        al16(P.out32) && al16(P.out16);
+    const size_t smem = staged ? sm.staged : sm.direct;
+    P.epi_nf = nf; P.epi_off = (uint32_t)sm.epi_off; P.epi_slab = (uint32_t)sm.slab_bytes;
     if (batch > kVocMaxItems) throw CudaError("conv1d_tc: batch exceeds kVocMaxItems");
     P.tile_rows = tile; P.tiles_n = pl.n_tiles; P.batch = batch;
     const int extra = P.up ? 1 : 0;
@@ -335,10 +481,10 @@ static void launch_tc_common(ConvTcParams& P, const ConvTcPlan& pl, int rows_to_
     dim3 grid(std::min(total_tiles, cap));           // one persistent CTA per SM (of the SMs this launch may take)
     ProfScope ps(KF_CONV1D_TC, st, flops, bytes);
     switch (pl.N) {
-        case 256: launch_inst<256, 1>(P, grid, smem, st); break;
-        case 128: launch_inst<128, 2>(P, grid, smem, st); break;
-        case 64: launch_inst<64, 4>(P, grid, smem, st); break;
-        case 32: launch_inst<32, 4>(P, grid, smem, st); break;
+        case 256: launch_inst<256, 1>(P, staged, grid, smem, st); break;
+        case 128: launch_inst<128, 2>(P, staged, grid, smem, st); break;
+        case 64: launch_inst<64, 4>(P, staged, grid, smem, st); break;
+        case 32: launch_inst<32, 4>(P, staged, grid, smem, st); break;
         default: throw CudaError("conv1d_tc: tile width must be 32, 64, 128 or 256");
     }
     COUNT_LAUNCH(); KERNEL_CHECK();

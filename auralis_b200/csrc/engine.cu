@@ -1869,6 +1869,7 @@ void Engine::set_option(const std::string& k, int64_t v) {
     }
     else if (k == "voc_segment") voc_segment = (int)std::max<int64_t>(0, v);
     else if (k == "voc_sms") voc_sms = (int)std::max<int64_t>(0, v);
+    else if (k == "tc_epilogue") g_conv_tc_epilogue = v ? 1 : 0;
     else if (k == "voc_batch") voc_max_items = (int)std::max<int64_t>(1, std::min<int64_t>(v, kVocMaxItems));
     else if (k == "gemm_wide") {                                  // 0 off, else the wide kernel's ring depth
         if (v != 0 && (v < 2 || v > 4)) throw std::runtime_error("gemm_wide: 0 (off) or a ring depth of 2, 3 or 4");

@@ -48,6 +48,20 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
+// contiguous bulk copy shared -> global (16-byte aligned addresses, size a multiple of 16), tracked per thread in bulk
+// groups: commit closes this thread's group, wait_read<n> returns once all but n of its groups have finished READING
+// shared memory (the source may be overwritten), wait_all<n> once their global writes are complete
+__device__ __forceinline__ void bulk_s2g(void* dst, const void* src, uint32_t bytes) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
+                 ::"l"(dst), "r"(smem_u32(src)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+// generic-proxy writes to shared memory made visible to the async proxy (a following bulk copy reads them)
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // wgmma shared-memory matrix descriptor:
 //   [0,14) start >> 4 | [16,30) leading byte offset >> 4 | [32,46) stride byte offset >> 4 | [62,64) layout

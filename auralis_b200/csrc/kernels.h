@@ -172,6 +172,10 @@ int atoms_lpad(int L);                                   // padded rows per plan
 struct ConvTcPlan { int N, CK, n_tiles, nacc; bool ok; size_t tile_halves, blob_halves; };
 ConvTcPlan conv1d_tc_plan(int Cin, int Cout, int K);
 void conv1d_tc_pack(const float* w /*[Cout][Cin][K]*/, int Cin, int Cout, int K, const ConvTcPlan& pl, __half* blob);
+// dynamic shared memory of a launch: `direct` epilogue; `staged` epilogue (0 = does not fit / transposed conv) with its
+// slab ring at `epi_off`, slabs of `slab_cols` GEMM columns x tile rows, `slab_bytes` each; nf = fp32 buffers per slab
+struct ConvTcSmem { size_t direct, staged, epi_off, slab_bytes; int slab_cols; };
+ConvTcSmem conv1d_tc_smem(const ConvTcPlan& pl, int K, int dil, int up, int nf);
 // y = bias + cbias + resid + conv(a16);  out32 (fp32 [C][L], store/accumulate) and/or out16 (lrelu(y, slope_out) atoms)
 // out16 = lrelu(y * scale16, slope_out)
 // (engine knobs of the launchers — attention grid cap, decode GEMM tile, vocoder SM cap — live in

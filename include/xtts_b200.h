@@ -154,6 +154,9 @@ int xtts_fetch(xtts_engine* e, uint64_t seq_id, int32_t* tokens, float* wav, flo
  *                         stream beside the decode step), 0 = one window per chunk when it ends.  Same samples either way.
  *   "voc_sms"             SMs the vocoder's persistent conv kernels may occupy while a decode step is in flight (0 = all)
  *   "voc_batch"           windows per vocoder launch (1..32, default 32; ragged lengths are batched together)
+ *   "tc_epilogue"         epilogue of the fast-mode vocoder's tensor-core Conv1d: 1 (default) = staged through shared
+ *                         memory (residual prefetched by a loader warp, outputs drained by bulk copies while the next
+ *                         tile's MMAs run), 0 = straight from the accumulators.  Bit-identical results either way.
  *   "attn_warps"          warps per (row, head) item of the 16-bit decode attention: 4 (default), 1 / 2 / 8 / 16 measured slower
  *   "attn_ctas_per_sm"    > 0 caps the decode-attention grid (each CTA walks several items); < 0: absolute grid size (tests)
  *   "attn_l2_pages"       n > 0: each warp of the decode attention asks L2 for n of its later pages per item
