@@ -70,15 +70,28 @@ class VocoderDims:
             p *= r
         return p
 
-    def z_frames(self, n_latents: int) -> int:
+    def z_frames(self, n_latents: int, speed: float = 1.0) -> int:
         """Length after the two linear interpolations (hifigan_decoder.py:787-800):
-        floor(floor(T*4.0) * 24000/22050) with torch's float rule."""
+        floor(floor(T*4.0) * 24000/22050) with torch's float rule.  A speaking rate other than 1 first time-scales the T
+        latents to floor(T * ls) frames, ls = 1 / speed with the speed rounded to float32 (what the engine receives)."""
         import math
+        if speed != 1.0:
+            n_latents = int(math.floor(n_latents * speed_scale(speed)))
         t1 = int(math.floor(n_latents * (self.code_stride / self.output_hop_length)))
         return int(math.floor(t1 * (self.output_sample_rate / self.input_sample_rate)))
 
-    def n_samples(self, n_latents: int) -> int:
-        return self.z_frames(n_latents) * self.hop
+    def n_samples(self, n_latents: int, speed: float = 1.0) -> int:
+        return self.z_frames(n_latents, speed) * self.hop
+
+
+SPEED_MIN, SPEED_MAX = 0.25, 4.0     # speaking-rate range (that of OpenAI's /v1/audio/speech)
+
+
+def speed_scale(speed: float) -> float:
+    """The time scale of a speaking rate, ls = 1 / speed, from the float32 value every layer receives (Xtts.inference:
+    length_scale = 1 / speed)."""
+    import numpy as np
+    return 1.0 / float(np.float32(speed))
 
 
 @dataclass

@@ -16,6 +16,7 @@
 #include <memory>
 #include <mutex>
 #include <thread>
+#include <tuple>
 #include <unordered_map>
 #include <vector>
 
@@ -88,6 +89,7 @@ struct Sequence {
     std::vector<int32_t> text_ids;
     int speaker = 0;
     xtts_sampling sp{};
+    float speed = 1.f;            // speaking rate (xtts_submit_speed): time-scales the latents before the vocoder
     int slot = -1;
     int n_prompt = 0;
     int max_tok = 0;              // min(sp.max_tokens, max_audio_tokens)
@@ -131,6 +133,7 @@ struct VocJob {
     int zw0 = 0, zw1 = 0, zk0 = 0, zk1 = 0;
     int tok_upto = 0;             // tokens [0, tok_upto) are final and copied out with this job
     bool final = false;
+    bool internal = false;        // a leading window of a finished chunk too long for one window: never a partial piece
     int fail_status = 0;          // final job of a cancelled / failed chunk: no vocoder work, this status is delivered
 };
 struct VocBatch {
@@ -154,7 +157,7 @@ public:
     void set_speaker(int slot, const float* cond, const float* g);
     void get_speaker(int slot, float* cond, float* g);
     void condition(int slot, const float* w22, int64_t n22, const float* w16, int64_t n16, int cond_len, int chunk_len);
-    void submit(uint64_t id, const int32_t* text, int n_text, int speaker, const xtts_sampling& sp);
+    void submit(uint64_t id, const int32_t* text, int n_text, int speaker, const xtts_sampling& sp, float speed);
     void cancel(uint64_t id);
     int poll(xtts_result* out, int timeout_ms);
     void fetch(uint64_t id, int32_t* tokens, float* wav, float* latents);
@@ -168,6 +171,7 @@ public:
     void vocode_sync(const float* latents, int T, int speaker, float* wav, int* n_out, const char* stage,
                      float* stage_out, int64_t stage_cap);
     void vocode_window_sync(const float* latents, int T, int speaker, int z0, int nz, float* wav);
+    void vocode_speed_sync(const float* latents, int T, int speaker, float speed, int z0, int nz, float* wav, int* n_out);
     void gpt_prefill_sync(const int32_t* text, int n_text, int speaker, const int32_t* audio, int n_audio,
                           float* hidden_out, float* logits_out, float* latents_out);
     void gpt_teacher_forced_sync(const int32_t* text, int n_text, int speaker, const int32_t* forced, int n,
@@ -333,15 +337,19 @@ private:
     void up(DBuf<float>& d, const std::vector<float>& h) { d.alloc(h.size()); d.upload(h.data(), h.size(), st); weight_bytes += h.size() * 4; }
     void make_linear(Linear& lin, const std::string& wname, const std::string& bname, bool conv1d_layout, int pad_n = 0);
     void make_conv(ConvW& c, const std::string& prefix, bool transposed, bool has_bias);
-    struct VocItem { const float* lat; int T; int z0, nz; int speaker; };
+    struct VocItem { const float* lat; int T; int z0, nz; int speaker; float speed = 1.f; };
+    InterpItem interp_item(const VocItem& v) const;
+    bool speed_stage(int T, float speed) const;
+    struct VocSpan { int zw0, zw1, zk0, zk1; };
+    std::vector<VocSpan> split_windows(int zk0, int Tz) const;
     void run_vocoder_tc(const VocItem* it, int nb, int Lz, float* wav_dev_out, const char* stage, float* stage_out,
                         int64_t stage_cap);
     void run_vocoder_f32(const VocItem* it, int nb, int Lz, float* wav_dev_out, const char* stage, float* stage_out,
                          int64_t stage_cap);
     bool voc_fits(int nb, int Lz) const;
     void compute_voc_margin(int pre_k);
-    int z_frames(int T) const;
-    int z_avail(int n) const;
+    int z_frames(int T, float speed = 1.f) const;
+    int z_avail(int n, float speed = 1.f) const;
     std::vector<float> folded(const std::string& prefix) const;
     GptTables tables() const {
         GptTables t; t.text_emb = text_emb.p; t.text_pos = text_pos.p; t.wte = wte.p; t.wpe = wpe.p;
@@ -371,7 +379,7 @@ private:
     void prefill(const std::vector<Sequence*>& seqs);
     void decode_step(const std::vector<int>& active);
     void run_vocoder(const VocItem* it, int nb, float* wav_dev_out, const char* stage, float* stage_out, int64_t stage_cap);
-    int samples_for(int T) const;
+    int samples_for(int T, float speed = 1.f) const;
     void on_finished(std::shared_ptr<Sequence> s, int n_tokens, int fail_status);
     void maybe_cut_window(std::shared_ptr<Sequence>& s);
     void dispatch_ready(bool decode_active);
@@ -1208,7 +1216,10 @@ void Engine::decode_step(const std::vector<int>& active) {
 // zero padding too, so the caller discards `voc_hz` z-frames of output next to them (receptive field).  Windows of one
 // batch may have different lengths: buffers are strided by the longest (Lz), kernels skip what lies beyond an item's end.
 // All vocoder work is issued on st_voc.  wav_dev_out: [nb][Lz * hop].
-int Engine::z_frames(int T) const {
+// A speaking rate other than 1 adds one level in front (Xtts.inference: F.interpolate(scale_factor = 1 / speed)): T latents
+// become T0 = floor(T * ls) frames, ls = 1 / (double)speed computed from the float32 speed.
+int Engine::z_frames(int T, float speed) const {
+    if (speed != 1.f) T = (int)std::floor((double)T * (1.0 / (double)speed));
     const double s1 = (double)cfg.code_stride / (double)cfg.output_hop_length;
     const double s2 = (double)cfg.output_sample_rate / (double)cfg.input_sample_rate;
     const int T1 = (int)std::floor((double)T * s1);
@@ -1217,18 +1228,63 @@ int Engine::z_frames(int T) const {
 
 // z-frames that can be interpolated from the first n latent frames of a chunk that is still growing, i.e. without touching
 // either interpolation's end clamp: z[j] reads y[a0], y[a0 + 1] with a0 = floor((j + .5) / s2 - .5) and y[a] reads
-// lat[b0], lat[b0 + 1] with b0 = floor((a + .5) / s1 - .5); one frame of slack on both levels (float rounding)
-int Engine::z_avail(int n) const {
+// lat[b0], lat[b0 + 1] with b0 = floor((a + .5) / s1 - .5); one frame of slack on both levels (float rounding).  With a
+// speaking rate the latents go through one more level first (same rule, same slack), and the two levels run on its output.
+int Engine::z_avail(int n, float speed) const {
     const double s1 = (double)cfg.code_stride / (double)cfg.output_hop_length;
     const bool resample = cfg.output_sample_rate != cfg.input_sample_rate;
     const double s2 = resample ? (double)cfg.output_sample_rate / (double)cfg.input_sample_rate : 1.0;
-    const int A = (int)std::floor(((double)n - 1.5) * s1 - 0.5) - 1;        // largest y index whose sources are < n - 1
+    int n0 = n;                                                             // frames the y level may read
+    if (speed != 1.f) {
+        const double ls = 1.0 / (double)speed;
+        const int A0 = (int)std::floor(((double)n - 1.5) * ls - 0.5) - 1;   // largest scaled index whose sources are < n - 1
+        if (A0 < 1) return 0;
+        n0 = A0 + 1;
+    }
+    const int A = (int)std::floor(((double)n0 - 1.5) * s1 - 0.5) - 1;       // largest y index whose sources are < n0 - 1
     if (A < 1) return 0;
     const int J = (int)std::floor(((double)A - 0.5) * s2 - 0.5) - 1;        // z indices < J read y indices <= A
-    return std::max(0, std::min(J, z_frames(n)));
+    return std::max(0, std::min(J, z_frames(n, speed)));
 }
 
-int Engine::samples_for(int T) const { return z_frames(T) * voc_hop; }
+int Engine::samples_for(int T, float speed) const { return z_frames(T, speed) * voc_hop; }
+
+// Whether T latents at `speed` go through the speed stage: not at speed 1 (skipped, as Coqui does), and not when
+// floor(T * ls) == T either (short chunks at speeds just below 1), where F.interpolate copies its input.  Once true for a
+// chunk still growing, it stays true for its final length (T * (ls - 1) >= 1 only grows with T).
+bool Engine::speed_stage(int T, float speed) const {
+    return speed != 1.f && (int)std::floor((double)T * (1.0 / (double)speed)) != T;
+}
+
+// the interpolation launch item of a vocoder window (clamp lengths of every level, the speed stage's T0 / r0)
+InterpItem Engine::interp_item(const VocItem& v) const {
+    const double s1 = (double)cfg.code_stride / (double)cfg.output_hop_length;
+    const bool resample = cfg.output_sample_rate != cfg.input_sample_rate;
+    InterpItem ii{v.lat, v.T, 0, v.z0, v.nz};
+    int Ty = v.T;                                   // frames the chunk-level interpolations run on
+    if (speed_stage(v.T, v.speed)) {
+        const double ls = 1.0 / (double)v.speed;
+        ii.T0 = Ty = (int)std::floor((double)v.T * ls);
+        ii.r0 = (float)(1.0 / ls);
+    }
+    ii.T1 = resample ? (int)std::floor((double)Ty * s1) : Ty;
+    return ii;
+}
+
+// The windows that produce z-frames [zk0, Tz) of a finished chunk, none longer than the workspace's voc_max_Tz: each keeps
+// [zk0_i, zk1_i) and carries voc_hz frames of margin on its inner edges.  One window unless a speaking rate < 1 stretched
+// the chunk past voc_max_Tz; every window but the last is exactly voc_max_Tz long.
+std::vector<Engine::VocSpan> Engine::split_windows(int zk0, int Tz) const {
+    std::vector<VocSpan> out;
+    for (int k0 = zk0;;) {
+        const int w0 = std::max(0, k0 - voc_hz);
+        if (Tz - w0 <= voc_max_Tz) { out.push_back(VocSpan{w0, Tz, k0, Tz}); break; }
+        const int k1 = w0 + voc_max_Tz - voc_hz;
+        out.push_back(VocSpan{w0, k1 + voc_hz, k0, k1});
+        k0 = k1;
+    }
+    return out;
+}
 
 bool Engine::voc_fits(int nb, int Lz) const {
     if (nb < 1 || nb > kVocMaxItems || Lz < 1 || Lz > voc_max_Tz) return false;
@@ -1282,11 +1338,7 @@ void Engine::run_vocoder_f32(const VocItem* it, int nb, int Lz, float* wav_dev_o
             }
         };
         InterpItem ii[kVocMaxItems];
-        for (int k = 0; k < rn; ++k) {
-            const VocItem& v = it[i0 + k];
-            ii[k] = InterpItem{v.lat, v.T, (int)std::floor((double)v.T * s1), v.z0, v.nz};
-            if (!resample) ii[k].T1 = ii[k].T;
-        }
+        for (int k = 0; k < rn; ++k) ii[k] = interp_item(it[i0 + k]);
         launch_interp(ii, rn, vz.p, nullptr, 0, c.voc_in_dim, Tz, s1, resample ? s2 : 1.0, sv);
         dump("z", vz.p, (size_t)c.voc_in_dim * Tz);
         launch_conv1d(vz.p, conv_pre.wt.p, conv_pre.b.p, cb + cbias_off[0], nullptr, vpre.p, conv_pre.Cin, conv_pre.Cout, Tz,
@@ -1352,7 +1404,7 @@ void Engine::run_vocoder_tc(const VocItem* it, int nb, int Lz, float* wav_dev_ou
     InterpItem ii[kVocMaxItems];
     int lens[kVocMaxItems];                  // per-item signal length at the current stage
     for (int k = 0; k < nb; ++k) {
-        ii[k] = InterpItem{it[k].lat, it[k].T, resample ? (int)std::floor((double)it[k].T * s1) : it[k].T, it[k].z0, it[k].nz};
+        ii[k] = interp_item(it[k]);
         lens[k] = it[k].nz;
     }
     auto conv_tc = [&](const ConvW& w, const __half* a16, const float* cbias, const float* resid, float* out32, __half* out16,
@@ -1448,14 +1500,15 @@ void Engine::dev_put(float* p, size_t cap) { std::lock_guard<std::mutex> lk(pin_
 
 void Engine::pinned_put(float* p, size_t cap) { std::lock_guard<std::mutex> lk(pin_mu); pinned_pool.emplace_back(p, cap); }
 
-void Engine::submit(uint64_t id, const int32_t* text, int n_text, int speaker, const xtts_sampling& sp) {
+void Engine::submit(uint64_t id, const int32_t* text, int n_text, int speaker, const xtts_sampling& sp, float speed) {
+    if (!(speed >= 0.25f && speed <= 4.0f)) throw std::runtime_error("speed out of range (0.25..4)");   // NaN included
     if (n_text <= 0 || n_text > cfg.max_text_tokens + 2) throw std::runtime_error("n_text out of range (1..max_text_tokens+2)");
     if (speaker < 0 || speaker >= S) throw std::runtime_error("speaker slot out of range");
     // ids are checked here so that a bad id fails this call alone, not the batched step it would have joined
     for (int i = 0; i < n_text; ++i)
         if (text[i] < 0 || text[i] >= cfg.n_text_tokens) throw std::runtime_error("text token id out of range");
     std::shared_ptr<Sequence> s(new Sequence());
-    s->id = id; s->text_ids.assign(text, text + n_text); s->speaker = speaker; s->sp = sp; s->t_submit = now_s();
+    s->id = id; s->text_ids.assign(text, text + n_text); s->speaker = speaker; s->sp = sp; s->speed = speed; s->t_submit = now_s();
     require_finalized();
     if (!spk_valid[speaker]) throw std::runtime_error("speaker slot not set");
     {
@@ -1519,9 +1572,20 @@ void Engine::on_finished(std::shared_ptr<Sequence> s, int n_tokens, int fail_sta
     VocJob j;
     j.s = s; j.final = true; j.fail_status = fail_status; j.T_clamp = std::max(1, s->n_tokens); j.tok_upto = s->n_tokens;
     if (fail_status == 0 && s->sp.vocode && s->n_tokens > 0) {
-        const int Tz = z_frames(s->n_tokens);
+        const int Tz = z_frames(s->n_tokens, s->speed);
         j.zk0 = std::min(s->voc_z_done, Tz); j.zk1 = Tz;
         j.zw0 = std::max(0, j.zk0 - voc_hz); j.zw1 = Tz;
+        if (j.zk0 < Tz) {
+            // a slow speaking rate can stretch the rest of the chunk past one window: internal windows, then the final one
+            const std::vector<VocSpan> w = split_windows(j.zk0, Tz);
+            for (size_t i = 0; i + 1 < w.size(); ++i) {
+                VocJob k;
+                k.s = s; k.T_clamp = j.T_clamp; k.internal = true;
+                k.zw0 = w[i].zw0; k.zw1 = w[i].zw1; k.zk0 = w[i].zk0; k.zk1 = w[i].zk1;
+                voc_pending.push_back(std::move(k));
+            }
+            j.zw0 = w.back().zw0; j.zw1 = w.back().zw1; j.zk0 = w.back().zk0; j.zk1 = w.back().zk1;
+        }
     }
     s->next_boundary = 0;
     voc_pending.push_back(std::move(j));
@@ -1533,8 +1597,10 @@ void Engine::maybe_cut_window(std::shared_ptr<Sequence>& s) {
     while (s->next_boundary > 0 && s->next_boundary < s->max_tok) {
         const int b = s->next_boundary;
         const int n_avail = s->steps + 1;                   // latent frames in the ring
-        const int zk1 = z_frames(b), zw1 = zk1 + voc_hz;
-        if (z_avail(n_avail) < zw1) return;
+        // a window has to use the speed stage exactly when the finished chunk will: not before it applies to n_avail
+        if (s->speed != 1.f && !speed_stage(n_avail, s->speed)) return;
+        const int zk1 = z_frames(b, s->speed), zw1 = zk1 + voc_hz;
+        if (z_avail(n_avail, s->speed) < zw1) return;
         const int zk0 = s->voc_z_done;
         const int zw0 = std::max(0, zk0 - voc_hz);
         if (zw1 - zw0 > voc_max_Tz) { s->next_boundary = 0; return; }
@@ -1563,10 +1629,10 @@ void Engine::dispatch_batch(std::vector<VocJob>& jobs, bool decode_active) {
             Sequence& s = *j.s;
             if (!s.tok_host) s.tok_host = reinterpret_cast<int32_t*>(pinned_get((size_t)std::max(1, s.max_tok), &s.tok_cap));
             if (j.zk1 > j.zk0) {
-                const size_t need = (size_t)std::max(1, samples_for(s.max_tok));
+                const size_t need = (size_t)std::max(1, samples_for(s.max_tok, s.speed));
                 if (d2h_wav) { if (!s.wav_host) s.wav_host = pinned_get(need, &s.wav_cap); }
                 else if (!s.wav_dev) s.wav_dev = dev_get(need, &s.wav_dev_cap);
-                items.push_back(VocItem{d_latents.p + (size_t)s.slot * CAP * H, j.T_clamp, j.zw0, j.zw1 - j.zw0, s.speaker});
+                items.push_back(VocItem{d_latents.p + (size_t)s.slot * CAP * H, j.T_clamp, j.zw0, j.zw1 - j.zw0, s.speaker, s.speed});
                 job_of.push_back((int)k);
             }
         }
@@ -1648,11 +1714,26 @@ void Engine::complete_batch(VocBatch& b) {
     float ms = 0.f;
     if (cudaEventElapsedTime(&ms, b.ev0, b.ev1) == cudaSuccess) st_voc_ms += ms;
     const double t = now_s();
-    for (auto& j : b.jobs) {
+    // dispatch_ready sorted the batch longest first: a chunk with several windows here gets them back in the order they
+    // were cut (ascending z), its final result last; chunks keep their batch order
+    const size_t n = b.jobs.size();
+    std::vector<size_t> first(n), ord(n);
+    for (size_t i = 0; i < n; ++i) {
+        first[i] = i;
+        for (size_t k = 0; k < i; ++k)
+            if (b.jobs[k].s == b.jobs[i].s) { first[i] = first[k]; break; }
+        ord[i] = i;
+    }
+    std::stable_sort(ord.begin(), ord.end(), [&](size_t x, size_t y) {
+        const VocJob &a = b.jobs[x], &c = b.jobs[y];
+        return std::make_tuple(first[x], a.final, a.zk0) < std::make_tuple(first[y], c.final, c.zk0);
+    });
+    for (size_t oi : ord) {
+        VocJob& j = b.jobs[oi];
         Sequence& s = *j.s;
         const int samp_end = j.zk1 > j.zk0 ? j.zk1 * voc_hop : s.samp_delivered;
         if (!j.final) {
-            if (!s.stream_pieces) continue;                 // accumulated silently: everything goes out with the final result
+            if (!s.stream_pieces || j.internal) continue;   // accumulated silently: everything goes out with the final result
             std::shared_ptr<Piece> p(new Piece());
             p->s = j.s; p->status = 1; p->tok0 = s.tok_delivered; p->tok1 = j.tok_upto;
             p->samp0 = s.samp_delivered; p->nsamp = samp_end - s.samp_delivered; p->t_done = t;
@@ -1663,7 +1744,7 @@ void Engine::complete_batch(VocBatch& b) {
         std::shared_ptr<Piece> p(new Piece());
         p->s = j.s; p->final = true; p->status = j.fail_status; p->t_done = s.t_done = t;
         if (j.fail_status == 0) {
-            const int total = s.sp.vocode ? samples_for(s.n_tokens) : 0;
+            const int total = s.sp.vocode ? samples_for(s.n_tokens, s.speed) : 0;
             p->tok0 = 0; p->tok1 = s.n_tokens;              // the final result lists every token; samples: what is left
             p->samp0 = s.samp_delivered; p->nsamp = std::max(0, total - s.samp_delivered);
         }
@@ -2012,6 +2093,39 @@ void Engine::vocode_window_sync(const float* latents, int T, int speaker, int z0
     run_vocoder(&it, 1, vwav.p, nullptr, nullptr, 0);
     if (wav) vwav.download(wav, (size_t)nz * voc_hop, st_voc);
     CUDA_CHECK(cudaStreamSynchronize(st_voc));
+}
+
+// The vocoder at a speaking rate: z-frames [z0, z0 + nz) as one window (nz >= 0), or the whole chunk (nz < 0) — in the
+// windows the scheduler would cut for it (split_windows) when it is longer than one, their kept samples stitched.
+void Engine::vocode_speed_sync(const float* latents, int T, int speaker, float speed, int z0, int nz, float* wav, int* n_out) {
+    ApiLock lk(this);
+    require_finalized();
+    CUDA_CHECK(cudaSetDevice(cfg.device));
+    if (!(speed >= 0.25f && speed <= 4.0f)) throw std::runtime_error("speed out of range (0.25..4)");
+    if (T <= 0 || T > voc_max_T) throw std::runtime_error("vocoder: latent count out of range");
+    if (speaker < 0 || speaker >= S || !spk_valid[speaker]) throw std::runtime_error("vocoder: speaker slot not set");
+    const int Tz = z_frames(T, speed);
+    std::vector<VocSpan> spans;
+    if (nz >= 0) {
+        if (z0 < 0 || nz == 0 || z0 + nz > Tz) throw std::runtime_error("vocoder: window outside the chunk");
+        spans.push_back(VocSpan{z0, z0 + nz, z0, z0 + nz});
+    } else if (Tz > 0) {
+        spans = split_windows(0, Tz);
+    }
+    const int zbase = nz >= 0 ? z0 : 0;
+    if (!spans.empty()) {
+        DBuf<float> lat; lat.alloc((size_t)T * cfg.voc_in_dim);
+        lat.upload(latents, (size_t)T * cfg.voc_in_dim, st_voc);
+        for (const VocSpan& w : spans) {
+            VocItem it{lat.p, T, w.zw0, w.zw1 - w.zw0, speaker, speed};
+            run_vocoder(&it, 1, vwav.p, nullptr, nullptr, 0);
+            if (wav)
+                CUDA_CHECK(cudaMemcpyAsync(wav + (size_t)(w.zk0 - zbase) * voc_hop, vwav.p + (size_t)(w.zk0 - w.zw0) * voc_hop,
+                                           (size_t)(w.zk1 - w.zk0) * voc_hop * sizeof(float), cudaMemcpyDeviceToHost, st_voc));
+        }
+        CUDA_CHECK(cudaStreamSynchronize(st_voc));
+    }
+    if (n_out) *n_out = (nz >= 0 ? nz : Tz) * voc_hop;
 }
 
 void Engine::gpt_prefill_sync(const int32_t* text, int n_text, int speaker, const int32_t* audio, int n_audio,
@@ -2481,7 +2595,11 @@ int xtts_condition(xtts_engine* e, int32_t slot, const float* wav22k, int64_t n2
 }
 int xtts_submit(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
                 const xtts_sampling* sp) {
-    XTTS_TRY(e->impl->submit(seq_id, text_ids, n_text, speaker_slot, *sp))
+    return xtts_submit_speed(e, seq_id, text_ids, n_text, speaker_slot, sp, 1.0f);
+}
+int xtts_submit_speed(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
+                      const xtts_sampling* sp, float speed) {
+    XTTS_TRY(e->impl->submit(seq_id, text_ids, n_text, speaker_slot, *sp, speed))
 }
 int xtts_cancel(xtts_engine* e, uint64_t seq_id) { XTTS_TRY(e->impl->cancel(seq_id)) }
 int xtts_poll(xtts_engine* e, xtts_result* out, int32_t timeout_ms) {
@@ -2506,6 +2624,10 @@ int xtts_vocode(xtts_engine* e, const float* latents, int32_t T, int32_t speaker
 }
 int xtts_vocode_window(xtts_engine* e, const float* latents, int32_t T, int32_t speaker_slot, int32_t z0, int32_t nz, float* wav) {
     XTTS_TRY(e->impl->vocode_window_sync(latents, T, speaker_slot, z0, nz, wav))
+}
+int xtts_vocode_speed(xtts_engine* e, const float* latents, int32_t T, int32_t speaker_slot, float speed, int32_t z0, int32_t nz,
+                      float* wav, int32_t* n_out) {
+    XTTS_TRY(e->impl->vocode_speed_sync(latents, T, speaker_slot, speed, z0, nz, wav, n_out))
 }
 int xtts_gpt_prefill(xtts_engine* e, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
                      const int32_t* audio_tokens, int32_t n_audio, float* hidden_out, float* logits_out, float* latents_out) {

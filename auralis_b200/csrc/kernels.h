@@ -154,7 +154,11 @@ constexpr int kVocMaxItems = 32;
 // One item of an interpolation launch: z-frames [z0, z0 + nz) of a chunk whose latents start at `lat` ([T][C] fp32, device).
 // T / T1 are the clamp lengths of the two linear interpolations (HifiDecoder.forward): the chunk's real length once it is
 // known, otherwise any length the window does not reach (a window of a still-growing chunk never touches the clamp).
-struct InterpItem { const float* lat; int T, T1, z0, nz; };
+// r0 > 0: the chunk has a speaking rate (Xtts.inference's speed): the latents are first time-scaled by one more linear
+// interpolation to T0 = floor(T * ls) frames, ls = 1 / (double)speed, source index r0 * (j + .5) - .5 with r0 = (float)(1 / ls)
+// (torch's rule for F.interpolate(scale_factor=ls)); T1 is then the clamp length of the next level on those T0 frames.
+// r0 == 0: no such stage (speed 1), the two-level code.
+struct InterpItem { const float* lat; int T, T1, z0, nz; int T0 = 0; float r0 = 0.f; };
 // z32 (fp32 [batch][C][Lz]) and/or z16 (fp16 atoms [batch][C/8][lpad][8]) — either may be null; Lz = row stride >= max nz
 void launch_interp(const InterpItem* items, int batch, float* z32, __half* z16, int lpad, int C, int Lz, double scale1,
                    double scale2, cudaStream_t st);

@@ -21,16 +21,32 @@ namespace {
 __device__ __forceinline__ float lrelu(float v, float slope) { return v > 0.f ? v : v * slope; }
 
 // ------------------------------------------------------------------------------------------------
-// fused double linear interpolation + transpose:  latents [T][C]  ->  z [C][Tz]
+// fused double (triple, with a speaking rate) linear interpolation + transpose:  latents [T][C]  ->  z [C][Tz]
 // ------------------------------------------------------------------------------------------------
+// The roundings of this stage are spelled out with intrinsics (no contraction left to the compiler), so that the two-level
+// code keeps its exact arithmetic whatever code surrounds it: chunks without a speaking rate get the same bits as before it.
 __device__ __forceinline__ void lin_src(int dst, float rscale, int in_len, int& i0, int& i1, float& l0, float& l1) {
-    float src = rscale * ((float)dst + 0.5f) - 0.5f;
+    float src = __fmaf_rn(rscale, (float)dst + 0.5f, -0.5f);
     if (src < 0.f) src = 0.f;
     i0 = (int)src;
     if (i0 > in_len - 1) i0 = in_len - 1;
     i1 = i0 + ((i0 < in_len - 1) ? 1 : 0);
     l1 = src - (float)i0;
     l0 = 1.0f - l1;
+}
+
+// speed stage, channel c: frame b of the time-scaled latents, then frame a of the first chunk-level interpolation on them;
+// l0 * x0 + l1 * x1 rounded as ATen's CPU kernel does, fma(l0, x0, l1 * x1)
+__device__ __forceinline__ float lerp_aten(float l0, float x0, float l1, float x1) { return __fmaf_rn(l0, x0, __fmul_rn(l1, x1)); }
+__device__ __forceinline__ float speed_frame(const float* __restrict__ lat, int b, float r0, int T, int C, int c) {
+    int i0, i1; float l0, l1;
+    lin_src(b, r0, T, i0, i1, l0, l1);
+    return lerp_aten(l0, lat[(size_t)i0 * C + c], l1, lat[(size_t)i1 * C + c]);
+}
+__device__ __forceinline__ float speed_level1(const float* __restrict__ lat, int a, float r1, int T0, float r0, int T, int C, int c) {
+    int b0, b1; float n0, n1;
+    lin_src(a, r1, T0, b0, b1, n0, n1);
+    return lerp_aten(n0, speed_frame(lat, b0, r0, T, C, c), n1, speed_frame(lat, b1, r0, T, C, c));
 }
 
 struct PostLens { int len[kVocMaxItems]; };
@@ -53,12 +69,18 @@ interp_kernel(const InterpBatch B, float* __restrict__ z_, uint4* __restrict__ z
         if (j < nz && c < C) {
             int a0, a1; float m0, m1;
             lin_src(it.z0 + j, r2, T1, a0, a1, m0, m1);
-            int b0, b1; float n0, n1;
-            lin_src(a0, r1, T, b0, b1, n0, n1);
-            const float za = n0 * lat[(size_t)b0 * C + c] + n1 * lat[(size_t)b1 * C + c];
-            lin_src(a1, r1, T, b0, b1, n0, n1);
-            const float zb = n0 * lat[(size_t)b0 * C + c] + n1 * lat[(size_t)b1 * C + c];
-            v = m0 * za + m1 * zb;
+            if (it.r0 > 0.f) {                          // three levels: up to 8 latent rows per value (L1 / L2 hits)
+                const float za = speed_level1(lat, a0, r1, it.T0, it.r0, T, C, c);
+                const float zb = speed_level1(lat, a1, r1, it.T0, it.r0, T, C, c);
+                v = lerp_aten(m0, za, m1, zb);
+            } else {                                    // n0 x0 + n1 x1 = fma(n1, x1, n0 x0);  m0 za + m1 zb = fma(m0, za, m1 zb)
+                int b0, b1; float n0, n1;
+                lin_src(a0, r1, T, b0, b1, n0, n1);
+                const float za = __fmaf_rn(n1, lat[(size_t)b1 * C + c], __fmul_rn(n0, lat[(size_t)b0 * C + c]));
+                lin_src(a1, r1, T, b0, b1, n0, n1);
+                const float zb = __fmaf_rn(n1, lat[(size_t)b1 * C + c], __fmul_rn(n0, lat[(size_t)b0 * C + c]));
+                v = __fmaf_rn(m0, za, __fmul_rn(m1, zb));
+            }
         }
         tile[ty + 8 * k][tx] = v;                       // tile[j][c]
     }

@@ -333,7 +333,8 @@ class XTTSv2Engine(BaseAsyncTTSEngine):
                                  repetition_penalty=request.repetition_penalty,
                                  max_tokens=self.dims.gpt.max_audio_tokens, stop_token=self.mel_eos_token_id,
                                  seed=base_seed, seq_seed=seq_index, vocode=True, priority=seq_index,
-                                 early_tokens=self.early_emit_tokens if (request.stream and seq_index == 0) else 0)
+                                 early_tokens=self.early_emit_tokens if (request.stream and seq_index == 0) else 0,
+                                 speed=getattr(request, "speed", 1.0))     # (the reference's own TTSRequest has none)
             rid = f"{request.request_id}_{seq_index}"
             generators.append(self._chunk_generator(rid, ids, gpt_cond_latent, speaker_embeddings, sp))
             request_ids.append(rid)

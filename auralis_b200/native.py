@@ -13,7 +13,7 @@ from typing import Dict, Optional, Tuple
 
 import numpy as np
 
-from .config import XTTSDims
+from .config import SPEED_MAX, SPEED_MIN, XTTSDims
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libxtts_b200.so")
@@ -74,8 +74,9 @@ class XttsKernelProfile(C.Structure):
 # every symbol include/xtts_b200.h declares (checked by tests/test_abi.py against the header text)
 ABI_SYMBOLS = [
     "xtts_last_error", "xtts_version", "xtts_create", "xtts_destroy", "xtts_load_weight", "xtts_finalize_weights",
-    "xtts_set_speaker", "xtts_get_speaker", "xtts_condition", "xtts_submit", "xtts_cancel", "xtts_poll", "xtts_fetch",
-    "xtts_set_option", "xtts_get_stats", "xtts_sync", "xtts_get_kernel_profile", "xtts_device_timer", "xtts_vocode", "xtts_vocode_window", "xtts_gpt_prefill", "xtts_gpt_teacher_forced",
+    "xtts_set_speaker", "xtts_get_speaker", "xtts_condition", "xtts_submit", "xtts_submit_speed", "xtts_cancel", "xtts_poll",
+    "xtts_fetch", "xtts_set_option", "xtts_get_stats", "xtts_sync", "xtts_get_kernel_profile", "xtts_device_timer", "xtts_vocode",
+    "xtts_vocode_window", "xtts_vocode_speed", "xtts_gpt_prefill", "xtts_gpt_teacher_forced",
     "xtts_debug_gemm", "xtts_debug_sample_slots", "xtts_debug_trace",
     "xtts_debug_attn_decode", "xtts_debug_attn_prefill", "xtts_debug_splitk_ln", "xtts_debug_conv_tc",
 ]
@@ -103,6 +104,7 @@ def load_library(path: Optional[str] = None):
     lib.xtts_get_speaker.argtypes = [vp, i32, f32p, f32p]
     lib.xtts_condition.argtypes = [vp, i32, f32p, i64, f32p, i64, i32, i32]
     lib.xtts_submit.argtypes = [vp, C.c_uint64, i32p, i32, i32, C.POINTER(XttsSampling)]
+    lib.xtts_submit_speed.argtypes = [vp, C.c_uint64, i32p, i32, i32, C.POINTER(XttsSampling), C.c_float]
     lib.xtts_cancel.argtypes = [vp, C.c_uint64]
     lib.xtts_poll.argtypes = [vp, C.POINTER(XttsResult), i32]
     lib.xtts_fetch.argtypes = [vp, C.c_uint64, i32p, f32p, f32p]
@@ -113,6 +115,7 @@ def load_library(path: Optional[str] = None):
     lib.xtts_device_timer.argtypes = [vp, i32, C.POINTER(C.c_double)]
     lib.xtts_vocode.argtypes = [vp, f32p, i32, i32, f32p, i32p, C.c_char_p, f32p, i64]
     lib.xtts_vocode_window.argtypes = [vp, f32p, i32, i32, i32, i32, f32p]
+    lib.xtts_vocode_speed.argtypes = [vp, f32p, i32, i32, C.c_float, i32, i32, f32p, i32p]
     lib.xtts_gpt_prefill.argtypes = [vp, i32p, i32, i32, i32p, i32, f32p, f32p, f32p]
     lib.xtts_gpt_teacher_forced.argtypes = [vp, i32p, i32, i32, i32p, i32, C.POINTER(XttsSampling), f32p, f32p, i32p]
     lib.xtts_debug_gemm.argtypes = [vp, i32, f32p, f32p, f32p, f32p, f32p, i32, i32, i32, i32, i32, f32p]
@@ -196,6 +199,7 @@ class Sampling:
     vocode: bool = True
     priority: int = 0
     early_tokens: int = 0          # > 0: stream the chunk's audio as partial results, first piece after n tokens (include/xtts_b200.h)
+    speed: float = 1.0             # speaking rate in [0.25, 4] (xtts_submit_speed; passed beside the struct, which cannot grow)
 
     def c(self) -> XttsSampling:
         s = XttsSampling()
@@ -270,7 +274,8 @@ class NativeEngine:
     def submit(self, seq_id: int, text_ids, speaker_slot: int, sp: Sampling):
         t = _i32(text_ids)
         cs = sp.c()
-        self._chk(self.lib.xtts_submit(self.h, seq_id, _ip(t), t.size, speaker_slot, C.byref(cs)), "submit")
+        self._chk(self.lib.xtts_submit_speed(self.h, seq_id, _ip(t), t.size, speaker_slot, C.byref(cs),
+                                             float(getattr(sp, "speed", 1.0))), "submit")
 
     def cancel(self, seq_id: int):
         self._chk(self.lib.xtts_cancel(self.h, seq_id), "cancel")
@@ -392,6 +397,20 @@ class NativeEngine:
         lat = _f32(latents)
         wav = np.empty((nz * self.dims.voc.hop,), np.float32)
         self._chk(self.lib.xtts_vocode_window(self.h, _fp(lat), lat.shape[0], speaker_slot, z0, nz, _fp(wav)), "vocode_window")
+        return wav
+
+    def vocode_speed(self, latents, speaker_slot: int, speed: float = 1.0, z0: int = 0, nz: int = -1) -> np.ndarray:
+        """The vocoder at a speaking rate (xtts_vocode_speed): the whole chunk (nz < 0) -> n_samples(T, speed) samples, or
+        z-frames [z0, z0 + nz) of the speed-scaled chunk as a window of its own -> nz * hop samples."""
+        lat = _f32(latents)
+        T = lat.shape[0]
+        ok = SPEED_MIN <= speed <= SPEED_MAX                      # (the library rejects anything else)
+        ns = (self.dims.voc.n_samples(T, speed) if ok else 0) if nz < 0 else nz * self.dims.voc.hop
+        wav = np.empty((ns,), np.float32)
+        n_out = C.c_int32(0)
+        self._chk(self.lib.xtts_vocode_speed(self.h, _fp(lat), T, speaker_slot, float(speed), z0, nz, _fp(wav),
+                                             C.byref(n_out)), "vocode_speed")
+        assert n_out.value == ns, (n_out.value, ns)
         return wav
 
     def gpt_prefill(self, text_ids, speaker_slot: int, audio_tokens=(), want_hidden: bool = False):

@@ -5,6 +5,11 @@ Differences, all outside the hot path: language auto-detection uses ``langid`` w
 otherwise falls back to "en" with a warning (the reference hard-requires langid); ``enhance_speech``
 (off by default, requests.py:171; CPU DSP on the reference wav) is not provided: when requested, the original speaker
 files are used and a warning is issued — the reference's own behaviour when its enhancer fails.
+
+Additions (not in the reference): ``seed`` (reproducible sampling) and ``speed``, the speaking rate in [0.25, 4.0] (> 1 is
+faster; the reference offers speed only in its OpenAI server, as a CPU phase vocoder on the finished waveform).  Here it
+time-scales the GPT latents on the GPU before the vocoder, as Coqui's ``Xtts.inference(speed=...)`` does, so the pitch
+stays; the tokens are the same at every speed.
 """
 from __future__ import annotations
 
@@ -13,6 +18,8 @@ import warnings
 from dataclasses import dataclass, field
 from functools import lru_cache
 from typing import AsyncGenerator, Callable, List, Optional, Union
+
+from .config import SPEED_MAX, SPEED_MIN
 
 SUPPORTED_LANGUAGES = ("en", "es", "fr", "de", "it", "pt", "pl", "tr", "ru", "nl", "cs", "ar", "zh-cn", "hu", "ko",
                        "ja", "hi", "auto", "")
@@ -70,10 +77,13 @@ class TTSRequest:
     repetition_penalty: float = 5.0
     length_penalty: float = 1.0     # carried, not consumed by the engine (SURVEY App. A.3)
     do_sample: bool = True          # carried, not consumed by the engine
-    # additions (not in the reference): reproducible sampling
+    # additions (not in the reference): reproducible sampling, speaking rate
     seed: Optional[int] = None
+    speed: float = 1.0
 
     def __post_init__(self):
+        if not (SPEED_MIN <= self.speed <= SPEED_MAX):                 # NaN fails the comparison too
+            raise ValueError(f"speed {self.speed} out of range [{SPEED_MIN}, {SPEED_MAX}]")
         if self.language == "auto" and len(self.text) > 0:
             self.language = get_language(self.text if isinstance(self.text, str) else " ".join(self.text))
         validate_language(self.language)
@@ -93,5 +103,5 @@ class TTSRequest:
         fields = {k: getattr(self, k) for k in (
             "text", "speaker_files", "enhance_speech", "audio_config", "language", "request_id", "load_sample_rate",
             "sound_norm_refs", "max_ref_length", "gpt_cond_len", "gpt_cond_chunk_len", "stream", "temperature", "top_p",
-            "top_k", "repetition_penalty", "length_penalty", "do_sample", "seed")}
+            "top_k", "repetition_penalty", "length_penalty", "do_sample", "seed", "speed")}
         return TTSRequest(**fields)

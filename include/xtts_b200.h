@@ -130,6 +130,16 @@ int xtts_condition(xtts_engine* e, int32_t slot, const float* wav22k, int64_t n2
  * Asynchronous: the scheduler thread admits, prefills, decodes (continuous batching), vocodes. */
 int xtts_submit(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
                 const xtts_sampling* sp);
+/* xtts_submit with a speaking rate (Coqui Xtts.inference(speed=...); xtts_submit = speed 1).  speed in [0.25, 4] (the range
+ * of OpenAI's /v1/audio/speech; > 1 is faster), anything else — NaN included — fails this call with XTTS_ERR_INVALID before
+ * anything is queued.  The GPT decode is untouched (same tokens, same latents); the T latents of the chunk are time-scaled
+ * by one more linear interpolation to T0 = floor(T * ls) frames, ls = 1 / (double)speed, before the vocoder's own two
+ * (F.interpolate(scale_factor = ls, mode "linear")), so the pitch stays.  n_samples = 256 * z_frames(T0); T0 == 0 (e.g. 3
+ * tokens at speed 4) gives a final result with every token and 0 samples.  Speed 1 skips the stage: bit-identical to
+ * xtts_submit (and so does T0 == T, where F.interpolate copies).  Streaming (early_tokens, "voc_segment") works at any
+ * speed; a finished chunk longer than one vocoder window is vocoded in several, none of them a partial result. */
+int xtts_submit_speed(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
+                      const xtts_sampling* sp, float speed);
 /* Aborts a chunk (the reference aborts the vLLM request when its generator is dropped).  A queued chunk is dropped, a
  * decoding one stops at the scheduler's next iteration and returns its batch slot and KV pages; either way exactly one
  * final result with status XTTS_ERR_CANCELLED is delivered.  Unknown / already finished ids are ignored. */
@@ -187,6 +197,13 @@ int xtts_vocode(xtts_engine* e, const float* latents, int32_t T, int32_t speaker
  * Samples further than the generator's receptive field (~14 z-frames) from an inner window edge equal the whole chunk's —
  * the property "voc_segment" / early_tokens rest on (tests/test_gpu_vocoder.py). */
 int xtts_vocode_window(xtts_engine* e, const float* latents, int32_t T, int32_t speaker_slot, int32_t z0, int32_t nz, float* wav);
+/* The vocoder at a speaking rate (speed in [0.25, 4], see xtts_submit_speed): z-frames [z0, z0 + nz) of the speed-scaled
+ * chunk as a window of its own (wav [nz * 256]), or with nz < 0 the whole chunk (wav [256 * z_frames(T0)]).
+ * A whole chunk longer than the vocoder workspace (slow rates: up to 4x the frames) is vocoded in the windows the scheduler
+ * cuts for it, their kept samples stitched — the same samples a submitted chunk gets.  *n_out = samples written (0 when
+ * T0 == 0).  At speed 1: nz < 0 is xtts_vocode, nz >= 0 is xtts_vocode_window, bit for bit. */
+int xtts_vocode_speed(xtts_engine* e, const float* latents, int32_t T, int32_t speaker_slot, float speed, int32_t z0, int32_t nz,
+                      float* wav, int32_t* n_out);
 /* one prefill over [prompt ; forced audio tokens] (the reference's 2nd pass, XTTSv2.py:617-687):
  * outputs ln_f hidden of every row, raw logits + latents of the last n_audio rows */
 int xtts_gpt_prefill(xtts_engine* e, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
