@@ -10,38 +10,6 @@
 namespace xtts {
 namespace {
 
-constexpr double kPi = 3.14159265358979323846;
-
-template <typename T>
-struct Dev {
-    T* p = nullptr; size_t n = 0;
-    ~Dev() { if (p) cudaFree(p); }
-    void alloc(size_t c) { if (p) cudaFree(p); p = nullptr; n = c; if (c) CUDA_CHECK(cudaMalloc(&p, c * sizeof(T))); }
-    void ensure(size_t c) { if (c > n) alloc(c); }
-    void up(const std::vector<T>& h, cudaStream_t st) { alloc(h.size()); CUDA_CHECK(cudaMemcpyAsync(p, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, st)); CUDA_CHECK(cudaStreamSynchronize(st)); }
-};
-
-// ---------------------------------------------------------------------------------------- front-ends
-// F[t][i] = win[i] * xp[t*hop + off + i],  xp = reflect-pad(x, pad)   (torch.stft center=True)
-__global__ void frame_window_kernel(const float* __restrict__ x, int n, const float* __restrict__ win, int wlen, int hop,
-                                    int off, int pad, float* __restrict__ F, int frames) {
-    const int t = blockIdx.x;
-    for (int i = threadIdx.x; i < wlen; i += blockDim.x) {
-        int p = t * hop + off + i - pad;
-        if (p < 0) p = -p;
-        if (p >= n) p = 2 * (n - 1) - p;
-        p = max(0, min(n - 1, p));
-        F[(size_t)t * wlen + i] = win[i] * x[p];
-    }
-}
-// P[t][k] = re^2 + im^2 from D [frames, 2*nb]
-__global__ void power_kernel(const float* __restrict__ D, float* __restrict__ P, int frames, int nb) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= (size_t)frames * nb) return;
-    const int t = (int)(i / nb), k = (int)(i % nb);
-    const float re = D[(size_t)t * 2 * nb + k], im = D[(size_t)t * 2 * nb + nb + k];
-    P[i] = re * re + im * im;
-}
 // mode 0: log(clamp(x,1e-5)) / stats[c]   (utilities.py:66-70);  mode 1: log(x + 1e-6)   (hifigan_decoder.py:616)
 __global__ void mel_log_kernel(float* __restrict__ M, const float* __restrict__ stats, size_t n, int C, int mode) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -221,7 +189,37 @@ __global__ void l2norm_kernel(float* __restrict__ x, int n) {
     for (int i = threadIdx.x; i < n; i += blockDim.x) x[i] /= nrm;
 }
 
-inline int nblk(size_t n, int t = 256) { return (int)((n + t - 1) / t); }
+}  // namespace
+
+// ---------------------------------------------------------------------------------------- STFT front-end (cond.h)
+// F[t][i] = win[i] * xp[t*hop + off + i].  PAD_REFLECT: xp = reflect-pad(x, pad) (torch.stft center=True);
+// PAD_ZERO: xp = zero-pad(nan_to_num(x), pad) (librosa.stft center=True after np.nan_to_num)
+__global__ void frame_window_kernel(const float* __restrict__ x, int n, const float* __restrict__ win, int wlen, int hop,
+                                    int off, int pad, int pad_mode, float* __restrict__ F, int frames) {
+    const int t = blockIdx.x;
+    for (int i = threadIdx.x; i < wlen; i += blockDim.x) {
+        int p = t * hop + off + i - pad;
+        float v;
+        if (pad_mode == PAD_ZERO) {
+            v = (p < 0 || p >= n) ? 0.f : x[p];
+            if (!isfinite(v)) v = 0.f;
+        } else {
+            if (p < 0) p = -p;
+            if (p >= n) p = 2 * (n - 1) - p;
+            p = max(0, min(n - 1, p));
+            v = x[p];
+        }
+        F[(size_t)t * wlen + i] = win[i] * v;
+    }
+}
+// P[t][k] = re^2 + im^2 from D [frames, 2*nb]
+__global__ void power_kernel(const float* __restrict__ D, float* __restrict__ P, int frames, int nb) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (size_t)frames * nb) return;
+    const int t = (int)(i / nb), k = (int)(i % nb);
+    const float re = D[(size_t)t * 2 * nb + k], im = D[(size_t)t * 2 * nb + nb + k];
+    P[i] = re * re + im * im;
+}
 
 std::vector<float> dft_basis(int n_fft, int wlen, int off) {          // [(2*nb)][wlen]: cos rows then -sin rows
     const int nb = n_fft / 2 + 1;
@@ -251,6 +249,8 @@ std::vector<float> mel_fb_t(int n_freqs, double f_min, double f_max, int n_mels,
     }
     return fb;
 }
+
+namespace {
 
 struct Lin { Dev<float> w, b; int N = 0, K = 0; bool has_b = false; };
 struct Bn { Dev<float> scale, shift; };
@@ -410,7 +410,7 @@ void Conditioner::run(const float* wav22k_host, int64_t n22, const float* wav16k
         const int len = (int)pc.second;
         const int T = 1 + len / 256;
         m.F.ensure((size_t)T * 1024); m.D.ensure((size_t)T * 2 * nb22); m.P.ensure((size_t)T * nb22); m.mel.ensure((size_t)T * c.n_mels);
-        frame_window_kernel<<<T, 256, 0, st>>>(m.wav22.p + pc.first, len, m.hann.p, 1024, 256, 512, 1024, m.F.p, T);
+        frame_window_kernel<<<T, 256, 0, st>>>(m.wav22.p + pc.first, len, m.hann.p, 1024, 256, 512, 1024, PAD_REFLECT, m.F.p, T);
         COUNT_LAUNCH(); KERNEL_CHECK();
         launch_gemm_f32(m.F.p, m.basis22.p, nullptr, nullptr, m.D.p, T, 2 * nb22, 1024, 0, st);
         power_kernel<<<nblk((size_t)T * nb22), 256, 0, st>>>(m.D.p, m.P.p, T, nb22); COUNT_LAUNCH(); KERNEL_CHECK();
@@ -477,7 +477,7 @@ void Conditioner::run(const float* wav22k_host, int64_t n22, const float* wav16k
         preemphasis_kernel<<<nblk(N), 256, 0, st>>>(m.wav16.p, m.pre16.p, N, 0.97f); COUNT_LAUNCH(); KERNEL_CHECK();
         const int T = 1 + N / 160, nb = 257, NM = c.spk_mels;
         m.F.ensure((size_t)T * 400); m.D.ensure((size_t)T * 2 * nb); m.P.ensure((size_t)T * nb); m.mel.ensure((size_t)T * NM);
-        frame_window_kernel<<<T, 128, 0, st>>>(m.pre16.p, N, m.hamm.p, 400, 160, 56, 256, m.F.p, T); COUNT_LAUNCH(); KERNEL_CHECK();
+        frame_window_kernel<<<T, 128, 0, st>>>(m.pre16.p, N, m.hamm.p, 400, 160, 56, 256, PAD_REFLECT, m.F.p, T); COUNT_LAUNCH(); KERNEL_CHECK();
         launch_gemm_f32(m.F.p, m.basis16.p, nullptr, nullptr, m.D.p, T, 2 * nb, 400, 0, st);
         power_kernel<<<nblk((size_t)T * nb), 256, 0, st>>>(m.D.p, m.P.p, T, nb); COUNT_LAUNCH(); KERNEL_CHECK();
         launch_gemm_f32(m.P.p, m.fb16.p, nullptr, nullptr, m.mel.p, T, NM, nb, 0, st);

@@ -157,6 +157,7 @@ public:
     void set_speaker(int slot, const float* cond, const float* g);
     void get_speaker(int slot, float* cond, float* g);
     void condition(int slot, const float* w22, int64_t n22, const float* w16, int64_t n16, int cond_len, int chunk_len);
+    int64_t enhance(const float* wav, int64_t n, const xtts_enhance_config& c, float* out, int64_t cap);
     void submit(uint64_t id, const int32_t* text, int n_text, int speaker, const xtts_sampling& sp, float speed);
     void cancel(uint64_t id);
     int poll(xtts_result* out, int timeout_ms);
@@ -232,6 +233,7 @@ private:
     std::vector<std::unique_ptr<CondLin>> conds;
     uint64_t weight_bytes = 0;
     std::unique_ptr<Conditioner> conditioner;
+    std::unique_ptr<Enhancer> enhancer;          // built on the first xtts_enhance
 
     // ---- speakers
     DBuf<float> spk_cond, spk_g, spk_cbias;
@@ -836,6 +838,17 @@ void Engine::condition(int slot, const float* w22, int64_t n22, const float* w16
                      spk_g.p + (size_t)slot * cfg.d_vector);
     finish_speaker(slot);
     st_cond_ms += (now_s() - t0) * 1e3;
+}
+
+// TTSRequest.enhance_speech (requests.py:199-248): the reference's audio enhancer, on the conditioning stream
+int64_t Engine::enhance(const float* wav, int64_t n, const xtts_enhance_config& c, float* out, int64_t cap) {
+    ApiLock lk(this);
+    CUDA_CHECK(cudaSetDevice(cfg.device));
+    const double t0 = now_s();
+    if (!enhancer) enhancer.reset(new Enhancer(st));
+    const int64_t n_out = enhancer->run(wav, n, c, out, cap);
+    st_cond_ms += (now_s() - t0) * 1e3;
+    return n_out;
 }
 
 void Engine::get_speaker(int slot, float* cond, float* g) {
@@ -2592,6 +2605,12 @@ int xtts_get_speaker(xtts_engine* e, int32_t slot, float* cond, float* g) { XTTS
 int xtts_condition(xtts_engine* e, int32_t slot, const float* wav22k, int64_t n22, const float* wav16k, int64_t n16,
                    int32_t gpt_cond_len_s, int32_t gpt_cond_chunk_len_s) {
     XTTS_TRY(e->impl->condition(slot, wav22k, n22, wav16k, n16, gpt_cond_len_s, gpt_cond_chunk_len_s))
+}
+int xtts_enhance(xtts_engine* e, const float* wav, int64_t n, const xtts_enhance_config* cfg, float* out, int64_t cap,
+                 int64_t* n_out) {
+    if (!cfg || !n_out) { xtts::set_error("null argument"); return XTTS_ERR_INVALID; }
+    *n_out = xtts::Enhancer::out_len(n, *cfg);
+    XTTS_TRY(*n_out = e->impl->enhance(wav, n, *cfg, out, cap))
 }
 int xtts_submit(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
                 const xtts_sampling* sp) {

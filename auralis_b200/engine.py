@@ -18,6 +18,7 @@ import asyncio
 import hashlib
 import threading
 import time
+from dataclasses import asdict
 from pathlib import Path
 from typing import AsyncGenerator, Dict, List, Optional, Tuple, Union
 
@@ -207,9 +208,14 @@ class XTTSv2Engine(BaseAsyncTTSEngine):
                 await asyncio.sleep(0.005)
 
     async def get_audio_conditioning(self, audio_reference, max_ref_length=30, gpt_cond_len=6, gpt_cond_chunk_len=6,
-                                     librosa_trim_db=None, sound_norm_refs=False, load_sr=22050):
+                                     librosa_trim_db=None, sound_norm_refs=False, load_sr=22050, enhance=None):
         """XTTSv2.py:409-468,579-615: -> (gpt_cond_latents [1,32,H], speaker_embedding [1,d,1]) computed on the GPU
-        by ``xtts_condition`` and cached per reference (the per-speaker cache of SURVEY §3.4)."""
+        by ``xtts_condition`` and cached per reference (the per-speaker cache of SURVEY §3.4).
+
+        `enhance` (an AudioPreprocessingConfig): each file is first enhanced on the GPU (``xtts_enhance``, the reference's
+        TTSRequest.preprocess_audio, requests.py:214-247): loaded at ``enhance.sample_rate``, enhanced, quantised to 16
+        bits as the reference's temporary WAV is, then resampled to `load_sr`.  A file the enhancer rejects
+        (XTTS_ERR_INVALID: too short, non-finite result) is used as it is, with a RuntimeWarning."""
         if not isinstance(audio_reference, (bytes, str, Path, list)):
             raise AssertionError(f"audio_reference must be a string, byte or a list but it is {type(audio_reference)}")
         paths = audio_reference if isinstance(audio_reference, list) else [audio_reference]
@@ -225,6 +231,8 @@ class XTTSv2Engine(BaseAsyncTTSEngine):
                 except OSError:
                     hk.update(str(p).encode())
         hk.update(f"{max_ref_length}|{gpt_cond_len}|{gpt_cond_chunk_len}|{sound_norm_refs}|{load_sr}".encode())
+        if enhance is not None:
+            hk.update(f"|enhance|{sorted(asdict(enhance).items())}".encode())
         key = hk.hexdigest()
         cached = self._spk_arrays.get(key)
         if cached is not None:
@@ -238,7 +246,8 @@ class XTTSv2Engine(BaseAsyncTTSEngine):
                 def work():
                     audios22 = []
                     for p in paths:
-                        a = load_audio(p, load_sr)[: load_sr * max_ref_length]
+                        a = self._enhanced(p, enhance, load_sr) if enhance is not None else load_audio(p, load_sr)
+                        a = a[: load_sr * max_ref_length]
                         if sound_norm_refs:
                             a = (a / np.abs(a).max()) * 0.75
                         audios22.append(a)
@@ -278,6 +287,18 @@ class XTTSv2Engine(BaseAsyncTTSEngine):
             self._spk_arrays.pop(next(iter(self._spk_arrays)))
         self._spk_arrays[key] = pair
         return pair
+
+    def _enhanced(self, source, cfg, load_sr: int) -> np.ndarray:
+        """`source` at `load_sr` after the GPU enhancer; the original audio when the enhancer rejects it."""
+        import warnings
+        try:
+            a = self.native.enhance(load_audio(source, cfg.sample_rate), cfg)
+        except native.NativeError as e:
+            if e.code != native.ERR_INVALID:
+                raise
+            warnings.warn(f"enhance_speech: {e}; using the original speaker file", RuntimeWarning, stacklevel=2)
+            return load_audio(source, load_sr)
+        return np.clip(_resample(a, cfg.sample_rate, load_sr), -1.0, 1.0).astype(np.float32)     # as load_audio leaves it
 
     def register_speaker(self, cond_latents: np.ndarray, d_vector: np.ndarray, dev: int = 0) -> Tuple["_SpeakerArray", "_SpeakerArray"]:
         """Pre-computed conditioning (the pair `prepare_for_streaming_generation` hands back, tts.py:91-105) uploaded to
@@ -323,8 +344,10 @@ class XTTSv2Engine(BaseAsyncTTSEngine):
 
     async def get_generation_context(self, request: TTSRequest, gpt_cond_latent=None, speaker_embeddings=None):
         if gpt_cond_latent is None or speaker_embeddings is None:
+            enh = request.enhance_config() if hasattr(request, "enhance_config") else None
             gpt_cond_latent, speaker_embeddings = await self.get_audio_conditioning(
-                request.speaker_files, request.max_ref_length, request.gpt_cond_len, request.gpt_cond_chunk_len)
+                request.speaker_files, request.max_ref_length, request.gpt_cond_len, request.gpt_cond_chunk_len,
+                **({"enhance": enh} if enh is not None else {}))
         token_lists = self.prepare_text_tokens(request.text, request.language)
         generators, request_ids = [], []
         base_seed = request.seed if getattr(request, "seed", None) is not None else int.from_bytes(hashlib.sha256(request.request_id.encode()).digest()[:6], "little")

@@ -21,11 +21,14 @@ LIB_PATH = os.path.join(_HERE, "libxtts_b200.so")
 PRECISION_FP32 = 0
 PRECISION_BF16 = 1
 PRECISION_FP16 = 2
+ERR_INVALID = -1
 ERR_CANCELLED = -5
 
 
 class NativeError(RuntimeError):
-    pass
+    def __init__(self, msg: str, code: int = 0):
+        super().__init__(msg)
+        self.code = code            # the XTTS_ERR_* the call returned (0 when not from a call)
 
 
 class XttsConfig(C.Structure):
@@ -66,6 +69,22 @@ class XttsStats(C.Structure):
                 ("hbm_bytes_weights", C.c_uint64)]
 
 
+class XttsEnhanceConfig(C.Structure):
+    _fields_ = [("sample_rate", C.c_int32), ("normalize", C.c_int32), ("trim_silence", C.c_int32),
+                ("remove_noise", C.c_int32), ("enhance_speech", C.c_int32), ("vad_frame_length", C.c_int32),
+                ("noise_reduce_frames", C.c_int32), ("vad_threshold", C.c_float), ("noise_reduce_margin", C.c_float),
+                ("enhance_amount", C.c_float), ("target_lufs", C.c_float)]
+
+    @classmethod
+    def of(cls, cfg) -> "XttsEnhanceConfig":
+        """From any object with the AudioPreprocessingConfig field names (requests.py)."""
+        c = cls()
+        for name, typ in cls._fields_:
+            v = getattr(cfg, name)
+            setattr(c, name, float(v) if typ is C.c_float else int(v))
+        return c
+
+
 class XttsKernelProfile(C.Structure):
     _fields_ = [("n", C.c_int32), ("name", (C.c_char * 32) * 16), ("ms", C.c_double * 16), ("flops", C.c_double * 16),
                 ("bytes", C.c_double * 16), ("launches", C.c_uint64 * 16)]
@@ -74,7 +93,7 @@ class XttsKernelProfile(C.Structure):
 # every symbol include/xtts_b200.h declares (checked by tests/test_abi.py against the header text)
 ABI_SYMBOLS = [
     "xtts_last_error", "xtts_version", "xtts_create", "xtts_destroy", "xtts_load_weight", "xtts_finalize_weights",
-    "xtts_set_speaker", "xtts_get_speaker", "xtts_condition", "xtts_submit", "xtts_submit_speed", "xtts_cancel", "xtts_poll",
+    "xtts_set_speaker", "xtts_get_speaker", "xtts_condition", "xtts_enhance", "xtts_submit", "xtts_submit_speed", "xtts_cancel", "xtts_poll",
     "xtts_fetch", "xtts_set_option", "xtts_get_stats", "xtts_sync", "xtts_get_kernel_profile", "xtts_device_timer", "xtts_vocode",
     "xtts_vocode_window", "xtts_vocode_speed", "xtts_gpt_prefill", "xtts_gpt_teacher_forced",
     "xtts_debug_gemm", "xtts_debug_sample_slots", "xtts_debug_trace",
@@ -103,6 +122,7 @@ def load_library(path: Optional[str] = None):
     lib.xtts_set_speaker.argtypes = [vp, i32, f32p, f32p]
     lib.xtts_get_speaker.argtypes = [vp, i32, f32p, f32p]
     lib.xtts_condition.argtypes = [vp, i32, f32p, i64, f32p, i64, i32, i32]
+    lib.xtts_enhance.argtypes = [vp, f32p, i64, C.POINTER(XttsEnhanceConfig), f32p, i64, C.POINTER(i64)]
     lib.xtts_submit.argtypes = [vp, C.c_uint64, i32p, i32, i32, C.POINTER(XttsSampling)]
     lib.xtts_submit_speed.argtypes = [vp, C.c_uint64, i32p, i32, i32, C.POINTER(XttsSampling), C.c_float]
     lib.xtts_cancel.argtypes = [vp, C.c_uint64]
@@ -229,7 +249,7 @@ class NativeEngine:
 
     def _chk(self, rc: int, what: str):
         if rc != 0:
-            raise NativeError(f"{what} failed ({rc}): {self.lib.xtts_last_error().decode()}")
+            raise NativeError(f"{what} failed ({rc}): {self.lib.xtts_last_error().decode()}", rc)
 
     def close(self):
         if getattr(self, "h", None):
@@ -269,6 +289,17 @@ class NativeEngine:
         a, b = _f32(wav22k).reshape(-1), _f32(wav16k).reshape(-1)
         self._chk(self.lib.xtts_condition(self.h, slot, _fp(a), a.size, _fp(b), b.size, gpt_cond_len, gpt_cond_chunk_len),
                   "condition")
+
+    def enhance(self, wav, cfg) -> np.ndarray:
+        """xtts_enhance: the reference's speaker-file enhancer (VAD trim, spectral gating, clarity, loudness) and its
+        16-bit write/read, on the GPU.  `wav` is mono at `cfg.sample_rate`; `cfg` has AudioPreprocessingConfig's
+        fields.  Raises NativeError with code ERR_INVALID where the reference's enhancer would fail."""
+        a = _f32(wav).reshape(-1)
+        out = np.empty((a.size,), np.float32)
+        n_out = C.c_int64(0)
+        self._chk(self.lib.xtts_enhance(self.h, _fp(a), a.size, C.byref(XttsEnhanceConfig.of(cfg)), _fp(out), out.size,
+                                        C.byref(n_out)), "enhance")
+        return out[: n_out.value]
 
     # ---- generation
     def submit(self, seq_id: int, text_ids, speaker_slot: int, sp: Sampling):

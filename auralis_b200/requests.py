@@ -2,9 +2,16 @@
 (`/root/reference/src/auralis/common/definitions/requests.py:135-204`).
 
 Differences, all outside the hot path: language auto-detection uses ``langid`` when it is installed and
-otherwise falls back to "en" with a warning (the reference hard-requires langid); ``enhance_speech``
-(off by default, requests.py:171; CPU DSP on the reference wav) is not provided: when requested, the original speaker
-files are used and a warning is issued — the reference's own behaviour when its enhancer fails.
+otherwise falls back to "en" with a warning (the reference hard-requires langid).
+
+``enhance_speech`` (off by default) cleans the speaker references before conditioning, as the reference's
+``EnhancedAudioProcessor`` does (enhancer.py:34-153: VAD trim, spectral gating, clarity shaping, loudness normalisation,
+each behind its ``audio_config`` flag), but on the GPU (``xtts_enhance``) and only when ``speaker_files`` is a list,
+like the reference.  Where the reference would fail (audio too short for a VAD frame or a 400 ms loudness block, a
+non-finite result) the original file is used, with a warning.  Unlike the reference, ``speaker_files`` is not rewritten to
+enhanced temporary files: the request keeps its paths, and the engine enhances while it conditions (the speaker cache
+key includes ``audio_config``).  The audio is loaded at ``audio_config.sample_rate`` with torchaudio's sinc resampler,
+not librosa's soxr.
 
 Additions (not in the reference): ``seed`` (reproducible sampling) and ``speed``, the speaking rate in [0.25, 4.0] (> 1 is
 faster; the reference offers speed only in its OpenAI server, as a CPU phase vocoder on the finished waveform).  Here it
@@ -45,12 +52,23 @@ def validate_language(language: str) -> str:
 
 @dataclass
 class AudioPreprocessingConfig:
-    """Placeholder with the reference's field names (enhancer.py:12-31); only carried, never applied here."""
+    """The reference's speaker-file enhancement settings (enhancer.py:12-31), same fields and defaults; applied by
+    ``xtts_enhance`` when a request sets ``enhance_speech``."""
     sample_rate: int = 22050
     normalize: bool = True
     trim_silence: bool = True
     remove_noise: bool = True
     enhance_speech: bool = True
+    # VAD
+    vad_threshold: float = 0.02
+    vad_frame_length: int = 1024 * 4
+    # noise reduction
+    noise_reduce_margin: float = 1.0
+    noise_reduce_frames: int = 25
+    # clarity
+    enhance_amount: float = 1.0
+    # loudness target
+    target_lufs: float = -18.0
 
 
 @dataclass
@@ -87,12 +105,10 @@ class TTSRequest:
         if self.language == "auto" and len(self.text) > 0:
             self.language = get_language(self.text if isinstance(self.text, str) else " ".join(self.text))
         validate_language(self.language)
-        if self.enhance_speech and isinstance(self.speaker_files, list):
-            # requests.py:199-203 + 214-247: the reference cleans the reference audio on the CPU (librosa / pyloudnorm) and
-            # falls back to the original file when that fails.  That DSP is outside the hot path and not provided here:
-            # same fallback, said once.
-            warnings.warn("enhance_speech: reference-audio enhancement is not provided, the original speaker files are used",
-                          RuntimeWarning, stacklevel=2)
+
+    def enhance_config(self) -> Optional[AudioPreprocessingConfig]:
+        """`audio_config` when the speaker files are to be enhanced (requests.py:199-203: a list and enhance_speech)."""
+        return self.audio_config if self.enhance_speech and isinstance(self.speaker_files, list) else None
 
     def infer_language(self):
         if self.language == "auto":

@@ -62,7 +62,9 @@ class TTS:
         """tts.py:91-105."""
         cc = self.tts_engine.conditioning_config
         if cc.speaker_embeddings or cc.gpt_like_decoder_conditioning:
-            gpt_cond_latent, speaker_embeddings = await self.tts_engine.get_audio_conditioning(request.speaker_files)
+            enh = request.enhance_config()
+            gpt_cond_latent, speaker_embeddings = await self.tts_engine.get_audio_conditioning(
+                request.speaker_files, **({"enhance": enh} if enh is not None else {}))
             return partial(self.tts_engine.get_generation_context, gpt_cond_latent=gpt_cond_latent,
                            speaker_embeddings=speaker_embeddings)
 

@@ -126,6 +126,24 @@ int xtts_get_speaker(xtts_engine* e, int32_t slot, float* cond_latents, float* d
 int xtts_condition(xtts_engine* e, int32_t slot, const float* wav22k, int64_t n22, const float* wav16k, int64_t n16,
                    int32_t gpt_cond_len_s, int32_t gpt_cond_chunk_len_s);
 
+/* TTSRequest.enhance_speech (requests.py:199-248, enhancer.py:12-153): the reference's AudioPreprocessingConfig.
+ * Flags are 0 / non-zero; the stages run in this order: trim_silence (VAD), remove_noise (spectral gating),
+ * enhance_speech (clarity shaping), normalize (BS.1770 loudness to target_lufs, tanh soft clip). */
+typedef struct xtts_enhance_config {
+    int32_t sample_rate;
+    int32_t normalize, trim_silence, remove_noise, enhance_speech;
+    int32_t vad_frame_length, noise_reduce_frames;
+    float vad_threshold, noise_reduce_margin, enhance_amount, target_lufs;
+} xtts_enhance_config;
+/* EnhancedAudioProcessor.process on the GPU, then the 16-bit PCM write/read of the reference's temp file
+ * (rint(x * 32767) / 32768).  wav: n mono samples at cfg->sample_rate.  Writes *n_out samples to out (n_out <= n:
+ * gating and clarity drop the tail past a multiple of 512); cap < *n_out fails with *n_out set.  Returns
+ * XTTS_ERR_INVALID for a bad config and where the reference's enhancer fails: non-finite input, n < vad_frame_length
+ * (or n <= 1024) with trim_silence, fewer than 0.4 s of audio at the loudness stage, a non-finite result.
+ * Runs on the conditioning stream; its time counts in xtts_stats.cond_ms. */
+int xtts_enhance(xtts_engine* e, const float* wav, int64_t n, const xtts_enhance_config* cfg, float* out, int64_t cap,
+                 int64_t* n_out);
+
 /* llm_engine.generate(...) per text chunk (XTTSv2.py:741-757): text_ids = [bos]+bpe+[eos] (XTTSv2.py:519-522).
  * Asynchronous: the scheduler thread admits, prefills, decodes (continuous batching), vocodes. */
 int xtts_submit(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
