@@ -39,6 +39,15 @@ std::vector<float> dft_basis(int n_fft, int wlen, int off);
 // torchaudio.functional.melscale_fbanks (htk mel scale; slaney-normalised when `slaney`), as [n_mels][n_freqs]
 std::vector<float> mel_fb_t(int n_freqs, double f_min, double f_max, int n_mels, int sr, bool slaney);
 
+// ---- librosa's iSTFT at n_fft 2048, hop 512 (enhance.cu), shared by the enhancer and the phase vocoder (pvoc.cu)
+// Periodic Hann window, its square, and irfft x window as an NT GEMM operand [2048][re 1025 | im 1025].
+void stft_tables(std::vector<float>& hann, std::vector<float>& win2, std::vector<float>& ibasis);
+// y[s] = overlap-add sample m = m0 + s of frames 0 .. T-1 (windowed, [.][2048], frame t in row t - t_base), divided by
+// the squared-window sum where that exceeds float32 tiny; m0 = 1024 drops librosa's centring pad.  Frames in ascending
+// order, so a sample's sum does not depend on which rows hold its frames.
+__global__ void ola_kernel(const float* __restrict__ Y, int t_base, int T, const float* __restrict__ win2,
+                           float* __restrict__ y, int64_t m0, int64_t ns);
+
 struct HostTensorView {
     const float* data;
     std::vector<int64_t> shape;
@@ -73,6 +82,25 @@ public:
     // wav: host, n samples at c.sample_rate.  Writes out_len(n, c) samples to `out` (host).  Throws std::invalid_argument
     // for a bad config and where the reference's enhancer raises (too short, non-finite input or result).
     int64_t run(const float* wav, int64_t n, const xtts_enhance_config& c, float* out, int64_t cap);
+
+private:
+    struct Impl;
+    std::unique_ptr<Impl> impl;
+};
+
+// Phase vocoder (pvoc.cu): the reference's TTSOutput.change_speed — librosa.stft (n_fft 2048, hop 512),
+// librosa.phase_vocoder, librosa.istft, librosa.util.normalize(norm=inf) — on the GPU.  Needs no weights.  Works in
+// blocks of at most `block_frames` output frames, so its spectral workspace does not grow with the input.
+class PhaseVocoder {
+public:
+    explicit PhaseVocoder(cudaStream_t st);
+    ~PhaseVocoder();
+    // Output length for n input samples at `rate` (> 0, finite): 512 * (ceil((1 + n / 512) / rate) - 1).
+    static int64_t out_len(int64_t n, double rate);
+    // wav: host, n samples.  Writes out_len(n, rate) samples to `out` (host).  Throws std::invalid_argument where the
+    // reference raises (rate not finite or <= 0, a non-finite sample, an empty or non-finite result) or cap is too small.
+    // The result does not depend on block_frames.
+    int64_t run(const float* wav, int64_t n, double rate, float* out, int64_t cap, int block_frames);
 
 private:
     struct Impl;

@@ -158,6 +158,7 @@ public:
     void get_speaker(int slot, float* cond, float* g);
     void condition(int slot, const float* w22, int64_t n22, const float* w16, int64_t n16, int cond_len, int chunk_len);
     int64_t enhance(const float* wav, int64_t n, const xtts_enhance_config& c, float* out, int64_t cap);
+    int64_t change_speed(const float* wav, int64_t n, double rate, float* out, int64_t cap);
     void submit(uint64_t id, const int32_t* text, int n_text, int speaker, const xtts_sampling& sp, float speed);
     void cancel(uint64_t id);
     int poll(xtts_result* out, int timeout_ms);
@@ -234,6 +235,8 @@ private:
     uint64_t weight_bytes = 0;
     std::unique_ptr<Conditioner> conditioner;
     std::unique_ptr<Enhancer> enhancer;          // built on the first xtts_enhance
+    std::unique_ptr<PhaseVocoder> pvoc;          // built on the first xtts_change_speed
+    int pvoc_block_frames = 4096;                // option "pvoc_block_frames"
 
     // ---- speakers
     DBuf<float> spk_cond, spk_g, spk_cbias;
@@ -847,6 +850,17 @@ int64_t Engine::enhance(const float* wav, int64_t n, const xtts_enhance_config& 
     const double t0 = now_s();
     if (!enhancer) enhancer.reset(new Enhancer(st));
     const int64_t n_out = enhancer->run(wav, n, c, out, cap);
+    st_cond_ms += (now_s() - t0) * 1e3;
+    return n_out;
+}
+
+// TTSOutput.change_speed (output.py:40-92): the reference's phase-vocoder time stretch, on the conditioning stream
+int64_t Engine::change_speed(const float* wav, int64_t n, double rate, float* out, int64_t cap) {
+    ApiLock lk(this);
+    CUDA_CHECK(cudaSetDevice(cfg.device));
+    const double t0 = now_s();
+    if (!pvoc) pvoc.reset(new PhaseVocoder(st));
+    const int64_t n_out = pvoc->run(wav, n, rate, out, cap, pvoc_block_frames);
     st_cond_ms += (now_s() - t0) * 1e3;
     return n_out;
 }
@@ -1964,6 +1978,10 @@ void Engine::set_option(const std::string& k, int64_t v) {
     else if (k == "voc_segment") voc_segment = (int)std::max<int64_t>(0, v);
     else if (k == "voc_sms") voc_sms = (int)std::max<int64_t>(0, v);
     else if (k == "tc_epilogue") g_conv_tc_epilogue = v ? 1 : 0;
+    else if (k == "pvoc_block_frames") {
+        if (v < 1 || v > (1 << 20)) throw std::runtime_error("pvoc_block_frames: 1 .. 2^20 output frames");
+        pvoc_block_frames = (int)v;
+    }
     else if (k == "voc_batch") voc_max_items = (int)std::max<int64_t>(1, std::min<int64_t>(v, kVocMaxItems));
     else if (k == "gemm_wide") {                                  // 0 off, else the wide kernel's ring depth
         if (v != 0 && (v < 2 || v > 4)) throw std::runtime_error("gemm_wide: 0 (off) or a ring depth of 2, 3 or 4");
@@ -2611,6 +2629,11 @@ int xtts_enhance(xtts_engine* e, const float* wav, int64_t n, const xtts_enhance
     if (!cfg || !n_out) { xtts::set_error("null argument"); return XTTS_ERR_INVALID; }
     *n_out = xtts::Enhancer::out_len(n, *cfg);
     XTTS_TRY(*n_out = e->impl->enhance(wav, n, *cfg, out, cap))
+}
+int xtts_change_speed(xtts_engine* e, const float* wav, int64_t n, double rate, float* out, int64_t cap, int64_t* n_out) {
+    if (!n_out) { xtts::set_error("null argument"); return XTTS_ERR_INVALID; }
+    *n_out = xtts::PhaseVocoder::out_len(n, rate);
+    XTTS_TRY(*n_out = e->impl->change_speed(wav, n, rate, out, cap))
 }
 int xtts_submit(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
                 const xtts_sampling* sp) {

@@ -176,25 +176,6 @@ __global__ void spec_scale_kernel(float* __restrict__ D, int T, const float* __r
     if (gain) g *= gain[k];
     *re *= g; *im *= g;
 }
-// librosa.istft's overlap-add, gathered per output sample (no atomics): frames Y [T][2048] are already windowed
-// (the inverse basis carries the window); divide by the squared-window sum where it exceeds float32 tiny; drop
-// n_fft/2 samples at each end.  Frames are summed in ascending order, as librosa accumulates them.
-__global__ void ola_kernel(const float* __restrict__ Y, int T, const float* __restrict__ win2, float* __restrict__ y,
-                           int64_t nout) {
-    const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= nout) return;
-    const int64_t m = s + kFft / 2;
-    const int t_hi = (int)(m / kHop < T - 1 ? m / kHop : T - 1);
-    const int t_lo = m >= kFft ? (int)((m - kFft) / kHop + 1) : 0;      // frames t with t*hop <= m < t*hop + n_fft
-    float acc = 0.f, wss = 0.f;
-    for (int t = t_lo; t <= t_hi; ++t) {
-        const int i = (int)(m - (int64_t)t * kHop);
-        acc += Y[(size_t)t * kFft + i];
-        wss += win2[i];
-    }
-    y[s] = wss > FLT_MIN ? acc / wss : acc;
-}
-
 // ---------------------------------------------------------------------------------------------------- loudness
 // K-weighting = two transposed-direct-form-II biquads (scipy.signal.lfilter), fp64.  State (z0, z1, w0, w1).
 struct KCoef { double b[3], a[3], c[3], d[3]; };
@@ -342,6 +323,44 @@ void invalid(const std::string& s) { throw std::invalid_argument("enhance: " + s
 
 }  // namespace
 
+// ---------------------------------------------------------------------------------------------------- iSTFT (cond.h)
+// librosa.istft's overlap-add, gathered per output sample (no atomics): frames are already windowed (the inverse basis
+// carries the window); divide by the squared-window sum where it exceeds float32 tiny.  Frames are summed in ascending
+// order, as librosa accumulates them.
+__global__ void ola_kernel(const float* __restrict__ Y, int t_base, int T, const float* __restrict__ win2,
+                           float* __restrict__ y, int64_t m0, int64_t ns) {
+    const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= ns) return;
+    const int64_t m = m0 + s;
+    const int t_hi = (int)(m / kHop < T - 1 ? m / kHop : T - 1);
+    const int t_lo = m >= kFft ? (int)((m - kFft) / kHop + 1) : 0;      // frames t with t*hop <= m < t*hop + n_fft
+    float acc = 0.f, wss = 0.f;
+    for (int t = t_lo; t <= t_hi; ++t) {
+        const int i = (int)(m - (int64_t)t * kHop);
+        acc += Y[(size_t)(t - t_base) * kFft + i];
+        wss += win2[i];
+    }
+    y[s] = wss > FLT_MIN ? acc / wss : acc;
+}
+
+void stft_tables(std::vector<float>& hann, std::vector<float>& win2, std::vector<float>& ibasis) {
+    hann.resize(kFft); win2.resize(kFft);
+    std::vector<double> wd(kFft);
+    for (int i = 0; i < kFft; ++i) {
+        wd[i] = 0.5 - 0.5 * std::cos(2.0 * kPi * i / kFft);         // periodic Hann
+        hann[i] = (float)wd[i]; win2[i] = (float)(wd[i] * wd[i]);
+    }
+    // irfft x window as an NT GEMM operand [2048][re 1025 | im 1025]: (1/N) c_k (Re cos - Im sin), c_k = 1 at DC
+    // and Nyquist (whose imaginary parts irfft ignores), 2 elsewhere
+    ibasis.assign((size_t)kFft * 2 * kBins, 0.f);
+    for (int i = 0; i < kFft; ++i)
+        for (int k = 0; k < kBins; ++k) {
+            const double a = 2.0 * kPi * (double)k * (double)i / kFft, ck = (k == 0 || k == kFft / 2) ? 1.0 : 2.0;
+            ibasis[(size_t)i * 2 * kBins + k] = (float)(wd[i] * ck * std::cos(a) / kFft);
+            ibasis[(size_t)i * 2 * kBins + kBins + k] = (k == 0 || k == kFft / 2) ? 0.f : (float)(-wd[i] * ck * std::sin(a) / kFft);
+        }
+}
+
 struct Enhancer::Impl {
     cudaStream_t st;
     Dev<float> hann, win2, basis, ibasis, gain, x, y, F, D, P, mel, magT, noise, energy, lsum;
@@ -353,23 +372,10 @@ struct Enhancer::Impl {
 
     void lazy_init() {
         if (basis.p) return;
-        std::vector<float> w(kFft), w2(kFft);
-        std::vector<double> wd(kFft);
-        for (int i = 0; i < kFft; ++i) {
-            wd[i] = 0.5 - 0.5 * std::cos(2.0 * kPi * i / kFft);         // periodic Hann
-            w[i] = (float)wd[i]; w2[i] = (float)(wd[i] * wd[i]);
-        }
+        std::vector<float> w, w2, ib;
+        stft_tables(w, w2, ib);
         hann.up(w, st); win2.up(w2, st);
         basis.up(dft_basis(kFft, kFft, 0), st);
-        // irfft x window as an NT GEMM operand [2048][re 1025 | im 1025]: (1/N) c_k (Re cos - Im sin), c_k = 1 at DC
-        // and Nyquist (whose imaginary parts irfft ignores), 2 elsewhere
-        std::vector<float> ib((size_t)kFft * 2 * kBins);
-        for (int i = 0; i < kFft; ++i)
-            for (int k = 0; k < kBins; ++k) {
-                const double a = 2.0 * kPi * (double)k * (double)i / kFft, ck = (k == 0 || k == kFft / 2) ? 1.0 : 2.0;
-                ib[(size_t)i * 2 * kBins + k] = (float)(wd[i] * ck * std::cos(a) / kFft);
-                ib[(size_t)i * 2 * kBins + kBins + k] = (k == 0 || k == kFft / 2) ? 0.f : (float)(-wd[i] * ck * std::sin(a) / kFft);
-            }
         ibasis.up(ib, st);
         ordmax.alloc(2); bad.alloc(1); lres.alloc(2); noise.alloc(kBins); gain.alloc(kBins); kp.alloc(16 * kScanLevels);
     }
@@ -386,7 +392,7 @@ struct Enhancer::Impl {
     void istft(int T, float* ys) {
         launch_gemm_f32(D.p, ibasis.p, nullptr, nullptr, F.p, T, kFft, 2 * kBins, 0, st);
         const int64_t nout = (int64_t)kHop * (T - 1);
-        if (nout > 0) { ola_kernel<<<nblk((size_t)nout), 256, 0, st>>>(F.p, T, win2.p, ys, nout); COUNT_LAUNCH(); KERNEL_CHECK(); }
+        if (nout > 0) { ola_kernel<<<nblk((size_t)nout), 256, 0, st>>>(F.p, 0, T, win2.p, ys, kFft / 2, nout); COUNT_LAUNCH(); KERNEL_CHECK(); }
     }
     void vad(const float* xs, int64_t N, const xtts_enhance_config& c, float* ys) {
         const int fl = c.vad_frame_length, fh = fl / 2;

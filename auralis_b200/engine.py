@@ -27,6 +27,7 @@ import numpy as np
 from . import native
 from .base import BaseAsyncTTSEngine, ConditioningConfig, register_model
 from .config import XTTSDims
+from . import output as _output
 from .output import TTSOutput
 from .requests import TTSRequest
 from .speakers import SpeakerSlots, SpeakerSlotsFull
@@ -151,6 +152,7 @@ class XTTSv2Engine(BaseAsyncTTSEngine):
         self._pollers = [threading.Thread(target=self._poll_loop, args=(i,), name=f"xtts-poll-{i}", daemon=True)
                          for i in range(len(self.natives))]
         [t.start() for t in self._pollers]
+        _output.register_gpu_provider(self)             # TTSOutput.change_speed runs here while this engine lives
 
     # ---- plugin API -------------------------------------------------------------------------
     @classmethod
@@ -460,7 +462,19 @@ class XTTSv2Engine(BaseAsyncTTSEngine):
                 tot[k] = tot.get(k, 0) + getattr(st, k)
         return tot
 
+    def change_speed(self, array, speed_factor: float) -> np.ndarray:
+        """`TTSOutput.change_speed` on the first GPU (``xtts_change_speed``): the reference's librosa phase-vocoder time
+        stretch (> 1 faster) and peak normalisation.  A factor or an input the reference would reject (not finite or
+        <= 0, a non-finite sample, a factor that leaves one STFT frame) raises ValueError."""
+        try:
+            return self.native.change_speed(np.asarray(array, np.float32), float(speed_factor))
+        except native.NativeError as e:
+            if e.code == native.ERR_INVALID:
+                raise ValueError(str(e)) from e
+            raise
+
     async def shutdown(self):
+        _output.unregister_gpu_provider(self)
         self._stop = True
         for t in getattr(self, "_pollers", []):
             t.join(timeout=5)

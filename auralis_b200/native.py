@@ -7,6 +7,7 @@ The library is CUDA-only; creating an engine without an sm_90 GPU raises ``Nativ
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 from dataclasses import dataclass
 from typing import Dict, Optional, Tuple
@@ -93,7 +94,7 @@ class XttsKernelProfile(C.Structure):
 # every symbol include/xtts_b200.h declares (checked by tests/test_abi.py against the header text)
 ABI_SYMBOLS = [
     "xtts_last_error", "xtts_version", "xtts_create", "xtts_destroy", "xtts_load_weight", "xtts_finalize_weights",
-    "xtts_set_speaker", "xtts_get_speaker", "xtts_condition", "xtts_enhance", "xtts_submit", "xtts_submit_speed", "xtts_cancel", "xtts_poll",
+    "xtts_set_speaker", "xtts_get_speaker", "xtts_condition", "xtts_enhance", "xtts_change_speed", "xtts_submit", "xtts_submit_speed", "xtts_cancel", "xtts_poll",
     "xtts_fetch", "xtts_set_option", "xtts_get_stats", "xtts_sync", "xtts_get_kernel_profile", "xtts_device_timer", "xtts_vocode",
     "xtts_vocode_window", "xtts_vocode_speed", "xtts_gpt_prefill", "xtts_gpt_teacher_forced",
     "xtts_debug_gemm", "xtts_debug_sample_slots", "xtts_debug_trace",
@@ -123,6 +124,7 @@ def load_library(path: Optional[str] = None):
     lib.xtts_get_speaker.argtypes = [vp, i32, f32p, f32p]
     lib.xtts_condition.argtypes = [vp, i32, f32p, i64, f32p, i64, i32, i32]
     lib.xtts_enhance.argtypes = [vp, f32p, i64, C.POINTER(XttsEnhanceConfig), f32p, i64, C.POINTER(i64)]
+    lib.xtts_change_speed.argtypes = [vp, f32p, i64, C.c_double, f32p, i64, C.POINTER(i64)]
     lib.xtts_submit.argtypes = [vp, C.c_uint64, i32p, i32, i32, C.POINTER(XttsSampling)]
     lib.xtts_submit_speed.argtypes = [vp, C.c_uint64, i32p, i32, i32, C.POINTER(XttsSampling), C.c_float]
     lib.xtts_cancel.argtypes = [vp, C.c_uint64]
@@ -299,6 +301,20 @@ class NativeEngine:
         n_out = C.c_int64(0)
         self._chk(self.lib.xtts_enhance(self.h, _fp(a), a.size, C.byref(XttsEnhanceConfig.of(cfg)), _fp(out), out.size,
                                         C.byref(n_out)), "enhance")
+        return out[: n_out.value]
+
+    def change_speed(self, wav, rate: float) -> np.ndarray:
+        """xtts_change_speed: the reference's TTSOutput.change_speed body (librosa phase-vocoder time stretch, then peak
+        normalisation) on the GPU; rate > 1 is faster.  -> float32 [512 * (ceil((1 + n // 512) / rate) - 1)].  Raises
+        NativeError with code ERR_INVALID where the reference raises (rate not finite or <= 0, a non-finite sample, an
+        empty result)."""
+        a = _f32(wav).reshape(-1)
+        rate = float(rate)
+        n_out = C.c_int64(0)
+        frames = math.ceil((1 + a.size // 512) / rate) if math.isfinite(rate) and rate > 0 else 1
+        cap = 512 * (frames - 1) if frames <= 1 << 22 else 0          # longer results are rejected by the call
+        out = np.empty((max(cap, 1),), np.float32)
+        self._chk(self.lib.xtts_change_speed(self.h, _fp(a), a.size, rate, _fp(out), cap, C.byref(n_out)), "change_speed")
         return out[: n_out.value]
 
     # ---- generation

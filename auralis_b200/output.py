@@ -1,14 +1,18 @@
 """TTSOutput — the boundary type of the hot path (array/sample_rate/token_length/start_time).
 
 Mirrors `/root/reference/src/auralis/common/definitions/output.py:17-38,95-111` for the fields and
-``combine_outputs``; the audio utilities (mp3/opus/aac encoders, phase-vocoder speed change, playback)
-are CPU post-processing outside the hot path (SURVEY.md §2.1 #3): wav/pcm/flac-free paths are provided
-with the standard library, the rest raise with a clear message when their optional dependency is absent.
+``combine_outputs``.  ``change_speed`` (the reference's librosa phase vocoder + peak normalisation) runs on the GPU of a
+live `XTTSv2Engine` (``register_gpu_provider``), and on librosa when no engine is alive.  The other audio utilities
+(mp3/opus/aac encoders, playback) are CPU post-processing outside the hot path (SURVEY.md §2.1 #3): wav/pcm/flac-free
+paths are provided with the standard library, the rest raise with a clear message when their optional dependency is
+absent.
 """
 from __future__ import annotations
 
 import io
+import threading
 import wave
+import weakref
 from dataclasses import dataclass
 from pathlib import Path
 from typing import List, Optional, Union
@@ -74,6 +78,35 @@ def _parse_riff_wav(blob: bytes):
         return None
     n = a.shape[0] // nch * nch
     return a[:n].reshape(-1, nch), int(sr)
+
+
+_providers: List["weakref.ref"] = []
+_providers_lock = threading.Lock()
+
+
+def register_gpu_provider(engine) -> None:
+    """Route `TTSOutput.change_speed` to `engine.change_speed(array, speed_factor) -> np.ndarray` while the engine is
+    alive (`XTTSv2Engine` registers itself when it is built).  Held through a weak reference, so the registry never keeps
+    an engine alive; the most recently registered live engine serves."""
+    with _providers_lock:
+        _providers[:] = [r for r in _providers if r() is not None and r() is not engine]
+        _providers.append(weakref.ref(engine))
+
+
+def unregister_gpu_provider(engine) -> None:
+    """Take `engine` out of the registry (its shutdown)."""
+    with _providers_lock:
+        _providers[:] = [r for r in _providers if r() is not None and r() is not engine]
+
+
+def gpu_provider():
+    """The engine `TTSOutput.change_speed` runs on, or None."""
+    with _providers_lock:
+        for r in reversed(_providers):
+            e = r()
+            if e is not None:
+                return e
+    return None
 
 
 @dataclass
@@ -203,10 +236,19 @@ class TTSOutput:
         return TTSOutput(array=y, sample_rate=new_sample_rate)
 
     def change_speed(self, speed_factor: float) -> "TTSOutput":
+        """output.py:40-92: time-stretch the audio by `speed_factor` (> 1 faster, < 1 slower) with librosa's phase
+        vocoder (STFT n_fft 2048, hop 512), then peak-normalise it to max |x| = 1.  `<= 0` raises ValueError, `== 1`
+        returns this object.  While an `XTTSv2Engine` is alive the stretch runs on its first GPU (`xtts_change_speed`,
+        the same arithmetic as librosa 0.10 under numpy's promotion rules) and a factor the reference would reject
+        raises ValueError; without one it needs librosa installed and raises RuntimeError otherwise.  Returns a new
+        TTSOutput with only `array` and `sample_rate` set, like the reference."""
         if speed_factor <= 0:
             raise ValueError("Speed factor must be positive")
         if speed_factor == 1.0:
             return self
+        gpu = gpu_provider()
+        if gpu is not None:
+            return TTSOutput(array=gpu.change_speed(self.array, speed_factor), sample_rate=self.sample_rate)
         try:
             import librosa
         except ImportError as e:

@@ -16,7 +16,10 @@ not librosa's soxr.
 Additions (not in the reference): ``seed`` (reproducible sampling) and ``speed``, the speaking rate in [0.25, 4.0] (> 1 is
 faster; the reference offers speed only in its OpenAI server, as a CPU phase vocoder on the finished waveform).  Here it
 time-scales the GPT latents on the GPU before the vocoder, as Coqui's ``Xtts.inference(speed=...)`` does, so the pitch
-stays; the tokens are the same at every speed.
+stays; the tokens are the same at every speed.  The reference's own tool for a finished waveform, the phase vocoder of
+``TTSOutput.change_speed`` (what its OpenAI server applies), is there too and also runs on the GPU while an engine is
+alive; it stretches any audio after the fact (a combined book, a file read with ``TTSOutput.from_file``) and
+peak-normalises it.
 """
 from __future__ import annotations
 

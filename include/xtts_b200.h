@@ -144,6 +144,16 @@ typedef struct xtts_enhance_config {
 int xtts_enhance(xtts_engine* e, const float* wav, int64_t n, const xtts_enhance_config* cfg, float* out, int64_t cap,
                  int64_t* n_out);
 
+/* TTSOutput.change_speed (output.py:40-92): librosa.stft (n_fft 2048, hop 512) -> librosa.phase_vocoder(rate) ->
+ * librosa.istft -> librosa.util.normalize(norm=inf) on the GPU, with librosa 0.10's arithmetic under NumPy's NEP 50
+ * promotion.  wav: n mono samples (any sample rate).  rate > 1 is faster; a double, so the frame count ceil(T / rate)
+ * (T = 1 + n / 512) and the frame positions t * rate are numpy's.  Writes *n_out = 512 * (ceil(T / rate) - 1) samples
+ * with max |out| == 1 (all-zero input stays zero); *n_out is always set, cap < *n_out fails.  Returns XTTS_ERR_INVALID
+ * where the reference raises: rate not finite or <= 0, a non-finite sample, an empty result (ceil(T / rate) == 1), a
+ * non-finite result.  Works in blocks of at most "pvoc_block_frames" output frames (bit-identical for every value).
+ * Runs on the conditioning stream; its time counts in xtts_stats.cond_ms. */
+int xtts_change_speed(xtts_engine* e, const float* wav, int64_t n, double rate, float* out, int64_t cap, int64_t* n_out);
+
 /* llm_engine.generate(...) per text chunk (XTTSv2.py:741-757): text_ids = [bos]+bpe+[eos] (XTTSv2.py:519-522).
  * Asynchronous: the scheduler thread admits, prefills, decodes (continuous batching), vocodes. */
 int xtts_submit(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
@@ -182,6 +192,9 @@ int xtts_fetch(xtts_engine* e, uint64_t seq_id, int32_t* tokens, float* wav, flo
  *                         stream beside the decode step), 0 = one window per chunk when it ends.  Same samples either way.
  *   "voc_sms"             SMs the vocoder's persistent conv kernels may occupy while a decode step is in flight (0 = all)
  *   "voc_batch"           windows per vocoder launch (1..32, default 32; ragged lengths are batched together)
+ *   "pvoc_block_frames"   xtts_change_speed's block: at most this many output STFT frames (and this many + 2 input frames)
+ *                         per pass, 1 .. 2^20, default 4096 (a spectral workspace of about 45 KB per frame, ~185 MB,
+ *                         whatever the input length).  Bit-identical results for every value.
  *   "tc_epilogue"         epilogue of the fast-mode vocoder's tensor-core Conv1d: 1 (default) = staged through shared
  *                         memory (residual prefetched by a loader warp, outputs drained by bulk copies while the next
  *                         tile's MMAs run), 0 = straight from the accumulators.  Bit-identical results either way.
