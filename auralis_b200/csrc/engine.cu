@@ -179,7 +179,22 @@ public:
     void gpt_teacher_forced_sync(const int32_t* text, int n_text, int speaker, const int32_t* forced, int n,
                                  const xtts_sampling& sp, float* logits_out, float* latents_out, int32_t* sampled_out);
     void debug_gemm(int mode, const float* A, const float* W, const float* bias, const float* resid, float* out, int M,
-                    int N, int K, int gelu, int iters, float* ms);
+                    int N, int K, int dflags, int iters, float* ms);
+    void debug_ln_gemm(int mode, int launch, int M, int N, int K, const float* X, const float* ln_w, const float* ln_b,
+                       const float* W, const float* bias, const float* resid, int dflags, float* Y, float* out, int32_t* n_ctas,
+                       uint32_t* counters);
+    void debug_norms(int out_type, int M, int H, const float* X, int x_rows, const int32_t* row_index, const float* w1,
+                     const float* b1, const float* w2, const float* b2, float* Y, float* latents, int n_slots, int lat_rows,
+                     const int32_t* slots, const int32_t* lat_pos, const int32_t* n_gen);
+    void debug_kv_write(int kv_type, int heads, int M, const float* qkv, const int32_t* row_slot, const int32_t* row_pos,
+                        int n_slots, const int32_t* ctx_len, const int32_t* block_tables, int max_pages, int n_pages,
+                        void* kpool, void* vpool);
+    void debug_build_rows(int H, int n_cond, const float* text_emb, int n_text, const float* text_pos, int n_tpos,
+                          const float* wte, int n_audio, const float* wpe, int n_wpe, const float* spk, int n_spk,
+                          const int32_t* rows, int n_rows, float* X);
+    void debug_build_decode_rows(int H, const float* wte, int n_audio, const float* wpe, int n_wpe, int M, const int32_t* active,
+                                 int n_slots, const int32_t* last_tok, const int32_t* n_gen, float* X, uint32_t* counters,
+                                 int n_flags, int n_words);
     void debug_sample_slots(int V, int M, const int32_t* active, int n_slots, const float* logits, int ld,
                             const xtts_sampling* sp, int cap, int advance_ctx, const int32_t* forced, int32_t* n_gen,
                             int32_t* ctx_len, int32_t* finished, int32_t* last_tok, uint8_t* seen, int32_t* tokens,
@@ -2228,39 +2243,75 @@ void Engine::gpt_teacher_forced_sync(const int32_t* text, int n_text, int speake
     release_slot(s);
 }
 
+// fp32 -> the 16-bit operand type of `mode` (1 bf16, 2 IEEE fp16 bits in the same buffer type)
+static void to16(int mode, const float* in, __nv_bfloat16* out, size_t n, cudaStream_t st) {
+    if (mode == 2) launch_f32_to_f16(in, reinterpret_cast<__half*>(out), n, st);
+    else launch_f32_to_bf16(in, out, n, st);
+}
+
+// 16-bit device values -> fp32 on the host (exact)
+static void widen16(const std::vector<uint16_t>& in, bool f16, float* out) {
+    for (size_t i = 0; i < in.size(); ++i) {
+        if (f16) { __half_raw r; r.x = in[i]; out[i] = __half2float(__half(r)); }
+        else { const uint32_t u = (uint32_t)in[i] << 16; std::memcpy(&out[i], &u, 4); }
+    }
+}
+
+// One GEMM launch on private buffers.  The weights are converted and synchronised first; the activation conversion is the
+// kernel right before the GEMM, so a PDL launch overlaps it exactly as the decode chain overlaps a GEMM with its producer
+// (weight tiles requested before griddepcontrol.wait, activation tiles and the residual after it).
 void Engine::debug_gemm(int mode, const float* A, const float* W, const float* bias, const float* resid, float* out, int M,
-                        int N, int K, int gelu, int iters, float* ms) {
+                        int N, int K, int dflags, int iters, float* ms) {
     ApiLock lk(this);
+    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
+    if (mode < 0 || mode > 2) throw std::runtime_error("debug_gemm: mode 0 (fp32), 1 (bf16) or 2 (fp16)");
+    if (M < 1 || N < 1 || K < 1 || !A || !W || !out) throw std::runtime_error("debug_gemm: empty problem");
+    if (dflags & ~(XTTS_DEBUG_GEMM_GELU | XTTS_DEBUG_GEMM_OUT16 | XTTS_DEBUG_GEMM_INPLACE | XTTS_DEBUG_GEMM_PDL))
+        throw std::runtime_error("debug_gemm: unknown flag bits");
+    const bool out16 = dflags & XTTS_DEBUG_GEMM_OUT16, inplace = dflags & XTTS_DEBUG_GEMM_INPLACE, pdl = dflags & XTTS_DEBUG_GEMM_PDL;
+    if (mode == 0 && (out16 || pdl)) throw std::runtime_error("debug_gemm: 16-bit output and PDL need mode 1 or 2");
+    if (inplace && (!resid || out16)) throw std::runtime_error("debug_gemm: an in-place residual needs resid and fp32 output");
+    if (mode >= 1 && (K % 64 != 0 || N % 32 != 0)) throw std::runtime_error("debug_gemm: modes 1 / 2 need K % 64 == 0 and N % 32 == 0");
     CUDA_CHECK(cudaSetDevice(cfg.device));
     DBuf<float> dA, dW, db, dr, dout;
-    dA.alloc((size_t)M * K); dW.alloc((size_t)N * K); dout.alloc((size_t)M * N);
+    DBuf<__nv_bfloat16> dout16;
+    dA.alloc((size_t)M * K); dW.alloc((size_t)N * K);
+    if (out16) dout16.alloc((size_t)M * N); else dout.alloc((size_t)M * N);
     dA.upload(A, (size_t)M * K, st); dW.upload(W, (size_t)N * K, st);
     if (bias) { db.alloc(N); db.upload(bias, N, st); }
-    if (resid) { dr.alloc((size_t)M * N); dr.upload(resid, (size_t)M * N, st); }
-    if (mode < 0 || mode > 2) throw std::runtime_error("debug_gemm: mode 0 (fp32), 1 (bf16) or 2 (fp16)");
-    const int flags = (gelu ? GEMM_GELU : 0) | (resid ? GEMM_RESID : 0) | (mode == 2 ? GEMM_F16 : 0);
+    if (resid && !inplace) { dr.alloc((size_t)M * N); dr.upload(resid, (size_t)M * N, st); }
+    const int flags = ((dflags & XTTS_DEBUG_GEMM_GELU) ? GEMM_GELU : 0) | (resid ? GEMM_RESID : 0) | (out16 ? GEMM_OUT_BF16 : 0) |
+                      (mode == 2 ? GEMM_F16 : 0);
     DBuf<__nv_bfloat16> hA, hW;                     // 16-bit operands (IEEE fp16 bits in mode 2)
     if (mode >= 1) {
         std::string err;
         if (!gemm_tc_init(&err)) throw std::runtime_error(err);
         hA.alloc((size_t)M * K); hW.alloc((size_t)N * K);
-        if (mode == 1) {
-            launch_f32_to_bf16(dA.p, hA.p, (size_t)M * K, st); launch_f32_to_bf16(dW.p, hW.p, (size_t)N * K, st);
-        } else {
-            launch_f32_to_f16(dA.p, reinterpret_cast<__half*>(hA.p), (size_t)M * K, st);
-            launch_f32_to_f16(dW.p, reinterpret_cast<__half*>(hW.p), (size_t)N * K, st);
-        }
+        to16(mode, dW.p, hW.p, (size_t)N * K, st);
     }
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    // in place: out holds the residual and is passed as both (the engine's o-proj / down-proj without split-K)
+    const float* rp = inplace ? dout.p : dr.p;
+    void* op = out16 ? (void*)dout16.p : (void*)dout.p;
     cudaEvent_t e0, e1;
     CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
     auto run = [&] {
-        if (mode >= 1) launch_gemm_bf16_tc(hA.p, hW.p, db.p, dr.p, dout.p, M, N, K, flags, st);
-        else launch_gemm_f32(dA.p, dW.p, db.p, dr.p, dout.p, M, N, K, flags, st);
+        if (mode >= 1) launch_gemm_bf16_tc(hA.p, hW.p, db.p, rp, op, M, N, K, flags, st, pdl);
+        else launch_gemm_f32(dA.p, dW.p, db.p, rp, dout.p, M, N, K, flags, st);
     };
+    if (inplace) dout.upload(resid, (size_t)M * N, st);
+    if (mode >= 1) to16(mode, dA.p, hA.p, (size_t)M * K, st);
     run();
     CUDA_CHECK(cudaStreamSynchronize(st));
-    dout.download(out, (size_t)M * N, st);
-    CUDA_CHECK(cudaStreamSynchronize(st));
+    if (out16) {
+        std::vector<uint16_t> o((size_t)M * N);
+        dout16.download(reinterpret_cast<__nv_bfloat16*>(o.data()), o.size(), st);
+        CUDA_CHECK(cudaStreamSynchronize(st));
+        widen16(o, mode == 2, out);
+    } else {
+        dout.download(out, (size_t)M * N, st);
+        CUDA_CHECK(cudaStreamSynchronize(st));
+    }
     if (iters > 0) {
         CUDA_CHECK(cudaEventRecord(e0, st));
         for (int i = 0; i < iters; ++i) run();
@@ -2342,14 +2393,6 @@ void Engine::debug_sample_slots(int Vn, int M, const int32_t* active, int n_slot
         for (int v = 0; v < Vn; ++v) seen[(size_t)s * Vn + v] = (uint8_t)((sb[(size_t)s * sw + (v >> 5)] >> (v & 31)) & 1u);
         if (Vn % 32 && (sb[(size_t)s * sw + sw - 1] >> (Vn % 32)))
             throw std::runtime_error("debug_sample_slots: the kernel set a seen bit at an id >= V");
-    }
-}
-
-// 16-bit device values -> fp32 on the host (exact)
-static void widen16(const std::vector<uint16_t>& in, bool f16, float* out) {
-    for (size_t i = 0; i < in.size(); ++i) {
-        if (f16) { __half_raw r; r.x = in[i]; out[i] = __half2float(__half(r)); }
-        else { const uint32_t u = (uint32_t)in[i] << 16; std::memcpy(&out[i], &u, 4); }
     }
 }
 
@@ -2498,6 +2541,217 @@ void Engine::debug_splitk_ln(int mode, int M, int N, int K, int splits, const fl
     if (ln_w) dY.download(reinterpret_cast<__nv_bfloat16*>(y.data()), y.size(), st);
     CUDA_CHECK(cudaStreamSynchronize(st));
     if (ln_w) widen16(y, mode == 2, Y);
+}
+
+// The decode step's LayerNorm -> GEMM pair as decode_layers_rows launches it: the 16-bit LayerNorm into the operand buffer,
+// then the one-tile GEMM on it.  launch 0: plain launches; 1: both with PDL; 2: PDL plus dependency counters (the LN waits
+// for its predecessor in full and counts its CTAs into counter 0, the GEMM polls counter 0 for M arrivals instead of
+// griddepcontrol.wait and counts its CTAs into counter 1).
+void Engine::debug_ln_gemm(int mode, int launch, int M, int N, int K, const float* X, const float* ln_w, const float* ln_b,
+                           const float* W, const float* bias, const float* resid, int dflags, float* Y, float* out,
+                           int32_t* n_ctas, uint32_t* counters) {
+    ApiLock lk(this);
+    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
+    if (mode != 1 && mode != 2) throw std::runtime_error("debug_ln_gemm: mode 1 (bf16) or 2 (fp16)");
+    if (launch < 0 || launch > 2) throw std::runtime_error("debug_ln_gemm: launch 0 (plain), 1 (PDL) or 2 (PDL + counters)");
+    if (M < 1 || N < 32 || N % 32 != 0 || K < 64 || K % 64 != 0 || K > 8192) throw std::runtime_error("debug_ln_gemm: need M >= 1, N % 32 == 0, K % 64 == 0 (<= 8192)");
+    if (dflags & ~(XTTS_DEBUG_GEMM_GELU | XTTS_DEBUG_GEMM_OUT16)) throw std::runtime_error("debug_ln_gemm: flags GELU / OUT16 only");
+    if (!X || !ln_w || !ln_b || !W || !Y || !out || !n_ctas || !counters) throw std::runtime_error("debug_ln_gemm: only bias and resid may be NULL");
+    if (resid && (dflags & XTTS_DEBUG_GEMM_OUT16)) throw std::runtime_error("debug_ln_gemm: a residual needs fp32 output");
+    // (launch_gemm_bf16_tc refuses it too, but only after the LayerNorm has been enqueued)
+    if (resid && launch == 2) throw std::runtime_error("debug_ln_gemm: a counter dependency cannot order a residual read");
+    CUDA_CHECK(cudaSetDevice(cfg.device));
+    std::string err;
+    if (!gemm_tc_init(&err)) throw std::runtime_error(err);
+    const bool out16 = dflags & XTTS_DEBUG_GEMM_OUT16;
+    DBuf<float> dX, dlw, dlb, dW, db, dr, dout;
+    DBuf<__nv_bfloat16> hW, dY, dout16;
+    DBuf<unsigned> dcnt;
+    dX.alloc((size_t)M * K); dlw.alloc(K); dlb.alloc(K); dW.alloc((size_t)N * K); hW.alloc((size_t)N * K); dY.alloc((size_t)M * K);
+    dcnt.alloc(2);
+    if (out16) dout16.alloc((size_t)M * N); else dout.alloc((size_t)M * N);
+    dX.upload(X, (size_t)M * K, st); dlw.upload(ln_w, K, st); dlb.upload(ln_b, K, st); dW.upload(W, (size_t)N * K, st);
+    if (bias) { db.alloc(N); db.upload(bias, N, st); }
+    if (resid) { dr.alloc((size_t)M * N); dr.upload(resid, (size_t)M * N, st); }
+    to16(mode, dW.p, hW.p, (size_t)N * K, st);
+    CUDA_CHECK(cudaMemsetAsync(dcnt.p, 0, 2 * sizeof(unsigned), st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    const bool pdl = launch >= 1;
+    DepFlag dln, dg;
+    if (launch == 2) { dln.arrive = dcnt.p; dg.wait = dcnt.p; dg.target = (unsigned)M; dg.arrive = dcnt.p + 1; }
+    if (mode == 2) launch_layernorm<__half>(dX.p, dlw.p, dlb.p, reinterpret_cast<__half*>(dY.p), M, K, cfg.ln_eps, st, pdl, dln);
+    else launch_layernorm<__nv_bfloat16>(dX.p, dlw.p, dlb.p, dY.p, M, K, cfg.ln_eps, st, pdl, dln);
+    const int flags = ((dflags & XTTS_DEBUG_GEMM_GELU) ? GEMM_GELU : 0) | (out16 ? GEMM_OUT_BF16 : 0) | (resid ? GEMM_RESID : 0) |
+                      (mode == 2 ? GEMM_F16 : 0);
+    *n_ctas = launch_gemm_bf16_tc(dY.p, hW.p, db.p, dr.p, out16 ? (void*)dout16.p : (void*)dout.p, M, N, K, flags, st, pdl, dg);
+    std::vector<uint16_t> y((size_t)M * K), o16(out16 ? (size_t)M * N : 0);
+    dY.download(reinterpret_cast<__nv_bfloat16*>(y.data()), y.size(), st);
+    if (out16) dout16.download(reinterpret_cast<__nv_bfloat16*>(o16.data()), o16.size(), st);
+    else dout.download(out, (size_t)M * N, st);
+    dcnt.download(counters, 2, st);
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    widen16(y, mode == 2, Y);
+    if (out16) widen16(o16, mode == 2, out);
+}
+
+// launch_layernorm (w2 == NULL) or launch_head_norms (w2 != NULL) in the output type `out_type` on private buffers
+void Engine::debug_norms(int out_type, int M, int H, const float* X, int x_rows, const int32_t* row_index, const float* w1,
+                         const float* b1, const float* w2, const float* b2, float* Y, float* latents, int n_slots,
+                         int lat_rows, const int32_t* slots, const int32_t* lat_pos, const int32_t* n_gen) {
+    ApiLock lk(this);
+    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
+    if (out_type < 0 || out_type > 2) throw std::runtime_error("debug_norms: out_type 0 (fp32), 1 (bf16) or 2 (fp16)");
+    if (M < 1 || H < 1 || H > 8192 || x_rows < 1) throw std::runtime_error("debug_norms: need M >= 1, 1 <= H <= 8192, x_rows >= 1");
+    if (!X || !w1 || !b1 || !Y || (w2 == nullptr) != (b2 == nullptr)) throw std::runtime_error("debug_norms: X, w1, b1, Y, and w2 / b2 together");
+    const bool head = w2 != nullptr;
+    if (!head && (row_index || latents || x_rows < M)) throw std::runtime_error("debug_norms: a plain LayerNorm reads rows 0 .. M-1 and has no latents");
+    if (row_index)
+        for (int i = 0; i < M; ++i)
+            if (row_index[i] < 0 || row_index[i] >= x_rows) throw std::runtime_error("debug_norms: row_index outside X");
+    if (!row_index && x_rows < M) throw std::runtime_error("debug_norms: X has fewer than M rows");
+    if (latents) {
+        if (!slots || n_slots < 1 || lat_rows < 1 || (!lat_pos && !n_gen)) throw std::runtime_error("debug_norms: latents need slots, n_slots, lat_rows and lat_pos or n_gen");
+        for (int i = 0; i < M; ++i)
+            if (slots[i] < 0 || slots[i] >= n_slots) throw std::runtime_error("debug_norms: slot outside n_slots");
+    }
+    CUDA_CHECK(cudaSetDevice(cfg.device));
+    const size_t esz = out_type == 0 ? 4 : 2, nlat = latents ? (size_t)n_slots * lat_rows * H : 0;
+    DBuf<float> dX, dw1, db1, dw2, db2, dlat;
+    DBuf<int> dri, dsl, dlp, dng;
+    DBuf<uint8_t> dY;
+    dX.alloc((size_t)x_rows * H); dw1.alloc(H); db1.alloc(H); dY.alloc((size_t)M * H * esz);
+    dX.upload(X, (size_t)x_rows * H, st); dw1.upload(w1, H, st); db1.upload(b1, H, st);
+    if (head) { dw2.alloc(H); db2.alloc(H); dw2.upload(w2, H, st); db2.upload(b2, H, st); }
+    if (row_index) { dri.alloc(M); dri.upload(row_index, M, st); }
+    if (latents) {
+        dlat.alloc(nlat); dlat.upload(latents, nlat, st);
+        dsl.alloc(M); dsl.upload(slots, M, st);
+        if (lat_pos) { dlp.alloc(M); dlp.upload(lat_pos, M, st); }
+        if (n_gen) { dng.alloc(n_slots); dng.upload(n_gen, n_slots, st); }
+    }
+    const float eps = cfg.ln_eps;
+    auto run = [&](auto* y) {
+        using T = std::remove_pointer_t<decltype(y)>;
+        if (!head) launch_layernorm<T>(dX.p, dw1.p, db1.p, y, M, H, eps, st);
+        else launch_head_norms<T>(dX.p, dri.p, dw1.p, db1.p, dw2.p, db2.p, y, latents ? dlat.p : nullptr, dsl.p, dlp.p, dng.p,
+                                  lat_rows, M, H, eps, st);
+    };
+    if (out_type == 0) run(reinterpret_cast<float*>(dY.p));
+    else if (out_type == 1) run(reinterpret_cast<__nv_bfloat16*>(dY.p));
+    else run(reinterpret_cast<__half*>(dY.p));
+    if (latents) dlat.download(latents, nlat, st);
+    if (out_type == 0) {
+        dY.download(reinterpret_cast<uint8_t*>(Y), (size_t)M * H * 4, st);
+        CUDA_CHECK(cudaStreamSynchronize(st));
+    } else {
+        std::vector<uint16_t> y((size_t)M * H);
+        dY.download(reinterpret_cast<uint8_t*>(y.data()), y.size() * 2, st);
+        CUDA_CHECK(cudaStreamSynchronize(st));
+        widen16(y, out_type == 2, Y);
+    }
+}
+
+// launch_kv_write (the prefill's paged-cache write) over raw pools in the device layout, updated in place
+void Engine::debug_kv_write(int kv_type, int heads, int M, const float* qkv, const int32_t* row_slot, const int32_t* row_pos,
+                            int n_slots, const int32_t* ctx_len, const int32_t* block_tables, int mp, int n_pages, void* kpool,
+                            void* vpool) {
+    ApiLock lk(this);
+    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
+    if (kv_type < 0 || kv_type > 2) throw std::runtime_error("debug_kv_write: kv_type 0 (fp32), 1 (bf16) or 2 (fp16)");
+    if (heads < 1 || M < 1 || n_slots < 1 || mp < 1 || n_pages < 1) throw std::runtime_error("debug_kv_write: empty problem");
+    if (!qkv || !row_slot || !block_tables || !kpool || !vpool || (!row_pos && !ctx_len)) throw std::runtime_error("debug_kv_write: row_pos or ctx_len, and every other pointer");
+    for (int r = 0; r < M; ++r) {
+        const int s = row_slot[r];
+        if (s < 0 || s >= n_slots) throw std::runtime_error("debug_kv_write: row slot outside n_slots");
+        const int pos = row_pos ? row_pos[r] : ctx_len[s];
+        if (pos < 0 || pos / kPageTokens >= mp) throw std::runtime_error("debug_kv_write: position outside the block table");
+        const int id = block_tables[(size_t)s * mp + pos / kPageTokens];
+        if (id < 0 || id >= n_pages) throw std::runtime_error("debug_kv_write: page id outside the pool");
+    }
+    CUDA_CHECK(cudaSetDevice(cfg.device));
+    const size_t esz = kv_type == 0 ? 4 : 2;
+    const size_t pool = (size_t)n_pages * heads * kPageTokens * kHeadDim, Hq = (size_t)heads * kHeadDim;
+    DBuf<int> dslot, dpos, dctx, dbt;
+    DBuf<float> dqkv;
+    DBuf<uint8_t> dk, dv;
+    dslot.alloc(M); dbt.alloc((size_t)n_slots * mp); dqkv.alloc((size_t)M * 3 * Hq); dk.alloc(pool * esz); dv.alloc(pool * esz);
+    dslot.upload(row_slot, M, st); dbt.upload(block_tables, (size_t)n_slots * mp, st); dqkv.upload(qkv, (size_t)M * 3 * Hq, st);
+    if (row_pos) { dpos.alloc(M); dpos.upload(row_pos, M, st); }
+    if (ctx_len) { dctx.alloc(n_slots); dctx.upload(ctx_len, n_slots, st); }
+    dk.upload(static_cast<const uint8_t*>(kpool), pool * esz, st); dv.upload(static_cast<const uint8_t*>(vpool), pool * esz, st);
+    if (kv_type == 0)
+        launch_kv_write<float>(dqkv.p, M, dslot.p, dpos.p, dctx.p, dbt.p, mp, reinterpret_cast<float*>(dk.p), reinterpret_cast<float*>(dv.p), heads, st);
+    else if (kv_type == 1)
+        launch_kv_write<__nv_bfloat16>(dqkv.p, M, dslot.p, dpos.p, dctx.p, dbt.p, mp, reinterpret_cast<__nv_bfloat16*>(dk.p),
+                                       reinterpret_cast<__nv_bfloat16*>(dv.p), heads, st);
+    else
+        launch_kv_write<__half>(dqkv.p, M, dslot.p, dpos.p, dctx.p, dbt.p, mp, reinterpret_cast<__half*>(dk.p), reinterpret_cast<__half*>(dv.p), heads, st);
+    dk.download(static_cast<uint8_t*>(kpool), pool * esz, st); dv.download(static_cast<uint8_t*>(vpool), pool * esz, st);
+    CUDA_CHECK(cudaStreamSynchronize(st));
+}
+
+// launch_build_rows over private embedding tables: rows [n_rows][4] = RowDesc (kind, a, b, c)
+void Engine::debug_build_rows(int Hd, int n_cond, const float* text_emb, int n_text, const float* text_pos, int n_tpos,
+                              const float* wte_h, int n_audio, const float* wpe_h, int n_wpe, const float* spk, int n_spk,
+                              const int32_t* rows, int n_rows, float* X) {
+    ApiLock lk(this);
+    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
+    if (Hd < 4 || Hd % 4 != 0 || n_rows < 1 || n_cond < 1 || n_text < 1 || n_tpos < 1 || n_audio < 1 || n_wpe < 1 || n_spk < 1)
+        throw std::runtime_error("debug_build_rows: need H % 4 == 0 and non-empty tables and rows");
+    if (!text_emb || !text_pos || !wte_h || !wpe_h || !spk || !rows || !X) throw std::runtime_error("debug_build_rows: NULL argument");
+    for (int i = 0; i < n_rows; ++i) {
+        const int32_t* r = rows + 4 * i;
+        const bool ok = r[0] == 0 ? (r[1] >= 0 && r[1] < n_cond && r[3] >= 0 && r[3] < n_spk)
+                      : r[0] == 1 ? (r[1] >= 0 && r[1] < n_text && r[2] >= 0 && r[2] < n_tpos)
+                      : r[0] == 2 ? (r[1] >= 0 && r[1] < n_audio && r[2] >= 0 && r[2] < n_wpe) : false;
+        if (!ok) throw std::runtime_error("debug_build_rows: row kind outside 0..2 or index outside its table");
+    }
+    CUDA_CHECK(cudaSetDevice(cfg.device));
+    DBuf<float> dte, dtp, dwte, dwpe, dspk, dX;
+    DBuf<RowDesc> drows;
+    dte.alloc((size_t)n_text * Hd); dtp.alloc((size_t)n_tpos * Hd); dwte.alloc((size_t)n_audio * Hd); dwpe.alloc((size_t)n_wpe * Hd);
+    dspk.alloc((size_t)n_spk * n_cond * Hd); dX.alloc((size_t)n_rows * Hd); drows.alloc(n_rows);
+    dte.upload(text_emb, (size_t)n_text * Hd, st); dtp.upload(text_pos, (size_t)n_tpos * Hd, st);
+    dwte.upload(wte_h, (size_t)n_audio * Hd, st); dwpe.upload(wpe_h, (size_t)n_wpe * Hd, st);
+    dspk.upload(spk, (size_t)n_spk * n_cond * Hd, st);
+    static_assert(sizeof(RowDesc) == 4 * sizeof(int32_t), "RowDesc crosses the ABI as four int32");
+    drows.upload(reinterpret_cast<const RowDesc*>(rows), n_rows, st);
+    GptTables t; t.text_emb = dte.p; t.text_pos = dtp.p; t.wte = dwte.p; t.wpe = dwpe.p; t.spk_cond = dspk.p; t.H = Hd; t.n_cond = n_cond;
+    launch_build_rows(drows.p, n_rows, t, dX.p, st);
+    dX.download(X, (size_t)n_rows * Hd, st);
+    CUDA_CHECK(cudaStreamSynchronize(st));
+}
+
+// launch_build_decode_rows over private tables and slot arrays; counters [n_words] in/out, the first n_flags of them are the
+// step's dependency counters the kernel zeroes (the rest are guard words it must not touch)
+void Engine::debug_build_decode_rows(int Hd, const float* wte_h, int n_audio, const float* wpe_h, int n_wpe, int M,
+                                     const int32_t* active, int n_slots, const int32_t* last_tok, const int32_t* n_gen, float* X,
+                                     uint32_t* counters, int n_flags, int n_words) {
+    ApiLock lk(this);
+    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
+    if (Hd < 4 || Hd % 4 != 0 || M < 1 || n_slots < 1 || n_audio < 1 || n_wpe < 1) throw std::runtime_error("debug_build_decode_rows: need H % 4 == 0, M >= 1 and non-empty tables");
+    if (!wte_h || !wpe_h || !active || !last_tok || !n_gen || !X) throw std::runtime_error("debug_build_decode_rows: NULL argument");
+    if (n_flags < 0 || n_words < n_flags || (n_words > 0 && !counters)) throw std::runtime_error("debug_build_decode_rows: need 0 <= n_flags <= n_words and the counters");
+    for (int i = 0; i < M; ++i) {
+        const int s = active[i];
+        if (s < 0 || s >= n_slots) throw std::runtime_error("debug_build_decode_rows: active slot outside n_slots");
+        if (last_tok[s] < 0 || last_tok[s] >= n_audio || n_gen[s] < 0 || n_gen[s] >= n_wpe)
+            throw std::runtime_error("debug_build_decode_rows: last_tok / n_gen outside the tables");
+    }
+    CUDA_CHECK(cudaSetDevice(cfg.device));
+    DBuf<float> dwte, dwpe, dX;
+    DBuf<int> dact, dlast, dng;
+    DBuf<unsigned> dcnt;
+    dwte.alloc((size_t)n_audio * Hd); dwpe.alloc((size_t)n_wpe * Hd); dX.alloc((size_t)M * Hd);
+    dact.alloc(M); dlast.alloc(n_slots); dng.alloc(n_slots);
+    dwte.upload(wte_h, (size_t)n_audio * Hd, st); dwpe.upload(wpe_h, (size_t)n_wpe * Hd, st);
+    dact.upload(active, M, st); dlast.upload(last_tok, n_slots, st); dng.upload(n_gen, n_slots, st);
+    if (n_words > 0) { dcnt.alloc(n_words); dcnt.upload(counters, n_words, st); }
+    GptTables t{}; t.wte = dwte.p; t.wpe = dwpe.p; t.H = Hd;
+    launch_build_decode_rows(dact.p, M, dlast.p, dng.p, t, dX.p, st, use_pdl, n_flags > 0 ? dcnt.p : nullptr, n_flags);
+    dX.download(X, (size_t)M * Hd, st);
+    if (n_words > 0) dcnt.download(counters, n_words, st);
+    CUDA_CHECK(cudaStreamSynchronize(st));
 }
 
 // One launch of the fast-mode vocoder convolution (launch_conv1d_tc, or launch_convT_tc for up > 0) with the weights
@@ -2681,8 +2935,38 @@ int xtts_gpt_teacher_forced(xtts_engine* e, const int32_t* text_ids, int32_t n_t
     XTTS_TRY(e->impl->gpt_teacher_forced_sync(text_ids, n_text, speaker_slot, forced_tokens, n, *sp, logits_out, latents_out, sampled_out))
 }
 int xtts_debug_gemm(xtts_engine* e, int32_t mode, const float* A, const float* W, const float* bias, const float* resid,
-                    float* out, int32_t M, int32_t N, int32_t K, int32_t gelu, int32_t iters, float* ms_per_iter) {
-    XTTS_TRY(e->impl->debug_gemm(mode, A, W, bias, resid, out, M, N, K, gelu, iters, ms_per_iter))
+                    float* out, int32_t M, int32_t N, int32_t K, int32_t flags, int32_t iters, float* ms_per_iter) {
+    XTTS_TRY(e->impl->debug_gemm(mode, A, W, bias, resid, out, M, N, K, flags, iters, ms_per_iter))
+}
+int xtts_debug_ln_gemm(xtts_engine* e, int32_t mode, int32_t launch, int32_t M, int32_t N, int32_t K, const float* X,
+                       const float* ln_w, const float* ln_b, const float* W, const float* bias, const float* resid, int32_t flags,
+                       float* Y, float* out, int32_t* n_ctas, uint32_t* counters) {
+    XTTS_TRY(e->impl->debug_ln_gemm(mode, launch, M, N, K, X, ln_w, ln_b, W, bias, resid, flags, Y, out, n_ctas, counters))
+}
+int xtts_debug_norms(xtts_engine* e, int32_t out_type, int32_t M, int32_t H, const float* X, int32_t x_rows,
+                     const int32_t* row_index, const float* w1, const float* b1, const float* w2, const float* b2, float* Y,
+                     float* latents, int32_t n_slots, int32_t lat_rows, const int32_t* slots, const int32_t* lat_pos,
+                     const int32_t* n_gen) {
+    XTTS_TRY(e->impl->debug_norms(out_type, M, H, X, x_rows, row_index, w1, b1, w2, b2, Y, latents, n_slots, lat_rows, slots,
+                                  lat_pos, n_gen))
+}
+int xtts_debug_kv_write(xtts_engine* e, int32_t kv_type, int32_t heads, int32_t M, const float* qkv, const int32_t* row_slot,
+                        const int32_t* row_pos, int32_t n_slots, const int32_t* ctx_len, const int32_t* block_tables,
+                        int32_t max_pages, int32_t n_pages, void* kpool, void* vpool) {
+    XTTS_TRY(e->impl->debug_kv_write(kv_type, heads, M, qkv, row_slot, row_pos, n_slots, ctx_len, block_tables, max_pages, n_pages,
+                                     kpool, vpool))
+}
+int xtts_debug_build_rows(xtts_engine* e, int32_t H, int32_t n_cond, const float* text_emb, int32_t n_text, const float* text_pos,
+                          int32_t n_text_pos, const float* wte, int32_t n_audio, const float* wpe, int32_t n_wpe,
+                          const float* spk_cond, int32_t n_spk, const int32_t* rows, int32_t n_rows, float* X) {
+    XTTS_TRY(e->impl->debug_build_rows(H, n_cond, text_emb, n_text, text_pos, n_text_pos, wte, n_audio, wpe, n_wpe, spk_cond, n_spk,
+                                       rows, n_rows, X))
+}
+int xtts_debug_build_decode_rows(xtts_engine* e, int32_t H, const float* wte, int32_t n_audio, const float* wpe, int32_t n_wpe,
+                                 int32_t M, const int32_t* active, int32_t n_slots, const int32_t* last_tok, const int32_t* n_gen,
+                                 float* X, uint32_t* counters, int32_t n_flags, int32_t n_words) {
+    XTTS_TRY(e->impl->debug_build_decode_rows(H, wte, n_audio, wpe, n_wpe, M, active, n_slots, last_tok, n_gen, X, counters, n_flags,
+                                              n_words))
 }
 int xtts_debug_sample_slots(xtts_engine* e, int32_t V, int32_t M, const int32_t* active, int32_t n_slots, const float* logits,
                             int32_t ld, const xtts_sampling* sp, int32_t cap, int32_t advance_ctx, const int32_t* forced,

@@ -99,7 +99,11 @@ ABI_SYMBOLS = [
     "xtts_vocode_window", "xtts_vocode_speed", "xtts_gpt_prefill", "xtts_gpt_teacher_forced",
     "xtts_debug_gemm", "xtts_debug_sample_slots", "xtts_debug_trace",
     "xtts_debug_attn_decode", "xtts_debug_attn_prefill", "xtts_debug_splitk_ln", "xtts_debug_conv_tc",
+    "xtts_debug_ln_gemm", "xtts_debug_norms", "xtts_debug_kv_write", "xtts_debug_build_rows", "xtts_debug_build_decode_rows",
 ]
+
+# flag bits of xtts_debug_gemm / xtts_debug_ln_gemm (include/xtts_b200.h)
+GEMM_GELU, GEMM_OUT16, GEMM_INPLACE, GEMM_PDL = 1, 2, 4, 8
 
 _lib = None
 
@@ -150,6 +154,13 @@ def load_library(path: Optional[str] = None):
     lib.xtts_debug_splitk_ln.argtypes = [vp, i32, i32, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, f32p, f32p]
     lib.xtts_debug_conv_tc.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, i32p, f32p, f32p, f32p, i32, f32p, f32p, i32,
                                        C.c_float, C.c_float, i32, f32p, f32p]
+    u32p = C.POINTER(C.c_uint32)
+    lib.xtts_debug_ln_gemm.argtypes = [vp, i32, i32, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, f32p, i32, f32p, f32p, i32p, u32p]
+    lib.xtts_debug_norms.argtypes = [vp, i32, i32, i32, f32p, i32, i32p, f32p, f32p, f32p, f32p, f32p, f32p, i32, i32, i32p, i32p,
+                                     i32p]
+    lib.xtts_debug_kv_write.argtypes = [vp, i32, i32, i32, f32p, i32p, i32p, i32, i32p, i32p, i32, i32, vp, vp]
+    lib.xtts_debug_build_rows.argtypes = [vp, i32, i32, f32p, i32, f32p, i32, f32p, i32, f32p, i32, f32p, i32, i32p, i32, f32p]
+    lib.xtts_debug_build_decode_rows.argtypes = [vp, i32, f32p, i32, f32p, i32, i32, i32p, i32, i32p, i32p, f32p, u32p, i32, i32]
     for s in ABI_SYMBOLS:
         if s not in ("xtts_last_error", "xtts_version"):
             getattr(lib, s).restype = C.c_int
@@ -484,7 +495,10 @@ class NativeEngine:
                                                    _fp(logits), _fp(lat), _ip(sampled)), "gpt_teacher_forced")
         return logits, lat, sampled
 
-    def debug_gemm(self, mode: int, A, W, bias=None, resid=None, gelu: bool = False, iters: int = 0):
+    def debug_gemm(self, mode: int, A, W, bias=None, resid=None, gelu: bool = False, iters: int = 0, out16: bool = False,
+                   inplace: bool = False, pdl: bool = False):
+        """One GEMM launch (xtts_debug_gemm): out16 = 16-bit output (returned widened), inplace = the residual preloaded in
+        `out` and passed as both, pdl = programmatic dependent launch.  -> (out [M, N] fp32, ms per timed iteration)."""
         A, W = _f32(A), _f32(W)
         M, K = A.shape
         N = W.shape[0]
@@ -492,9 +506,88 @@ class NativeEngine:
         r = _f32(resid) if resid is not None else None
         out = np.empty((M, N), np.float32)
         ms = C.c_float(0)
+        flags = (GEMM_GELU if gelu else 0) | (GEMM_OUT16 if out16 else 0) | (GEMM_INPLACE if inplace else 0) | (GEMM_PDL if pdl else 0)
         self._chk(self.lib.xtts_debug_gemm(self.h, mode, _fp(A), _fp(W), _fp(b), _fp(r), _fp(out), M, N, K,
-                                           1 if gelu else 0, iters, C.byref(ms)), "debug_gemm")
+                                           flags, iters, C.byref(ms)), "debug_gemm")
         return out, ms.value
+
+    LN_GEMM_PLAIN, LN_GEMM_PDL, LN_GEMM_COUNTERS = 0, 1, 2
+
+    def debug_ln_gemm(self, mode: int, launch: int, X, ln_w, ln_b, W, bias=None, resid=None, gelu: bool = False,
+                      out16: bool = False):
+        """The decode LayerNorm -> GEMM pair (xtts_debug_ln_gemm).  -> (Y [M, K] the 16-bit LN output, out [M, N], the GEMM's
+        CTA count, counters [2] after the launch)."""
+        X, W, lw, lb = _f32(X), _f32(W), _f32(ln_w), _f32(ln_b)
+        M, K = X.shape
+        N = W.shape[0]
+        b = _f32(bias) if bias is not None else None
+        r = _f32(resid) if resid is not None else None
+        Y = np.empty((M, K), np.float32)
+        out = np.empty((M, N), np.float32)
+        n = C.c_int32(0)
+        cnt = np.zeros(2, np.uint32)
+        flags = (GEMM_GELU if gelu else 0) | (GEMM_OUT16 if out16 else 0)
+        self._chk(self.lib.xtts_debug_ln_gemm(self.h, mode, launch, M, N, K, _fp(X), _fp(lw), _fp(lb), _fp(W), _fp(b), _fp(r),
+                                              flags, _fp(Y), _fp(out), C.byref(n),
+                                              cnt.ctypes.data_as(C.POINTER(C.c_uint32))), "debug_ln_gemm")
+        return Y, out, int(n.value), cnt
+
+    def debug_norms(self, out_type: int, X, w1, b1, w2=None, b2=None, M: Optional[int] = None, row_index=None, latents=None,
+                    slots=None, lat_pos=None, n_gen=None):
+        """LayerNorm (w2 None) or the GPT head norms (xtts_debug_norms).  X [x_rows, H]; latents [n_slots, lat_rows, H] is the
+        incoming contents.  -> (Y [M, H] fp32, latents after or None)."""
+        x = _f32(X)
+        x_rows, H = x.shape
+        M = M if M is not None else (len(row_index) if row_index is not None else x_rows)
+        Y = np.empty((M, H), np.float32)
+        lat = _f32(latents).copy() if latents is not None else None
+        n_slots, lat_rows = (lat.shape[0], lat.shape[1]) if lat is not None else (0, 0)
+        ri, sl, lp, ng = (_i32(a) if a is not None else None for a in (row_index, slots, lat_pos, n_gen))
+        w2a = _f32(w2) if w2 is not None else None
+        b2a = _f32(b2) if b2 is not None else None
+        self._chk(self.lib.xtts_debug_norms(self.h, out_type, M, H, _fp(x), x_rows, _ip(ri), _fp(_f32(w1)), _fp(_f32(b1)),
+                                            _fp(w2a), _fp(b2a), _fp(Y), _fp(lat), n_slots, lat_rows, _ip(sl), _ip(lp), _ip(ng)),
+                  "debug_norms")
+        return Y, lat
+
+    def debug_kv_write(self, kv_type: int, heads: int, qkv, row_slot, block_tables, kpool, vpool, row_pos=None, ctx_len=None):
+        """The prefill's paged-cache write (xtts_debug_kv_write).  kpool / vpool as in debug_attn_decode; ctx_len [n_slots]
+        (n_slots = rows of block_tables).  -> (kpool after, vpool after)."""
+        q, rs, bt = _f32(qkv), _i32(row_slot), _i32(block_tables)
+        rp = _i32(row_pos) if row_pos is not None else None
+        ctx = _i32(ctx_len) if ctx_len is not None else None
+        dt = self.KV_DTYPES[kv_type]
+        k = np.ascontiguousarray(kpool, dtype=dt).copy()
+        v = np.ascontiguousarray(vpool, dtype=dt).copy()
+        assert k.shape == v.shape and k.shape[1] == heads and bt.ndim == 2
+        self._chk(self.lib.xtts_debug_kv_write(self.h, kv_type, heads, rs.size, _fp(q), _ip(rs), _ip(rp), bt.shape[0], _ip(ctx),
+                                               _ip(bt), bt.shape[1], k.shape[0], k.ctypes.data, v.ctypes.data), "debug_kv_write")
+        return k, v
+
+    def debug_build_rows(self, rows, text_emb, text_pos, wte, wpe, spk_cond):
+        """Prompt row build (xtts_debug_build_rows): rows [n, 4] = (kind, a, b, c); spk_cond [n_spk, n_cond, H].  -> X [n, H]."""
+        r = _i32(rows).reshape(-1, 4)
+        te, tp, a, p, s = (_f32(t) for t in (text_emb, text_pos, wte, wpe, spk_cond))
+        H = te.shape[1]
+        X = np.empty((r.shape[0], H), np.float32)
+        self._chk(self.lib.xtts_debug_build_rows(self.h, H, s.shape[1], _fp(te), te.shape[0], _fp(tp), tp.shape[0], _fp(a), a.shape[0],
+                                                 _fp(p), p.shape[0], _fp(s), s.shape[0], _ip(r), r.shape[0], _fp(X)),
+                  "debug_build_rows")
+        return X
+
+    def debug_build_decode_rows(self, active, last_tok, n_gen, wte, wpe, counters=None, n_flags: int = 0):
+        """Decode row build (xtts_debug_build_decode_rows): last_tok / n_gen [n_slots]; counters (uint32, incoming contents)
+        whose first n_flags words the kernel zeroes.  -> (X [M, H], counters after or None)."""
+        act, lt, ng = _i32(active), _i32(last_tok), _i32(n_gen)
+        a, p = _f32(wte), _f32(wpe)
+        H = a.shape[1]
+        X = np.empty((act.size, H), np.float32)
+        cnt = np.ascontiguousarray(counters, dtype=np.uint32).copy() if counters is not None else None
+        self._chk(self.lib.xtts_debug_build_decode_rows(self.h, H, _fp(a), a.shape[0], _fp(p), p.shape[0], act.size, _ip(act), lt.size,
+                                                        _ip(lt), _ip(ng), _fp(X),
+                                                        cnt.ctypes.data_as(C.POINTER(C.c_uint32)) if cnt is not None else None,
+                                                        n_flags, cnt.size if cnt is not None else 0), "debug_build_decode_rows")
+        return X, cnt
 
     def debug_sample(self, logits, seen, sp: Sampling, step: int = 0):
         """Row b of logits [B, V] sampled as slot b with sp and seq_seed sp.seq_seed + b at step `step`; seen [B, V] (0/1)

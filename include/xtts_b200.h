@@ -244,9 +244,22 @@ int xtts_gpt_prefill(xtts_engine* e, const int32_t* text_ids, int32_t n_text, in
 int xtts_gpt_teacher_forced(xtts_engine* e, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
                             const int32_t* forced_tokens, int32_t n, const xtts_sampling* sp, float* logits_out,
                             float* latents_out, int32_t* sampled_out);
-/* GEMM under test: mode 0 = fp32 CUDA-core, 1 = bf16 wgmma, 2 = fp16 wgmma.  A [M,K], W [N,K], bias [N] or NULL, resid [M,N] or NULL */
+/* GEMM under test: mode 0 = fp32 CUDA-core, 1 = bf16 wgmma, 2 = fp16 wgmma.  A [M,K], W [N,K], bias [N] or NULL, resid [M,N] or NULL;
+ * out [M,N] = epi(A . W^T + bias) under the engine's current GEMM options ("gemm_wide", "gemm_bn", "gemm_deep_ring",
+ * "gemm_l2_prefetch").  flags (XTTS_DEBUG_GEMM_*; 0 / 1 = without / with GELU, as before the flag word):
+ *   GELU    gelu_new after the bias, before the residual
+ *   OUT16   16-bit output in the operand type (modes 1 / 2, no resid), returned widened to fp32
+ *   INPLACE out is preloaded with resid and passed as the residual too (the engine's o-proj / down-proj without split-K)
+ *   PDL     launched with programmatic dependent launch behind the kernel that converts A (modes 1 / 2; the launch then never
+ *           goes to the wide-tile kernel)
+ * Rejected before any launch: unknown bits, OUT16 / PDL in mode 0, INPLACE without resid or with OUT16, K % 64 or N % 32 in
+ * modes 1 / 2.  iters > 0: *ms_per_iter = mean time of that many further launches. */
+#define XTTS_DEBUG_GEMM_GELU 1
+#define XTTS_DEBUG_GEMM_OUT16 2
+#define XTTS_DEBUG_GEMM_INPLACE 4
+#define XTTS_DEBUG_GEMM_PDL 8
 int xtts_debug_gemm(xtts_engine* e, int32_t mode, const float* A, const float* W, const float* bias, const float* resid,
-                    float* out, int32_t M, int32_t N, int32_t K, int32_t gelu, int32_t iters, float* ms_per_iter);
+                    float* out, int32_t M, int32_t N, int32_t K, int32_t flags, int32_t iters, float* ms_per_iter);
 /* debug timeline: op 1 arms %globaltimer stamps in the decode / vocoder kernels (first and last CTA: entry, dependency
  * resolved, exit), op 0 disarms and copies up to `cap` records [n][2] u64 = (ns, id<<32 | grid<<40 | last<<8 | phase) into
  * `out`; returns the count (>= 0) or a negative error.  Nothing is serialised: shows the step as it really runs. */
@@ -285,6 +298,45 @@ int xtts_debug_attn_prefill(xtts_engine* e, int32_t out_type, int32_t heads, con
  * 16-bit type (returned as fp32); ln_w = ln_b = NULL: X only (the last layer) */
 int xtts_debug_splitk_ln(xtts_engine* e, int32_t mode, int32_t M, int32_t N, int32_t K, int32_t splits, const float* A,
                          const float* W, const float* bias, float* X, const float* ln_w, const float* ln_b, float* Y);
+/* the decode step's LayerNorm -> GEMM pair as the fast-mode decode launches it (mode 1 bf16 / 2 fp16): Y [M,K] =
+ * LayerNorm(X [M,K]; ln_w, ln_b, the engine's eps) in the 16-bit type (returned as fp32), then out [M,N] = epi(Y . W^T + bias)
+ * + resid on the one-tile GEMM, flags XTTS_DEBUG_GEMM_GELU / OUT16 only (OUT16: 16-bit out, returned as fp32, no resid).
+ * launch 0: plain launches; 1: both with PDL; 2: PDL plus dependency counters (LN counts its M CTAs into counters[0], the
+ * GEMM waits for counters[0] == M instead of griddepcontrol.wait and counts its CTAs into counters[1]).  *n_ctas = the CTA
+ * count the GEMM launcher returned; counters [2] = their final values (0 unless launch 2).  Rejected before any launch: a
+ * resid with launch 2 (a counter cannot order the residual read), N % 32, K % 64, K > 8192, NULL except bias / resid. */
+int xtts_debug_ln_gemm(xtts_engine* e, int32_t mode, int32_t launch, int32_t M, int32_t N, int32_t K, const float* X,
+                       const float* ln_w, const float* ln_b, const float* W, const float* bias, const float* resid, int32_t flags,
+                       float* Y, float* out, int32_t* n_ctas, uint32_t* counters);
+/* LayerNorms in the output type out_type (0 fp32, 1 bf16, 2 fp16; returned as fp32), eps = the engine's, H <= 8192.
+ * w2 == b2 == NULL: Y[i] = LN(X[i]; w1, b1) for i < M (row_index, latents NULL; x_rows >= M).
+ * w2 != NULL, the GPT head: r = row_index ? row_index[i] : i (< x_rows), y = LN(LN(X[r]; w1, b1); w2, b2), Y[i] = y, and with
+ * latents [n_slots][lat_rows][H] (in/out, may be NULL): latents[slots[i]][p] = LN(y; w2, b2), p = lat_pos ? lat_pos[i] :
+ * n_gen[slots[i]], written only when 0 <= p < lat_rows.  Rejected before any launch: a row index outside X, a slot outside
+ * n_slots, latents without slots / lat_rows / lat_pos or n_gen. */
+int xtts_debug_norms(xtts_engine* e, int32_t out_type, int32_t M, int32_t H, const float* X, int32_t x_rows,
+                     const int32_t* row_index, const float* w1, const float* b1, const float* w2, const float* b2, float* Y,
+                     float* latents, int32_t n_slots, int32_t lat_rows, const int32_t* slots, const int32_t* lat_pos,
+                     const int32_t* n_gen);
+/* the prefill's paged-cache write: k / v of QKV row r (qkv [M][3 * heads * 64]) go to slot row_slot[r] at token position
+ * p = row_pos ? row_pos[r] : ctx_len[row_slot[r]], page block_tables[slot][p / 32], rounded to kv_type (0 fp32, 1 bf16,
+ * 2 fp16).  kpool / vpool: raw pools in the layout of xtts_debug_attn_decode, updated in place.  Rejected before any
+ * launch: a slot outside n_slots, a position outside the block table, a page id outside the pool. */
+int xtts_debug_kv_write(xtts_engine* e, int32_t kv_type, int32_t heads, int32_t M, const float* qkv, const int32_t* row_slot,
+                        const int32_t* row_pos, int32_t n_slots, const int32_t* ctx_len, const int32_t* block_tables,
+                        int32_t max_pages, int32_t n_pages, void* kpool, void* vpool);
+/* prompt row build over private fp32 tables [rows][H] (H % 4 == 0): rows [n_rows][4] = (kind, a, b, c) as the engine builds
+ * them: kind 0 X = spk_cond[c][a] (spk_cond [n_spk][n_cond][H]); 1 X = text_emb[a] + text_pos[b]; 2 X = wte[a] + wpe[b].
+ * Rejected before any launch: another kind, an index outside its table. */
+int xtts_debug_build_rows(xtts_engine* e, int32_t H, int32_t n_cond, const float* text_emb, int32_t n_text, const float* text_pos,
+                          int32_t n_text_pos, const float* wte, int32_t n_audio, const float* wpe, int32_t n_wpe,
+                          const float* spk_cond, int32_t n_spk, const int32_t* rows, int32_t n_rows, float* X);
+/* decode row build: X[i] = wte[last_tok[s]] + wpe[n_gen[s]], s = active[i] < n_slots; counters [n_words] in/out: the kernel
+ * zeroes the first n_flags words (the step's dependency counters) and must leave the rest alone.  Launched with PDL when
+ * option "pdl" is on.  Rejected before any launch: a slot, token or position outside its table, n_flags > n_words. */
+int xtts_debug_build_decode_rows(xtts_engine* e, int32_t H, const float* wte, int32_t n_audio, const float* wpe, int32_t n_wpe,
+                                 int32_t M, const int32_t* active, int32_t n_slots, const int32_t* last_tok, const int32_t* n_gen,
+                                 float* X, uint32_t* counters, int32_t n_flags, int32_t n_words);
 /* fast-mode vocoder convolution on the tensor cores (fp16 operands, fp32 accumulate), weights packed as the engine packs
  * them.  up 0: Conv1d(Cin -> Cout, odd K, dilation dil, "same" padding), w [Cout][Cin][K]; up u in {2, 4, 8}:
  * ConvTranspose1d(Cin -> Cout, kernel K = 2u, stride u, padding u/2), w [Cin][Cout][2u], dil 1, no resid, mode 0,
