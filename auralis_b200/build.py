@@ -11,7 +11,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libxtts_b200.so")
-SOURCES = ["engine.cu", "gpt_kernels.cu", "gemm_simt.cu", "gemm_wgmma.cu", "gemm_wgmma_wide.cu", "vocoder.cu", "conv1d_tc.cu", "cond.cu", "enhance.cu", "pvoc.cu"]
+SOURCES = ["engine.cu", "gpt_kernels.cu", "gemm_simt.cu", "gemm_wgmma.cu", "gemm_wgmma_wide.cu", "vocoder.cu", "conv1d_tc.cu", "cond.cu", "enhance.cu", "pvoc.cu", "flac.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [*ARCH, "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-pthread"]

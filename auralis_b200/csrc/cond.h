@@ -107,4 +107,25 @@ private:
     std::unique_ptr<Impl> impl;
 };
 
+// FLAC encoder (flac.cu): mono 16-bit PCM -> a complete lossless FLAC stream (RFC 9639), for TTSOutput.to_bytes("flac").
+// Needs no weights.  Works in batches of at most `batch_frames` 4096-sample frames, so its device memory does not grow
+// with the input; only the host holds the whole input and stream.
+class FlacEncoder {
+public:
+    explicit FlacEncoder(cudaStream_t st);
+    ~FlacEncoder();
+    // The most bytes a stream of n samples can take: 42 + ceil(n / 4096) * 8211.
+    static int64_t max_bytes(int64_t n);
+    // pcm: host, n samples.  md5: 16 bytes or NULL (zeros).  Writes the stream to `out` (host) and its length to
+    // *n_out, which is always set (the needed length when cap is too small).  Throws std::invalid_argument for a sample
+    // rate outside 1 .. 2^20 - 1, n < 0, a NULL input with n > 0, or cap < *n_out.  The bytes do not depend on
+    // batch_frames.
+    int64_t run(const int16_t* pcm, int64_t n, int sample_rate, const uint8_t* md5, uint8_t* out, int64_t cap,
+                int batch_frames, int64_t* n_out);
+
+private:
+    struct Impl;
+    std::unique_ptr<Impl> impl;
+};
+
 }  // namespace xtts

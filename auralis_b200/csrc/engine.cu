@@ -159,6 +159,8 @@ public:
     void condition(int slot, const float* w22, int64_t n22, const float* w16, int64_t n16, int cond_len, int chunk_len);
     int64_t enhance(const float* wav, int64_t n, const xtts_enhance_config& c, float* out, int64_t cap);
     int64_t change_speed(const float* wav, int64_t n, double rate, float* out, int64_t cap);
+    int64_t encode_flac(const int16_t* pcm, int64_t n, int sample_rate, const uint8_t* md5, uint8_t* out, int64_t cap,
+                        int64_t* n_out);
     void submit(uint64_t id, const int32_t* text, int n_text, int speaker, const xtts_sampling& sp, float speed);
     void cancel(uint64_t id);
     int poll(xtts_result* out, int timeout_ms);
@@ -252,6 +254,8 @@ private:
     std::unique_ptr<Enhancer> enhancer;          // built on the first xtts_enhance
     std::unique_ptr<PhaseVocoder> pvoc;          // built on the first xtts_change_speed
     int pvoc_block_frames = 4096;                // option "pvoc_block_frames"
+    std::unique_ptr<FlacEncoder> flac;           // built on the first xtts_encode_flac
+    int flac_batch_frames = 8192;                // option "flac_batch_frames"
 
     // ---- speakers
     DBuf<float> spk_cond, spk_g, spk_cbias;
@@ -878,6 +882,18 @@ int64_t Engine::change_speed(const float* wav, int64_t n, double rate, float* ou
     const int64_t n_out = pvoc->run(wav, n, rate, out, cap, pvoc_block_frames);
     st_cond_ms += (now_s() - t0) * 1e3;
     return n_out;
+}
+
+// TTSOutput.to_bytes("flac") (output.py:119-187): a lossless FLAC stream of 16-bit PCM, on the conditioning stream
+int64_t Engine::encode_flac(const int16_t* pcm, int64_t n, int sample_rate, const uint8_t* md5, uint8_t* out,
+                            int64_t cap, int64_t* n_out) {
+    ApiLock lk(this);
+    CUDA_CHECK(cudaSetDevice(cfg.device));
+    const double t0 = now_s();
+    if (!flac) flac.reset(new FlacEncoder(st));
+    const int64_t n_bytes = flac->run(pcm, n, sample_rate, md5, out, cap, flac_batch_frames, n_out);
+    st_cond_ms += (now_s() - t0) * 1e3;
+    return n_bytes;
 }
 
 void Engine::get_speaker(int slot, float* cond, float* g) {
@@ -1997,6 +2013,10 @@ void Engine::set_option(const std::string& k, int64_t v) {
         if (v < 1 || v > (1 << 20)) throw std::runtime_error("pvoc_block_frames: 1 .. 2^20 output frames");
         pvoc_block_frames = (int)v;
     }
+    else if (k == "flac_batch_frames") {
+        if (v < 1 || v > (1 << 20)) throw std::runtime_error("flac_batch_frames: 1 .. 2^20 frames");
+        flac_batch_frames = (int)v;
+    }
     else if (k == "voc_batch") voc_max_items = (int)std::max<int64_t>(1, std::min<int64_t>(v, kVocMaxItems));
     else if (k == "gemm_wide") {                                  // 0 off, else the wide kernel's ring depth
         if (v != 0 && (v < 2 || v > 4)) throw std::runtime_error("gemm_wide: 0 (off) or a ring depth of 2, 3 or 4");
@@ -2888,6 +2908,12 @@ int xtts_change_speed(xtts_engine* e, const float* wav, int64_t n, double rate, 
     if (!n_out) { xtts::set_error("null argument"); return XTTS_ERR_INVALID; }
     *n_out = xtts::PhaseVocoder::out_len(n, rate);
     XTTS_TRY(*n_out = e->impl->change_speed(wav, n, rate, out, cap))
+}
+int xtts_encode_flac(xtts_engine* e, const int16_t* pcm, int64_t n, int32_t sample_rate, const uint8_t* md5,
+                     uint8_t* out, int64_t cap, int64_t* n_out) {
+    if (!n_out) { xtts::set_error("null argument"); return XTTS_ERR_INVALID; }
+    *n_out = 0;
+    XTTS_TRY(e->impl->encode_flac(pcm, n, sample_rate, md5, out, cap, n_out))
 }
 int xtts_submit(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
                 const xtts_sampling* sp) {

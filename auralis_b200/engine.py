@@ -152,7 +152,7 @@ class XTTSv2Engine(BaseAsyncTTSEngine):
         self._pollers = [threading.Thread(target=self._poll_loop, args=(i,), name=f"xtts-poll-{i}", daemon=True)
                          for i in range(len(self.natives))]
         [t.start() for t in self._pollers]
-        _output.register_gpu_provider(self)             # TTSOutput.change_speed runs here while this engine lives
+        _output.register_gpu_provider(self)             # change_speed and to_bytes("flac") run here while it lives
 
     # ---- plugin API -------------------------------------------------------------------------
     @classmethod
@@ -468,6 +468,17 @@ class XTTSv2Engine(BaseAsyncTTSEngine):
         <= 0, a non-finite sample, a factor that leaves one STFT frame) raises ValueError."""
         try:
             return self.native.change_speed(np.asarray(array, np.float32), float(speed_factor))
+        except native.NativeError as e:
+            if e.code == native.ERR_INVALID:
+                raise ValueError(str(e)) from e
+            raise
+
+    def encode_flac(self, pcm_i16, sample_rate: int, md5: Optional[bytes] = None) -> bytes:
+        """`TTSOutput.to_bytes("flac")` on the first GPU (``xtts_encode_flac``): a lossless FLAC stream of mono int16
+        samples, with `md5` (16 bytes, or None for zeros) in its STREAMINFO.  A sample rate outside 1 .. 1048575 raises
+        ValueError."""
+        try:
+            return self.native.encode_flac(pcm_i16, int(sample_rate), md5)
         except native.NativeError as e:
             if e.code == native.ERR_INVALID:
                 raise ValueError(str(e)) from e

@@ -94,7 +94,7 @@ class XttsKernelProfile(C.Structure):
 # every symbol include/xtts_b200.h declares (checked by tests/test_abi.py against the header text)
 ABI_SYMBOLS = [
     "xtts_last_error", "xtts_version", "xtts_create", "xtts_destroy", "xtts_load_weight", "xtts_finalize_weights",
-    "xtts_set_speaker", "xtts_get_speaker", "xtts_condition", "xtts_enhance", "xtts_change_speed", "xtts_submit", "xtts_submit_speed", "xtts_cancel", "xtts_poll",
+    "xtts_set_speaker", "xtts_get_speaker", "xtts_condition", "xtts_enhance", "xtts_change_speed", "xtts_encode_flac", "xtts_submit", "xtts_submit_speed", "xtts_cancel", "xtts_poll",
     "xtts_fetch", "xtts_set_option", "xtts_get_stats", "xtts_sync", "xtts_get_kernel_profile", "xtts_device_timer", "xtts_vocode",
     "xtts_vocode_window", "xtts_vocode_speed", "xtts_gpt_prefill", "xtts_gpt_teacher_forced",
     "xtts_debug_gemm", "xtts_debug_sample_slots", "xtts_debug_trace",
@@ -129,6 +129,8 @@ def load_library(path: Optional[str] = None):
     lib.xtts_condition.argtypes = [vp, i32, f32p, i64, f32p, i64, i32, i32]
     lib.xtts_enhance.argtypes = [vp, f32p, i64, C.POINTER(XttsEnhanceConfig), f32p, i64, C.POINTER(i64)]
     lib.xtts_change_speed.argtypes = [vp, f32p, i64, C.c_double, f32p, i64, C.POINTER(i64)]
+    u8p = C.POINTER(C.c_uint8)
+    lib.xtts_encode_flac.argtypes = [vp, C.POINTER(C.c_int16), i64, i32, u8p, u8p, i64, C.POINTER(i64)]
     lib.xtts_submit.argtypes = [vp, C.c_uint64, i32p, i32, i32, C.POINTER(XttsSampling)]
     lib.xtts_submit_speed.argtypes = [vp, C.c_uint64, i32p, i32, i32, C.POINTER(XttsSampling), C.c_float]
     lib.xtts_cancel.argtypes = [vp, C.c_uint64]
@@ -327,6 +329,23 @@ class NativeEngine:
         out = np.empty((max(cap, 1),), np.float32)
         self._chk(self.lib.xtts_change_speed(self.h, _fp(a), a.size, rate, _fp(out), cap, C.byref(n_out)), "change_speed")
         return out[: n_out.value]
+
+    def encode_flac(self, pcm_i16, sample_rate: int, md5: Optional[bytes] = None) -> bytes:
+        """xtts_encode_flac: a lossless FLAC stream of mono int16 samples, encoded on the GPU.  `md5` is the 16-byte MD5
+        of the samples as little-endian bytes for STREAMINFO, or None (zeros, "not computed").  Raises NativeError with
+        code ERR_INVALID for a sample rate outside 1 .. 1048575."""
+        a = np.ascontiguousarray(pcm_i16).reshape(-1)
+        if a.dtype != np.int16:
+            raise TypeError(f"encode_flac takes int16 samples, not {a.dtype}")
+        if md5 is not None and len(md5) != 16:
+            raise ValueError("md5 must be 16 bytes")
+        digest = None if md5 is None else (C.c_uint8 * 16).from_buffer_copy(bytes(md5))
+        out = np.empty((42 + -(-a.size // 4096) * 8211,), np.uint8)       # no frame is larger than VERBATIM
+        n_out = C.c_int64(0)
+        u8p = C.POINTER(C.c_uint8)
+        self._chk(self.lib.xtts_encode_flac(self.h, a.ctypes.data_as(C.POINTER(C.c_int16)), a.size, int(sample_rate),
+                                            digest, out.ctypes.data_as(u8p), out.size, C.byref(n_out)), "encode_flac")
+        return out[: n_out.value].tobytes()
 
     # ---- generation
     def submit(self, seq_id: int, text_ids, speaker_slot: int, sp: Sampling):

@@ -1,14 +1,15 @@
 """TTSOutput — the boundary type of the hot path (array/sample_rate/token_length/start_time).
 
 Mirrors `/root/reference/src/auralis/common/definitions/output.py:17-38,95-111` for the fields and
-``combine_outputs``.  ``change_speed`` (the reference's librosa phase vocoder + peak normalisation) runs on the GPU of a
-live `XTTSv2Engine` (``register_gpu_provider``), and on librosa when no engine is alive.  The other audio utilities
-(mp3/opus/aac encoders, playback) are CPU post-processing outside the hot path (SURVEY.md §2.1 #3): wav/pcm/flac-free
-paths are provided with the standard library, the rest raise with a clear message when their optional dependency is
-absent.
+``combine_outputs``.  ``change_speed`` (the reference's librosa phase vocoder + peak normalisation) and 16-bit FLAC
+(``to_bytes("flac")``, a lossless LPC + partitioned-Rice encoder) run on the GPU of a live `XTTSv2Engine`
+(``register_gpu_provider``), and on librosa / torchaudio when no engine is alive.  The other audio utilities (mp3/opus/aac
+encoders, playback) are CPU post-processing outside the hot path (SURVEY.md §2.1 #3): wav/pcm paths are provided with the
+standard library, the rest raise with a clear message when their optional dependency is absent.
 """
 from __future__ import annotations
 
+import hashlib
 import io
 import threading
 import wave
@@ -85,8 +86,9 @@ _providers_lock = threading.Lock()
 
 
 def register_gpu_provider(engine) -> None:
-    """Route `TTSOutput.change_speed` to `engine.change_speed(array, speed_factor) -> np.ndarray` while the engine is
-    alive (`XTTSv2Engine` registers itself when it is built).  Held through a weak reference, so the registry never keeps
+    """Route `TTSOutput.change_speed` to `engine.change_speed(array, speed_factor) -> np.ndarray`, and 16-bit
+    `TTSOutput.to_bytes("flac")` to `engine.encode_flac(pcm_i16, sample_rate, md5) -> bytes` when the engine has that
+    method, while the engine is alive (`XTTSv2Engine` registers itself when it is built).  Held through a weak reference, so the registry never keeps
     an engine alive; the most recently registered live engine serves."""
     with _providers_lock:
         _providers[:] = [r for r in _providers if r() is not None and r() is not engine]
@@ -100,7 +102,7 @@ def unregister_gpu_provider(engine) -> None:
 
 
 def gpu_provider():
-    """The engine `TTSOutput.change_speed` runs on, or None."""
+    """The engine `TTSOutput.change_speed` and `TTSOutput.to_bytes("flac")` run on, or None."""
     with _providers_lock:
         for r in reversed(_providers):
             e = r()
@@ -175,7 +177,14 @@ class TTSOutput:
         return self.array
 
     def to_bytes(self, format: str = "wav", sample_width: int = 2) -> bytes:
-        """output.py:119-187; wav and pcm are native here, compressed codecs need torchaudio+ffmpeg."""
+        """output.py:119-187; wav and pcm are native here, mp3/opus/aac need torchaudio+ffmpeg.
+
+        ``flac`` at ``sample_width=2`` (the only width at which the reference writes 16-bit FLAC; it asks for PCM_F at
+        any other) runs on the GPU while an `XTTSv2Engine` is alive: the samples are quantised exactly as ``pcm`` /
+        ``wav`` quantise them, so the stream decodes to the very samples ``to_bytes("pcm", 2)`` returns, and their MD5
+        goes into STREAMINFO.  There is one configuration (fixed 4096-sample blocks, FIXED and LPC predictors up to
+        order 12, partitioned Rice residuals): ``compression`` selects nothing on that path.  With no engine alive, with
+        one that cannot encode FLAC, or at another width, flac goes through torchaudio like the other codecs."""
         wav = np.clip(np.asarray(self.array, dtype=np.float32), -1.0, 1.0)
         if format == "pcm":
             if sample_width == 2:
@@ -194,6 +203,11 @@ class TTSOutput:
                     w.writeframes((wav * 32767).astype(np.int16).tobytes())
                 return buf.getvalue()
             return _riff_wav(wav, self.sample_rate, 8 * sample_width)
+        if format == "flac" and sample_width == 2:
+            gpu = gpu_provider()
+            if gpu is not None and hasattr(gpu, "encode_flac"):
+                pcm = (wav * 32767).astype(np.int16)
+                return gpu.encode_flac(pcm, self.sample_rate, hashlib.md5(pcm.astype("<i2").tobytes()).digest())
         if format in ("flac", "mp3", "opus", "aac"):
             try:
                 import torch

@@ -154,6 +154,22 @@ int xtts_enhance(xtts_engine* e, const float* wav, int64_t n, const xtts_enhance
  * Runs on the conditioning stream; its time counts in xtts_stats.cond_ms. */
 int xtts_change_speed(xtts_engine* e, const float* wav, int64_t n, double rate, float* out, int64_t cap, int64_t* n_out);
 
+/* TTSOutput.to_bytes("flac") (output.py:119-187): a complete, lossless FLAC stream (RFC 9639) of n mono 16-bit samples
+ * at sample_rate Hz, encoded on the GPU.  "fLaC", one STREAMINFO block (min/max block size 4096, the real min/max frame
+ * sizes, total samples n, the 16-byte md5 the caller passes or zeros for NULL = "not computed"), then fixed blocks of
+ * 4096 samples (the last holds the remainder), 16 bits, no wasted bits.  Each block keeps the smallest of these
+ * subframes, exactly costed in bits (ties: the first): CONSTANT (all samples equal), VERBATIM, FIXED orders 0..4, LPC
+ * orders 1..12 at 12-bit precision with shift 0..15 (Tukey(0.5)-windowed fp64 autocorrelation, Levinson-Durbin; an
+ * order whose residual would reach |r| >= 2^31 is dropped).  An order o is tried only on blocks of more than o
+ * samples; a 1-sample block is CONSTANT.  Residuals: partitioned Rice (method 00, parameters 0..14, no escape),
+ * partition orders 0..6 where the block allows, each parameter by exact cost.  No subframe is larger than VERBATIM, so
+ * the stream is at most 42 + ceil(n / 4096) * 8211 bytes.  *n_out is always set (the length needed when cap is too
+ * small); cap < *n_out fails.  XTTS_ERR_INVALID: sample_rate outside 1 .. 1048575, n < 0, a NULL pcm with n > 0,
+ * cap < *n_out.  n == 0 gives STREAMINFO and no frames.  Works in batches of at most "flac_batch_frames" frames (the
+ * bytes are identical for every value).  Runs on the conditioning stream; its time counts in xtts_stats.cond_ms. */
+int xtts_encode_flac(xtts_engine* e, const int16_t* pcm, int64_t n, int32_t sample_rate, const uint8_t* md5,
+                     uint8_t* out, int64_t cap, int64_t* n_out);
+
 /* llm_engine.generate(...) per text chunk (XTTSv2.py:741-757): text_ids = [bos]+bpe+[eos] (XTTSv2.py:519-522).
  * Asynchronous: the scheduler thread admits, prefills, decodes (continuous batching), vocodes. */
 int xtts_submit(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
@@ -195,6 +211,9 @@ int xtts_fetch(xtts_engine* e, uint64_t seq_id, int32_t* tokens, float* wav, flo
  *   "pvoc_block_frames"   xtts_change_speed's block: at most this many output STFT frames (and this many + 2 input frames)
  *                         per pass, 1 .. 2^20, default 4096 (a spectral workspace of about 45 KB per frame, ~185 MB,
  *                         whatever the input length).  Bit-identical results for every value.
+ *   "flac_batch_frames"   xtts_encode_flac's batch: at most this many 4096-sample frames on the device at once, 1 .. 2^20,
+ *                         default 8192 (about 16 KB of device memory per frame, ~135 MB, whatever the input length).
+ *                         Identical bytes for every value.
  *   "tc_epilogue"         epilogue of the fast-mode vocoder's tensor-core Conv1d: 1 (default) = staged through shared
  *                         memory (residual prefetched by a loader warp, outputs drained by bulk copies while the next
  *                         tile's MMAs run), 0 = straight from the accumulators.  Bit-identical results either way.
