@@ -128,4 +128,24 @@ private:
     std::unique_ptr<Impl> impl;
 };
 
+// FLAC decoder (flac.cu): a FLAC stream (RFC 9639: 1-8 channels, 4-32 bits, fixed or variable blocking, every
+// subframe and residual coding) -> planar int32 samples, for speaker references and TTSOutput.from_file.  Frame
+// headers are found by a scan of every byte position on the device; frames are decoded in parallel, in batches of at
+// most `batch_frames` frames and batch_frames * 4096 samples (all channels; one larger frame is a batch alone).
+class FlacDecoder {
+public:
+    explicit FlacDecoder(cudaStream_t st);
+    ~FlacDecoder();
+    // data: host, n bytes.  Fills *info as soon as STREAMINFO parses (total_samples: STREAMINFO's once the data can
+    // hold it, the decoded count at the end).
+    // Writes [channels][total] int32 to `out` (host) and returns total.  Throws std::invalid_argument for a stream
+    // that breaks the format or fails a check, and for cap < channels * total.  The samples do not depend on
+    // batch_frames.
+    int64_t run(const uint8_t* data, int64_t n, int32_t* out, int64_t cap, int batch_frames, xtts_flac_info* info);
+
+private:
+    struct Impl;
+    std::unique_ptr<Impl> impl;
+};
+
 }  // namespace xtts

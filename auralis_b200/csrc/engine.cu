@@ -161,6 +161,7 @@ public:
     int64_t change_speed(const float* wav, int64_t n, double rate, float* out, int64_t cap);
     int64_t encode_flac(const int16_t* pcm, int64_t n, int sample_rate, const uint8_t* md5, uint8_t* out, int64_t cap,
                         int64_t* n_out);
+    int64_t decode_flac(const uint8_t* data, int64_t n, int32_t* out, int64_t cap, xtts_flac_info* info);
     void submit(uint64_t id, const int32_t* text, int n_text, int speaker, const xtts_sampling& sp, float speed);
     void cancel(uint64_t id);
     int poll(xtts_result* out, int timeout_ms);
@@ -255,7 +256,8 @@ private:
     std::unique_ptr<PhaseVocoder> pvoc;          // built on the first xtts_change_speed
     int pvoc_block_frames = 4096;                // option "pvoc_block_frames"
     std::unique_ptr<FlacEncoder> flac;           // built on the first xtts_encode_flac
-    int flac_batch_frames = 8192;                // option "flac_batch_frames"
+    std::unique_ptr<FlacDecoder> flac_dec;       // built on the first xtts_decode_flac
+    int flac_batch_frames = 8192;                // option "flac_batch_frames" (encoder and decoder)
 
     // ---- speakers
     DBuf<float> spk_cond, spk_g, spk_cbias;
@@ -894,6 +896,17 @@ int64_t Engine::encode_flac(const int16_t* pcm, int64_t n, int sample_rate, cons
     const int64_t n_bytes = flac->run(pcm, n, sample_rate, md5, out, cap, flac_batch_frames, n_out);
     st_cond_ms += (now_s() - t0) * 1e3;
     return n_bytes;
+}
+
+// FLAC input (engine.load_audio, TTSOutput.from_file): a FLAC stream -> planar int32 samples, on the conditioning stream
+int64_t Engine::decode_flac(const uint8_t* data, int64_t n, int32_t* out, int64_t cap, xtts_flac_info* info) {
+    ApiLock lk(this);
+    CUDA_CHECK(cudaSetDevice(cfg.device));
+    const double t0 = now_s();
+    if (!flac_dec) flac_dec.reset(new FlacDecoder(st));
+    const int64_t total = flac_dec->run(data, n, out, cap, flac_batch_frames, info);
+    st_cond_ms += (now_s() - t0) * 1e3;
+    return total;
 }
 
 void Engine::get_speaker(int slot, float* cond, float* g) {
@@ -2914,6 +2927,12 @@ int xtts_encode_flac(xtts_engine* e, const int16_t* pcm, int64_t n, int32_t samp
     if (!n_out) { xtts::set_error("null argument"); return XTTS_ERR_INVALID; }
     *n_out = 0;
     XTTS_TRY(e->impl->encode_flac(pcm, n, sample_rate, md5, out, cap, n_out))
+}
+int xtts_decode_flac(xtts_engine* e, const uint8_t* data, int64_t n_bytes, int32_t* out, int64_t cap,
+                     xtts_flac_info* info) {
+    if (!info) { xtts::set_error("null argument"); return XTTS_ERR_INVALID; }
+    std::memset(info, 0, sizeof(*info));
+    XTTS_TRY(e->impl->decode_flac(data, n_bytes, out, cap, info))
 }
 int xtts_submit(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
                 const xtts_sampling* sp) {

@@ -68,14 +68,19 @@ class ChunkOutput:
 def load_audio(source: Union[str, Path, bytes], sampling_rate: int) -> np.ndarray:
     """Mono float32 in [-1,1] at `sampling_rate` (common/utilities.py:72-97: mean over channels, torchaudio sinc resampling,
     clip).  RIFF/WAV — integer PCM and IEEE float — is decoded here (torchaudio.load needs a codec backend this image does
-    not ship); any other container goes through torchaudio.load when it can."""
-    from .output import _parse_riff_wav
+    not ship).  FLAC (optionally behind an ID3v2 tag) is decoded losslessly on the GPU while an `XTTSv2Engine` is alive
+    and scaled v / 2^(bits - 1) into the same [frames, channels] float32 array an integer WAV gives, so a FLAC
+    reference conditions exactly like the same PCM in a WAV; a corrupt stream raises ValueError.  Any other container,
+    and FLAC with no engine alive, goes through torchaudio.load when it can."""
+    from .output import _parse_flac, _parse_riff_wav
     if isinstance(source, (bytes, bytearray)):
         blob = bytes(source)
     else:
         with open(str(source), "rb") as f:
             blob = f.read()
     parsed = _parse_riff_wav(blob)
+    if parsed is None:
+        parsed = _parse_flac(blob)
     if parsed is None:
         import io
         import torchaudio
@@ -152,7 +157,7 @@ class XTTSv2Engine(BaseAsyncTTSEngine):
         self._pollers = [threading.Thread(target=self._poll_loop, args=(i,), name=f"xtts-poll-{i}", daemon=True)
                          for i in range(len(self.natives))]
         [t.start() for t in self._pollers]
-        _output.register_gpu_provider(self)             # change_speed and to_bytes("flac") run here while it lives
+        _output.register_gpu_provider(self)             # change_speed and FLAC output / input run here while it lives
 
     # ---- plugin API -------------------------------------------------------------------------
     @classmethod
@@ -479,6 +484,17 @@ class XTTSv2Engine(BaseAsyncTTSEngine):
         ValueError."""
         try:
             return self.native.encode_flac(pcm_i16, int(sample_rate), md5)
+        except native.NativeError as e:
+            if e.code == native.ERR_INVALID:
+                raise ValueError(str(e)) from e
+            raise
+
+    def decode_flac(self, data) -> Tuple[np.ndarray, int, int]:
+        """FLAC input (`TTSOutput.from_file`, `load_audio`) on the first GPU (``xtts_decode_flac``): a whole FLAC stream
+        -> (int32 [channels, samples], sample rate, bits per sample), lossless, its MD5 checked when STREAMINFO has one.
+        A stream that breaks the format or fails a check raises ValueError."""
+        try:
+            return self.native.decode_flac(data)
         except native.NativeError as e:
             if e.code == native.ERR_INVALID:
                 raise ValueError(str(e)) from e

@@ -7,6 +7,7 @@ The library is CUDA-only; creating an engine without an sm_90 GPU raises ``Nativ
 from __future__ import annotations
 
 import ctypes as C
+import hashlib
 import math
 import os
 from dataclasses import dataclass
@@ -86,6 +87,21 @@ class XttsEnhanceConfig(C.Structure):
         return c
 
 
+class XttsFlacInfo(C.Structure):
+    _fields_ = [("sample_rate", C.c_int32), ("channels", C.c_int32), ("bits_per_sample", C.c_int32),
+                ("min_block", C.c_int32), ("max_block", C.c_int32), ("total_samples", C.c_int64),
+                ("md5", C.c_uint8 * 16)]
+
+
+def flac_md5(samples: np.ndarray, bits_per_sample: int) -> bytes:
+    """The MD5 FLAC's STREAMINFO carries: samples [C, N] interleaved, little-endian, ceil(bps / 8) bytes each."""
+    nb = (bits_per_sample + 7) // 8
+    inter = np.ascontiguousarray(np.asarray(samples).T)
+    if nb in (1, 2, 4):
+        return hashlib.md5(inter.astype({1: "<i1", 2: "<i2", 4: "<i4"}[nb]).tobytes()).digest()
+    return hashlib.md5(inter.astype("<i4").view(np.uint8).reshape(-1, 4)[:, :nb].tobytes()).digest()
+
+
 class XttsKernelProfile(C.Structure):
     _fields_ = [("n", C.c_int32), ("name", (C.c_char * 32) * 16), ("ms", C.c_double * 16), ("flops", C.c_double * 16),
                 ("bytes", C.c_double * 16), ("launches", C.c_uint64 * 16)]
@@ -94,7 +110,7 @@ class XttsKernelProfile(C.Structure):
 # every symbol include/xtts_b200.h declares (checked by tests/test_abi.py against the header text)
 ABI_SYMBOLS = [
     "xtts_last_error", "xtts_version", "xtts_create", "xtts_destroy", "xtts_load_weight", "xtts_finalize_weights",
-    "xtts_set_speaker", "xtts_get_speaker", "xtts_condition", "xtts_enhance", "xtts_change_speed", "xtts_encode_flac", "xtts_submit", "xtts_submit_speed", "xtts_cancel", "xtts_poll",
+    "xtts_set_speaker", "xtts_get_speaker", "xtts_condition", "xtts_enhance", "xtts_change_speed", "xtts_encode_flac", "xtts_decode_flac", "xtts_submit", "xtts_submit_speed", "xtts_cancel", "xtts_poll",
     "xtts_fetch", "xtts_set_option", "xtts_get_stats", "xtts_sync", "xtts_get_kernel_profile", "xtts_device_timer", "xtts_vocode",
     "xtts_vocode_window", "xtts_vocode_speed", "xtts_gpt_prefill", "xtts_gpt_teacher_forced",
     "xtts_debug_gemm", "xtts_debug_sample_slots", "xtts_debug_trace",
@@ -131,6 +147,7 @@ def load_library(path: Optional[str] = None):
     lib.xtts_change_speed.argtypes = [vp, f32p, i64, C.c_double, f32p, i64, C.POINTER(i64)]
     u8p = C.POINTER(C.c_uint8)
     lib.xtts_encode_flac.argtypes = [vp, C.POINTER(C.c_int16), i64, i32, u8p, u8p, i64, C.POINTER(i64)]
+    lib.xtts_decode_flac.argtypes = [vp, u8p, i64, i32p, i64, C.POINTER(XttsFlacInfo)]
     lib.xtts_submit.argtypes = [vp, C.c_uint64, i32p, i32, i32, C.POINTER(XttsSampling)]
     lib.xtts_submit_speed.argtypes = [vp, C.c_uint64, i32p, i32, i32, C.POINTER(XttsSampling), C.c_float]
     lib.xtts_cancel.argtypes = [vp, C.c_uint64]
@@ -346,6 +363,28 @@ class NativeEngine:
         self._chk(self.lib.xtts_encode_flac(self.h, a.ctypes.data_as(C.POINTER(C.c_int16)), a.size, int(sample_rate),
                                             digest, out.ctypes.data_as(u8p), out.size, C.byref(n_out)), "encode_flac")
         return out[: n_out.value].tobytes()
+
+    def decode_flac(self, data) -> Tuple[np.ndarray, int, int]:
+        """xtts_decode_flac: a whole FLAC stream (bytes), decoded losslessly on the GPU -> (int32 [channels, samples],
+        sample rate, bits per sample); each sample is the signed integer the stream codes.  Sizes the output from the
+        call's own report (a stream whose STREAMINFO leaves the total at 0 is decoded twice), then checks STREAMINFO's
+        MD5 when it is set.  Raises NativeError with code ERR_INVALID for a stream that breaks the format or fails a
+        check, the MD5 included."""
+        buf = np.frombuffer(bytes(data), np.uint8)
+        u8p = C.POINTER(C.c_uint8)
+        info = XttsFlacInfo()
+        out = np.empty((0, 0), np.int32)
+        rc = self.lib.xtts_decode_flac(self.h, buf.ctypes.data_as(u8p), buf.size, None, 0, C.byref(info))
+        need = info.channels * info.total_samples
+        if rc == ERR_INVALID and need > 0:          # the output did not fit: allocate what the call reported
+            out = np.empty((info.channels, info.total_samples), np.int32)
+            rc = self.lib.xtts_decode_flac(self.h, buf.ctypes.data_as(u8p), buf.size, _ip(out), out.size, C.byref(info))
+        self._chk(rc, "decode_flac")
+        out = out.reshape(info.channels, info.total_samples)
+        md5 = bytes(info.md5)
+        if md5 != bytes(16) and flac_md5(out, info.bits_per_sample) != md5:
+            raise NativeError("decode_flac failed: MD5 mismatch", ERR_INVALID)
+        return out, int(info.sample_rate), int(info.bits_per_sample)
 
     # ---- generation
     def submit(self, seq_id: int, text_ids, speaker_slot: int, sp: Sampling):

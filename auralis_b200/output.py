@@ -1,9 +1,10 @@
 """TTSOutput — the boundary type of the hot path (array/sample_rate/token_length/start_time).
 
 Mirrors `/root/reference/src/auralis/common/definitions/output.py:17-38,95-111` for the fields and
-``combine_outputs``.  ``change_speed`` (the reference's librosa phase vocoder + peak normalisation) and 16-bit FLAC
-(``to_bytes("flac")``, a lossless LPC + partitioned-Rice encoder) run on the GPU of a live `XTTSv2Engine`
-(``register_gpu_provider``), and on librosa / torchaudio when no engine is alive.  The other audio utilities (mp3/opus/aac
+``combine_outputs``.  ``change_speed`` (the reference's librosa phase vocoder + peak normalisation), 16-bit FLAC
+(``to_bytes("flac")``, a lossless LPC + partitioned-Rice encoder) and FLAC input (``from_file``, a lossless RFC 9639
+decoder) run on the GPU of a live `XTTSv2Engine` (``register_gpu_provider``), and on librosa / torchaudio when no
+engine is alive.  The other audio utilities (mp3/opus/aac
 encoders, playback) are CPU post-processing outside the hot path (SURVEY.md §2.1 #3): wav/pcm paths are provided with the
 standard library, the rest raise with a clear message when their optional dependency is absent.
 """
@@ -81,15 +82,39 @@ def _parse_riff_wav(blob: bytes):
     return a[:n].reshape(-1, nch), int(sr)
 
 
+def _is_flac(blob: bytes) -> bool:
+    """A FLAC stream: "fLaC" at the start, or right after an ID3v2 tag."""
+    pos = 0
+    if blob[:3] == b"ID3" and len(blob) >= 10:
+        pos = 10 + ((blob[6] & 0x7F) << 21 | (blob[7] & 0x7F) << 14 | (blob[8] & 0x7F) << 7 | (blob[9] & 0x7F))
+        pos += 10 if blob[5] & 0x10 else 0
+    return blob[pos:pos + 4] == b"fLaC"
+
+
+def _parse_flac(blob: bytes):
+    """-> (float32 [frames, channels], sample_rate) of a FLAC stream, decoded by the live engine's `decode_flac`; None
+    when `blob` is not FLAC or no live engine can decode it.  Integer samples v become v / 2^(bits - 1), as
+    `_parse_riff_wav` (and torchaudio) scale integer PCM."""
+    if not _is_flac(blob):
+        return None
+    gpu = gpu_provider()
+    if gpu is None or not hasattr(gpu, "decode_flac"):
+        return None
+    samples, sr, bps = gpu.decode_flac(blob)
+    return np.ascontiguousarray(samples.T).astype(np.float32) / float(1 << (bps - 1)), int(sr)
+
+
 _providers: List["weakref.ref"] = []
 _providers_lock = threading.Lock()
 
 
 def register_gpu_provider(engine) -> None:
-    """Route `TTSOutput.change_speed` to `engine.change_speed(array, speed_factor) -> np.ndarray`, and 16-bit
-    `TTSOutput.to_bytes("flac")` to `engine.encode_flac(pcm_i16, sample_rate, md5) -> bytes` when the engine has that
-    method, while the engine is alive (`XTTSv2Engine` registers itself when it is built).  Held through a weak reference, so the registry never keeps
-    an engine alive; the most recently registered live engine serves."""
+    """Route `TTSOutput.change_speed` to `engine.change_speed(array, speed_factor) -> np.ndarray`, 16-bit
+    `TTSOutput.to_bytes("flac")` to `engine.encode_flac(pcm_i16, sample_rate, md5) -> bytes`, and FLAC input
+    (`TTSOutput.from_file`, `engine.load_audio`) to `engine.decode_flac(blob) -> (int32 [C, N], sample_rate,
+    bits_per_sample)`, each when the engine has that method, while the engine is alive (`XTTSv2Engine` registers itself
+    when it is built).  Held through a weak reference, so the registry never keeps an engine alive; the most recently
+    registered live engine serves."""
     with _providers_lock:
         _providers[:] = [r for r in _providers if r() is not None and r() is not engine]
         _providers.append(weakref.ref(engine))
@@ -102,7 +127,7 @@ def unregister_gpu_provider(engine) -> None:
 
 
 def gpu_provider():
-    """The engine `TTSOutput.change_speed` and `TTSOutput.to_bytes("flac")` run on, or None."""
+    """The engine `TTSOutput.change_speed`, `TTSOutput.to_bytes("flac")` and FLAC input run on, or None."""
     with _providers_lock:
         for r in reversed(_providers):
             e = r()
@@ -285,11 +310,16 @@ class TTSOutput:
     @classmethod
     def from_file(cls, filename: Union[str, Path]) -> "TTSOutput":
         """output.py:274-285.  RIFF/WAV through the standard library (the reference's torchaudio.load needs a codec
-        backend that this image does not ship); other containers go through torchaudio when it can load them."""
+        backend that this image does not ship); FLAC (optionally behind an ID3v2 tag) on the GPU while an
+        `XTTSv2Engine` is alive (lossless, scaled v / 2^(bits - 1) like integer WAV: mono gives [N], C channels [C, N];
+        a corrupt stream raises ValueError); other containers, and FLAC with no engine alive, go through torchaudio
+        when it can load them."""
         with open(str(filename), "rb") as f:
             blob = f.read()
         parsed = _parse_riff_wav(blob)
-        if parsed is None:                                   # not RIFF/WAVE (or an exotic encoding): torchaudio's loaders
+        if parsed is None:
+            parsed = _parse_flac(blob)
+        if parsed is None:                                   # not RIFF/WAVE or FLAC (or an exotic encoding): torchaudio's loaders
             import torchaudio
             wav, sr = torchaudio.load(str(filename))
             return cls.from_tensor(wav, sr)

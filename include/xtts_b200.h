@@ -170,6 +170,31 @@ int xtts_change_speed(xtts_engine* e, const float* wav, int64_t n, double rate, 
 int xtts_encode_flac(xtts_engine* e, const int16_t* pcm, int64_t n, int32_t sample_rate, const uint8_t* md5,
                      uint8_t* out, int64_t cap, int64_t* n_out);
 
+/* FLAC input for speaker references (engine.load_audio) and TTSOutput.from_file (common/utilities.py:72-97,
+ * output.py:274-285, where torchaudio.load decodes it through ffmpeg): a whole FLAC stream (RFC 9639) -> planar int32
+ * samples out[channels][total_samples], each the signed integer the frames code, right-aligned (lossless).  Accepts
+ * an ID3v2 tag before "fLaC", any metadata blocks after STREAMINFO, 1-8 channels, 4-32 bits per sample, fixed and
+ * variable blocking, independent / left-side / side-right / mid-side channels, CONSTANT, VERBATIM, FIXED 0-4 and LPC
+ * 1-32 subframes with wasted bits, RICE and RICE2 residuals with escapes and partition orders up to 15.  The stream
+ * ends after the frames holding STREAMINFO's total (trailing bytes are ignored); a total of 0 means the frames run to
+ * the end of the data, before a 128-byte ID3v1 "TAG" trailer if there is one, and the total is what they hold.
+ * *info is filled whenever the metadata parses (total_samples: the decoded count); cap < channels * total_samples
+ * fails with *info telling the caller what to allocate.  XTTS_ERR_INVALID, never a wrong sample, for: no "fLaC", a
+ * first block that is not a 34-byte STREAMINFO, block type 127, truncation anywhere, a sync code / reserved value /
+ * reserved bit / header field that disagrees with STREAMINFO, a CRC-8 or CRC-16 mismatch, frame or sample numbers
+ * out of sequence, a fixed-blocksize stream whose block size changes before its last frame, non-zero padding, LPC
+ * precision 1111 or a negative shift, a residual outside 32 bits, a sample outside its bit depth.  The MD5 is NOT
+ * checked here (native.py checks it).  Frames are found by a scan of every byte position on the GPU and decoded in
+ * batches of at most "flac_batch_frames" frames and flac_batch_frames * 4096 samples (identical samples for every
+ * value).  Runs on the conditioning stream; its time counts in xtts_stats.cond_ms. */
+typedef struct xtts_flac_info {
+    int32_t sample_rate, channels, bits_per_sample, min_block, max_block;
+    int64_t total_samples;          /* per channel, as decoded */
+    uint8_t md5[16];                /* STREAMINFO's; all zero = not set */
+} xtts_flac_info;
+int xtts_decode_flac(xtts_engine* e, const uint8_t* data, int64_t n_bytes, int32_t* out, int64_t cap,
+                     xtts_flac_info* info);
+
 /* llm_engine.generate(...) per text chunk (XTTSv2.py:741-757): text_ids = [bos]+bpe+[eos] (XTTSv2.py:519-522).
  * Asynchronous: the scheduler thread admits, prefills, decodes (continuous batching), vocodes. */
 int xtts_submit(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
@@ -213,7 +238,10 @@ int xtts_fetch(xtts_engine* e, uint64_t seq_id, int32_t* tokens, float* wav, flo
  *                         whatever the input length).  Bit-identical results for every value.
  *   "flac_batch_frames"   xtts_encode_flac's batch: at most this many 4096-sample frames on the device at once, 1 .. 2^20,
  *                         default 8192 (about 16 KB of device memory per frame, ~135 MB, whatever the input length).
- *                         Identical bytes for every value.
+ *                         Identical bytes for every value.  xtts_decode_flac's batch: at most this many frames and this
+ *                         many x 4096 samples, all channels together (one larger frame is a batch alone); about 4 B
+ *                         per sample (12 B at 32 bits) beside the compressed stream, which is whole on the device.
+ *                         Identical samples for every value.
  *   "tc_epilogue"         epilogue of the fast-mode vocoder's tensor-core Conv1d: 1 (default) = staged through shared
  *                         memory (residual prefetched by a loader warp, outputs drained by bulk copies while the next
  *                         tile's MMAs run), 0 = straight from the accumulators.  Bit-identical results either way.
