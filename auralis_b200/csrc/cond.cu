@@ -2,7 +2,9 @@
 // 1x1 convolution / nn.Linear is one call of the shared NT GEMM; the STFTs are DFT-by-GEMM against
 // precomputed (cos | -sin) bases restricted to the window support (n_fft 2048 -> 1024 live taps).
 // Per-speaker, cached by the engine: clarity over peak speed, fp32 throughout.
+#include <algorithm>
 #include <cmath>
+#include <cstring>
 #include <functional>
 
 #include "cond.h"
@@ -221,6 +223,82 @@ __global__ void power_kernel(const float* __restrict__ D, float* __restrict__ P,
     P[i] = re * re + im * im;
 }
 
+// ---------------------------------------------------------------------------------------- launches
+// One helper per kernel, called by Conditioner::run and by cond_debug (xtts_debug_cond), so a kernel under test runs with
+// the production grid, block size and shared memory.
+namespace {
+
+int conv_out(int n, int k, int stride) { return (n + 2 * (k / 2) - k) / stride + 1; }
+size_t conv2d_smem(int Cin, int k) { return (size_t)C2_CO * Cin * k * k * sizeof(float); }
+constexpr size_t kSmemLimit = 48 * 1024;           // dynamic shared memory without an opt-in attribute
+
+// block size: 256 threads for the 22.05 kHz front-end (wlen 1024), 128 for the 16 kHz one (wlen 400)
+void launch_frame_window(const float* x, int n, const float* win, int wlen, int hop, int off, int pad, int pad_mode, float* F,
+                         int frames, int threads, cudaStream_t st) {
+    frame_window_kernel<<<frames, threads, 0, st>>>(x, n, win, wlen, hop, off, pad, pad_mode, F, frames);
+    COUNT_LAUNCH(); KERNEL_CHECK();
+}
+void launch_power(const float* D, float* P, int frames, int nb, cudaStream_t st) {
+    power_kernel<<<nblk((size_t)frames * nb), 256, 0, st>>>(D, P, frames, nb); COUNT_LAUNCH(); KERNEL_CHECK();
+}
+void launch_mel_log(float* M, const float* stats, size_t n, int C, int mode, cudaStream_t st) {
+    mel_log_kernel<<<nblk(n), 256, 0, st>>>(M, stats, n, C, mode); COUNT_LAUNCH(); KERNEL_CHECK();
+}
+void launch_preemphasis(const float* x, float* y, int n, float coef, cudaStream_t st) {
+    preemphasis_kernel<<<nblk(n), 256, 0, st>>>(x, y, n, coef); COUNT_LAUNCH(); KERNEL_CHECK();
+}
+void launch_instnorm_t(const float* in, float* out, int T, int C, float eps, cudaStream_t st) {
+    instnorm_transpose_kernel<<<C, 256, 0, st>>>(in, out, T, C, eps); COUNT_LAUNCH(); KERNEL_CHECK();
+}
+void launch_groupnorm(const float* X, const float* w, const float* b, float* Y, int T, int C, int groups, float eps, cudaStream_t st) {
+    groupnorm_rows_kernel<<<groups, 256, 0, st>>>(X, w, b, Y, T, C, groups, eps); COUNT_LAUNCH(); KERNEL_CHECK();
+}
+void launch_geglu(const float* Hc, float* out, int rows, int F, cudaStream_t st) {
+    geglu_kernel<<<nblk((size_t)rows * F), 256, 0, st>>>(Hc, out, rows, F); COUNT_LAUNCH(); KERNEL_CHECK();
+}
+void launch_rmsnorm_accum(const float* X, const float* gamma, float* acc, int rows, int C, float scale, cudaStream_t st) {
+    rmsnorm_accum_kernel<<<rows, 256, 0, st>>>(X, gamma, acc, C, scale); COUNT_LAUNCH(); KERNEL_CHECK();
+}
+// out [Cout][Hout][Wout] must fit in `cap` floats; throws before the launch otherwise, or when the weight slice of C2_CO
+// output channels exceeds 48 KB of shared memory
+void launch_conv2d(const float* in, const float* w, const float* bias, const float* bn_scale, const float* bn_shift, float* out,
+                   size_t cap, int Cin, int Cout, int Hin, int Win, int k, int stride, int relu_before_bn, int& Hout, int& Wout,
+                   cudaStream_t st) {
+    Hout = conv_out(Hin, k, stride); Wout = conv_out(Win, k, stride);
+    if ((size_t)Cout * Hout * Wout > cap)
+        throw std::runtime_error("conv2d: output [" + std::to_string(Cout) + "][" + std::to_string(Hout) + "][" + std::to_string(Wout) +
+                                 "] exceeds its buffer of " + std::to_string(cap) + " floats");
+    if (conv2d_smem(Cin, k) > kSmemLimit) throw std::runtime_error("conv2d: weight slice exceeds 48 KB of shared memory");
+    dim3 grid(ceil_div(Wout, 128), Hout, ceil_div(Cout, C2_CO));
+    conv2d_kernel<<<grid, 128, conv2d_smem(Cin, k), st>>>(in, w, bias, bn_scale, bn_shift, out, Cin, Cout, Hin, Win, Hout, Wout, k,
+                                                           stride, relu_before_bn);
+    COUNT_LAUNCH(); KERNEL_CHECK();
+}
+void launch_channel_mean(const float* x, float* m, int C, int HW, cudaStream_t st) {
+    channel_mean_kernel<<<C, 256, 0, st>>>(x, m, HW); COUNT_LAUNCH(); KERNEL_CHECK();
+}
+void launch_se_gate(const float* m, const float* w1, const float* b1, const float* w2, const float* b2, float* gate, int C, int R,
+                    cudaStream_t st) {
+    se_gate_kernel<<<1, 256, (size_t)R * sizeof(float), st>>>(m, w1, b1, w2, b2, gate, C, R); COUNT_LAUNCH(); KERNEL_CHECK();
+}
+void launch_se_apply(const float* x, const float* gate, const float* resid, float* out, int HW, size_t n, cudaStream_t st) {
+    se_apply_kernel<<<nblk(n), 256, 0, st>>>(x, gate, resid, out, HW, n); COUNT_LAUNCH(); KERNEL_CHECK();
+}
+void launch_transpose(const float* in, float* out, int R, int Cc, cudaStream_t st) {
+    transpose_kernel<<<nblk((size_t)R * Cc), 256, 0, st>>>(in, out, R, Cc); COUNT_LAUNCH(); KERNEL_CHECK();
+}
+void launch_relu_bn_rows(float* X, const float* sc, const float* sh, size_t n, int C, cudaStream_t st) {
+    relu_bn_rows_kernel<<<nblk(n), 256, 0, st>>>(X, sc, sh, n, C); COUNT_LAUNCH(); KERNEL_CHECK();
+}
+void launch_asp(const float* A, const float* X, float* out, int T, int C, cudaStream_t st) {
+    asp_kernel<<<C, 128, 0, st>>>(A, X, out, T, C); COUNT_LAUNCH(); KERNEL_CHECK();
+}
+void launch_l2norm(float* x, int n, cudaStream_t st) {
+    l2norm_kernel<<<1, 256, 0, st>>>(x, n); COUNT_LAUNCH(); KERNEL_CHECK();
+}
+
+}  // namespace
+
 std::vector<float> dft_basis(int n_fft, int wlen, int off) {          // [(2*nb)][wlen]: cos rows then -sin rows
     const int nb = n_fft / 2 + 1;
     std::vector<float> B((size_t)2 * nb * wlen);
@@ -272,7 +350,7 @@ struct Conditioner::Impl {
     // speaker encoder
     Dev<float> conv1_w, conv1_b; Bn bn1; std::vector<std::unique_ptr<Block>> res; Lin att0, att3, fc; Bn att_bn;
     // workspaces
-    Dev<float> wav22, wav16, pre16, F, D, P, mel, h0, h1, xn, qkv, att, kvin, q, kv, o, lat, ff, gg, img, a0, a1, a2,
+    Dev<float> wav22, wav16, pre16, F, D, P, mel, h0, h1, xn, qkv, att, kvin, q, kv, o, lat, ff, gg, img, a0, a1, a2, ds,
         chm, gate, xT, at1, at2, pooled;
     Dev<AttnSeq> seq;
 
@@ -293,15 +371,35 @@ struct Conditioner::Impl {
     void gemm(const float* A, const Lin& l, const float* resid, float* out, int M, int flags = 0) {
         launch_gemm_f32(A, l.w.p, l.b.p, resid, out, M, l.N, l.K, flags | (resid ? GEMM_RESID : 0), st);
     }
-    void conv2d(const float* in, const float* w, const float* bias, const Bn* bnp, float* out, int Cin, int Cout, int Hin,
-                int Win, int k, int stride, int relu_before_bn, int& Hout, int& Wout) {
-        const int pad = k / 2;
-        Hout = (Hin + 2 * pad - k) / stride + 1; Wout = (Win + 2 * pad - k) / stride + 1;
-        dim3 grid(ceil_div(Wout, 128), Hout, ceil_div(Cout, C2_CO));
-        conv2d_kernel<<<grid, 128, (size_t)C2_CO * Cin * k * k * sizeof(float), st>>>(
-            in, w, bias, bnp ? bnp->scale.p : nullptr, bnp ? bnp->shift.p : nullptr, out, Cin, Cout, Hin, Win, Hout, Wout, k,
-            stride, relu_before_bn);
-        COUNT_LAUNCH(); KERNEL_CHECK();
+    // `cap`: floats `out` holds (launch_conv2d throws before launching when the output does not fit)
+    void conv2d(const float* in, const float* w, const float* bias, const Bn* bnp, float* out, size_t cap, int Cin, int Cout,
+                int Hin, int Win, int k, int stride, int relu_before_bn, int& Hout, int& Wout) {
+        launch_conv2d(in, w, bias, bnp ? bnp->scale.p : nullptr, bnp ? bnp->shift.p : nullptr, out, cap, Cin, Cout, Hin, Win, k,
+                      stride, relu_before_bn, Hout, Wout, st);
+    }
+    // 22.05 kHz front-end: x [len] (device) -> mel [1 + len/256][n_mels] (utilities.py:53-70 with XTTSv2.py:374-386)
+    void mel22(const float* x, int len, float* mel_out, size_t cap) {
+        const int T = 1 + len / 256, nb = 1025;
+        if ((size_t)T * c.n_mels > cap) throw std::runtime_error("mel22: output exceeds its buffer");
+        F.ensure((size_t)T * 1024); D.ensure((size_t)T * 2 * nb); P.ensure((size_t)T * nb);
+        launch_frame_window(x, len, hann.p, 1024, 256, 512, 1024, PAD_REFLECT, F.p, T, 256, st);
+        launch_gemm_f32(F.p, basis22.p, nullptr, nullptr, D.p, T, 2 * nb, 1024, 0, st);
+        launch_power(D.p, P.p, T, nb, st);
+        launch_gemm_f32(P.p, fb22.p, nullptr, nullptr, mel_out, T, c.n_mels, nb, 0, st);
+        launch_mel_log(mel_out, mel_stats.p, (size_t)T * c.n_mels, c.n_mels, 0, st);
+    }
+    // 16 kHz front-end: x [N] (device) -> InstanceNorm'd log-mel image [spk_mels][1 + N/160] (hifigan_decoder.py:602-613)
+    void mel16(const float* x, int N, float* img_out, size_t cap) {
+        const int T = 1 + N / 160, nb = 257, NM = c.spk_mels;
+        if ((size_t)NM * T > cap) throw std::runtime_error("mel16: output exceeds its buffer");
+        pre16.ensure(N); F.ensure((size_t)T * 400); D.ensure((size_t)T * 2 * nb); P.ensure((size_t)T * nb); mel.ensure((size_t)T * NM);
+        launch_preemphasis(x, pre16.p, N, 0.97f, st);
+        launch_frame_window(pre16.p, N, hamm.p, 400, 160, 56, 256, PAD_REFLECT, F.p, T, 128, st);
+        launch_gemm_f32(F.p, basis16.p, nullptr, nullptr, D.p, T, 2 * nb, 400, 0, st);
+        launch_power(D.p, P.p, T, nb, st);
+        launch_gemm_f32(P.p, fb16.p, nullptr, nullptr, mel.p, T, NM, nb, 0, st);
+        launch_mel_log(mel.p, nullptr, (size_t)T * NM, NM, 1, st);
+        launch_instnorm_t(mel.p, img_out, T, NM, 1e-5f, st);
     }
 };
 
@@ -404,24 +502,11 @@ void Conditioner::run(const float* wav22k_host, int64_t n22, const float* wav16k
     }
     if (pieces.empty()) throw std::runtime_error("condition: no usable reference piece (>= 0.33 s)");
     CUDA_CHECK(cudaMemsetAsync(cond_dev, 0, (size_t)NC * H * sizeof(float), st));
-    const int nb22 = 1025;
-    bool first = true;
     for (auto& pc : pieces) {
         const int len = (int)pc.second;
         const int T = 1 + len / 256;
-        m.F.ensure((size_t)T * 1024); m.D.ensure((size_t)T * 2 * nb22); m.P.ensure((size_t)T * nb22); m.mel.ensure((size_t)T * c.n_mels);
-        frame_window_kernel<<<T, 256, 0, st>>>(m.wav22.p + pc.first, len, m.hann.p, 1024, 256, 512, 1024, PAD_REFLECT, m.F.p, T);
-        COUNT_LAUNCH(); KERNEL_CHECK();
-        launch_gemm_f32(m.F.p, m.basis22.p, nullptr, nullptr, m.D.p, T, 2 * nb22, 1024, 0, st);
-        power_kernel<<<nblk((size_t)T * nb22), 256, 0, st>>>(m.D.p, m.P.p, T, nb22); COUNT_LAUNCH(); KERNEL_CHECK();
-        launch_gemm_f32(m.P.p, m.fb22.p, nullptr, nullptr, m.mel.p, T, c.n_mels, nb22, 0, st);
-        mel_log_kernel<<<nblk((size_t)T * c.n_mels), 256, 0, st>>>(m.mel.p, m.mel_stats.p, (size_t)T * c.n_mels, c.n_mels, 0);
-        COUNT_LAUNCH(); KERNEL_CHECK();
-        if (first) {
-            last_mel.resize((size_t)T * c.n_mels); last_mel_frames = T;
-            CUDA_CHECK(cudaMemcpyAsync(last_mel.data(), m.mel.p, last_mel.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
-            first = false;
-        }
+        m.mel.ensure((size_t)T * c.n_mels);
+        m.mel22(m.wav22.p + pc.first, len, m.mel.p, m.mel.n);
         // ---- ConditioningEncoder (latent_encoder.py:242-253)
         m.h0.ensure((size_t)T * H); m.h1.ensure((size_t)T * H); m.xn.ensure((size_t)T * H); m.qkv.ensure((size_t)T * 3 * H); m.att.ensure((size_t)T * H);
         m.gemm(m.mel.p, m.init, nullptr, m.h0.p, T);
@@ -430,8 +515,7 @@ void Conditioner::run(const float* wav22k_host, int64_t n22, const float* wav16k
         if (H <= 16) groups = 8; else if (H <= 64) groups = 16;
         while (H % groups != 0) groups /= 2;
         for (auto& ab : m.blocks) {
-            groupnorm_rows_kernel<<<groups, 256, 0, st>>>(h, ab->nw.p, ab->nb.p, m.xn.p, T, H, groups, 1e-5f);
-            COUNT_LAUNCH(); KERNEL_CHECK();
+            launch_groupnorm(h, ab->nw.p, ab->nb.p, m.xn.p, T, H, groups, 1e-5f, st);
             m.gemm(m.xn.p, ab->qkv, nullptr, m.qkv.p, T);
             AttnSeq sq{0, T, 0, T};
             CUDA_CHECK(cudaMemcpyAsync(m.seq.p, &sq, sizeof(sq), cudaMemcpyHostToDevice, st));
@@ -462,68 +546,214 @@ void Conditioner::run(const float* wav22k_host, int64_t n22, const float* wav16k
             launch_attn_generic<float>(A, m.seq.p, 1, NC, m.o.p, inner, st);
             m.gemm(m.o.p, pl->o, m.lat.p, m.lat.p, NC);
             m.gemm(m.lat.p, pl->f1, nullptr, m.ff.p, NC);
-            geglu_kernel<<<nblk((size_t)NC * ffi), 256, 0, st>>>(m.ff.p, m.gg.p, NC, ffi); COUNT_LAUNCH(); KERNEL_CHECK();
+            launch_geglu(m.ff.p, m.gg.p, NC, ffi, st);
             m.gemm(m.gg.p, pl->f2, m.lat.p, m.lat.p, NC);
         }
-        rmsnorm_accum_kernel<<<NC, 256, 0, st>>>(m.lat.p, m.gamma.p, cond_dev, H, 1.0f / (float)pieces.size());
-        COUNT_LAUNCH(); KERNEL_CHECK();
+        launch_rmsnorm_accum(m.lat.p, m.gamma.p, cond_dev, NC, H, 1.0f / (float)pieces.size(), st);
     }
     // ================= d-vector (hifigan_decoder.py:602-646)
     {
         const int N = (int)n16;
         if (N < 400) throw std::runtime_error("condition: 16 kHz reference too short");
-        m.wav16.ensure(N); m.pre16.ensure(N);
+        const int T = 1 + N / 160, NM = c.spk_mels;
+        m.wav16.ensure(N); m.img.ensure((size_t)NM * T);
         CUDA_CHECK(cudaMemcpyAsync(m.wav16.p, wav16k_host, (size_t)N * sizeof(float), cudaMemcpyHostToDevice, st));
-        preemphasis_kernel<<<nblk(N), 256, 0, st>>>(m.wav16.p, m.pre16.p, N, 0.97f); COUNT_LAUNCH(); KERNEL_CHECK();
-        const int T = 1 + N / 160, nb = 257, NM = c.spk_mels;
-        m.F.ensure((size_t)T * 400); m.D.ensure((size_t)T * 2 * nb); m.P.ensure((size_t)T * nb); m.mel.ensure((size_t)T * NM);
-        frame_window_kernel<<<T, 128, 0, st>>>(m.pre16.p, N, m.hamm.p, 400, 160, 56, 256, PAD_REFLECT, m.F.p, T); COUNT_LAUNCH(); KERNEL_CHECK();
-        launch_gemm_f32(m.F.p, m.basis16.p, nullptr, nullptr, m.D.p, T, 2 * nb, 400, 0, st);
-        power_kernel<<<nblk((size_t)T * nb), 256, 0, st>>>(m.D.p, m.P.p, T, nb); COUNT_LAUNCH(); KERNEL_CHECK();
-        launch_gemm_f32(m.P.p, m.fb16.p, nullptr, nullptr, m.mel.p, T, NM, nb, 0, st);
-        mel_log_kernel<<<nblk((size_t)T * NM), 256, 0, st>>>(m.mel.p, nullptr, (size_t)T * NM, NM, 1); COUNT_LAUNCH(); KERNEL_CHECK();
-        m.img.ensure((size_t)NM * T);
-        instnorm_transpose_kernel<<<NM, 256, 0, st>>>(m.mel.p, m.img.p, T, NM, 1e-5f); COUNT_LAUNCH(); KERNEL_CHECK();
+        m.mel16(m.wav16.p, N, m.img.p, m.img.n);
         const size_t big = (size_t)c.spk_filters[0] * NM * T;
         m.a0.ensure(big); m.a1.ensure(big); m.a2.ensure(big);
+        const size_t acap = std::min(m.a0.n, std::min(m.a1.n, m.a2.n));
         int Hc = NM, Wc = T, Ho, Wo;
-        m.conv2d(m.img.p, m.conv1_w.p, m.conv1_b.p, &m.bn1, m.a0.p, 1, c.spk_filters[0], Hc, Wc, 3, 1, 1, Ho, Wo);
+        m.conv2d(m.img.p, m.conv1_w.p, m.conv1_b.p, &m.bn1, m.a0.p, acap, 1, c.spk_filters[0], Hc, Wc, 3, 1, 1, Ho, Wo);
         float* x = m.a0.p; float* t1 = m.a1.p; float* t2 = m.a2.p;
         m.chm.ensure(4096); m.gate.ensure(4096);
-        Dev<float> dsbuf; dsbuf.alloc(big / 2 + 16);
         for (auto& blk : m.res) {
             int H1, W1, H2, W2;
-            m.conv2d(x, blk->c1.p, nullptr, &blk->bn1, t1, blk->cin, blk->cout, Hc, Wc, 3, blk->stride, 1, H1, W1);
-            m.conv2d(t1, blk->c2.p, nullptr, &blk->bn2, t2, blk->cout, blk->cout, H1, W1, 3, 1, 0, H2, W2);
+            m.conv2d(x, blk->c1.p, nullptr, &blk->bn1, t1, acap, blk->cin, blk->cout, Hc, Wc, 3, blk->stride, 1, H1, W1);
+            m.conv2d(t1, blk->c2.p, nullptr, &blk->bn2, t2, acap, blk->cout, blk->cout, H1, W1, 3, 1, 0, H2, W2);
             const int HW = H2 * W2;
-            channel_mean_kernel<<<blk->cout, 256, 0, st>>>(t2, m.chm.p, HW); COUNT_LAUNCH(); KERNEL_CHECK();
-            se_gate_kernel<<<1, 256, blk->se1.N * sizeof(float), st>>>(m.chm.p, blk->se1.w.p, blk->se1.b.p, blk->se2.w.p,
-                                                                        blk->se2.b.p, m.gate.p, blk->cout, blk->se1.N);
-            COUNT_LAUNCH(); KERNEL_CHECK();
+            launch_channel_mean(t2, m.chm.p, blk->cout, HW, st);
+            launch_se_gate(m.chm.p, blk->se1.w.p, blk->se1.b.p, blk->se2.w.p, blk->se2.b.p, m.gate.p, blk->cout, blk->se1.N, st);
             const float* resid = x;
-            if (blk->has_ds) {
+            if (blk->has_ds) {      // 1x1 conv at the block's stride: [cout][(Hc-1)/stride+1][(Wc-1)/stride+1]
                 int Hd, Wd;
-                m.conv2d(x, blk->ds.p, nullptr, &blk->bnd, dsbuf.p, blk->cin, blk->cout, Hc, Wc, 1, blk->stride, 0, Hd, Wd);
-                resid = dsbuf.p;
+                m.ds.ensure((size_t)blk->cout * conv_out(Hc, 1, blk->stride) * conv_out(Wc, 1, blk->stride));
+                m.conv2d(x, blk->ds.p, nullptr, &blk->bnd, m.ds.p, m.ds.n, blk->cin, blk->cout, Hc, Wc, 1, blk->stride, 0, Hd, Wd);
+                resid = m.ds.p;
             }
-            const size_t ne = (size_t)blk->cout * HW;
-            se_apply_kernel<<<nblk(ne), 256, 0, st>>>(t2, m.gate.p, resid, t1, HW, ne); COUNT_LAUNCH(); KERNEL_CHECK();
+            launch_se_apply(t2, m.gate.p, resid, t1, HW, (size_t)blk->cout * HW, st);
             std::swap(x, t1);
             Hc = H2; Wc = W2;
         }
         // x: [C4][Hc][Wc] -> feats [C4*Hc][Wc]
         const int CF = c.spk_filters[3] * Hc, Tt = Wc;
         m.xT.ensure((size_t)Tt * CF); m.at1.ensure((size_t)Tt * m.att0.N); m.at2.ensure((size_t)Tt * CF); m.pooled.ensure(2 * CF);
-        transpose_kernel<<<nblk((size_t)CF * Tt), 256, 0, st>>>(x, m.xT.p, CF, Tt); COUNT_LAUNCH(); KERNEL_CHECK();
+        launch_transpose(x, m.xT.p, CF, Tt, st);
         m.gemm(m.xT.p, m.att0, nullptr, m.at1.p, Tt);
-        relu_bn_rows_kernel<<<nblk((size_t)Tt * m.att0.N), 256, 0, st>>>(m.at1.p, m.att_bn.scale.p, m.att_bn.shift.p, (size_t)Tt * m.att0.N, m.att0.N);
-        COUNT_LAUNCH(); KERNEL_CHECK();
+        launch_relu_bn_rows(m.at1.p, m.att_bn.scale.p, m.att_bn.shift.p, (size_t)Tt * m.att0.N, m.att0.N, st);
         m.gemm(m.at1.p, m.att3, nullptr, m.at2.p, Tt);
-        asp_kernel<<<CF, 128, 0, st>>>(m.at2.p, x, m.pooled.p, Tt, CF); COUNT_LAUNCH(); KERNEL_CHECK();
+        launch_asp(m.at2.p, x, m.pooled.p, Tt, CF, st);
         launch_gemv(m.fc.w.p, m.fc.b.p, m.pooled.p, g_dev, m.fc.N, m.fc.K, st);
-        l2norm_kernel<<<1, 256, 0, st>>>(g_dev, m.fc.N); COUNT_LAUNCH(); KERNEL_CHECK();
-        CUDA_CHECK(cudaStreamSynchronize(st));      // dsbuf goes out of scope
+        launch_l2norm(g_dev, m.fc.N, st);
     }
+}
+
+void Conditioner::frontend(int op, const float* x_dev, int n, float* out_dev, size_t cap) {
+    if (op == XTTS_COND_MEL22) impl->mel22(x_dev, n, out_dev, cap);
+    else impl->mel16(x_dev, n, out_dev, cap);
+}
+int Conditioner::n_mels() const { return impl->c.n_mels; }
+int Conditioner::spk_mels() const { return impl->c.spk_mels; }
+
+// ---------------------------------------------------------------------------------------- xtts_debug_cond
+namespace {
+constexpr int kGuardWords = 256;
+constexpr uint32_t kGuardBits = 0x7fc5a5a5u;       // a quiet-NaN payload no kernel here produces
+}  // namespace
+
+void cond_debug(Conditioner* cnd, int op, const int32_t* dims, int n_dims, const float* scal, int n_scal, const float* const* in,
+                const int64_t* in_len, int n_in, float* out, int64_t out_len, cudaStream_t st) {
+    static const int kDims[XTTS_COND_N_OPS] = {8, 2, 3, 1, 2, 3, 2, 2, 9, 2, 2, 2, 2, 2, 2, 1, 3, 1, 1};
+    static const int kScal[XTTS_COND_N_OPS] = {0, 0, 0, 1, 1, 1, 0, 1, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    auto bad = [](const std::string& s) { return std::runtime_error("debug_cond: " + s); };
+    if (op < 0 || op >= XTTS_COND_N_OPS) throw bad("unknown op " + std::to_string(op));
+    if (n_dims != kDims[op] || n_scal != kScal[op])
+        throw bad("op " + std::to_string(op) + " takes " + std::to_string(kDims[op]) + " dims and " + std::to_string(kScal[op]) + " scalars");
+    if ((n_dims && !dims) || (n_scal && !scal) || (n_in > 0 && (!in || !in_len)) || !out) throw bad("NULL argument");
+    for (int i = 0; i < n_dims; ++i)
+        if (dims[i] < 0) throw bad("negative dim");
+    auto d = [&](int i) { return (int64_t)dims[i]; };
+    auto pos = [&](std::initializer_list<int> idx) {
+        for (int i : idx) if (dims[i] < 1) throw bad("dim " + std::to_string(i) + " must be >= 1");
+    };
+    std::vector<int64_t> need;       // in_len each input must have
+    int64_t need_out = 0;
+    switch (op) {
+    case XTTS_COND_FRAME_WINDOW:     // n, wlen, hop, off, pad, pad_mode, frames, threads
+        pos({0, 1, 2, 6});
+        if (d(5) != PAD_REFLECT && d(5) != PAD_ZERO) throw bad("pad_mode must be 0 (reflect) or 1 (zero)");
+        if (d(7) != 128 && d(7) != 256) throw bad("frame_window runs 128 or 256 threads");
+        need = {d(0), d(1)}; need_out = d(6) * d(1); break;
+    case XTTS_COND_POWER:            // frames, nb
+        pos({0, 1}); need = {d(0) * 2 * d(1)}; need_out = d(0) * d(1); break;
+    case XTTS_COND_MEL_LOG:          // n, C, mode
+        pos({0, 1});
+        if (d(2) > 1) throw bad("mel_log mode must be 0 or 1");
+        need = d(2) == 0 ? std::vector<int64_t>{d(1)} : std::vector<int64_t>{}; need_out = d(0); break;
+    case XTTS_COND_PREEMPHASIS:      // n
+        if (d(0) < 2) throw bad("preemphasis needs n >= 2");
+        need = {d(0)}; need_out = d(0); break;
+    case XTTS_COND_INSTNORM_T:       // T, C
+        pos({0, 1}); need = {d(0) * d(1)}; need_out = d(0) * d(1); break;
+    case XTTS_COND_GROUPNORM:        // T, C, groups
+        pos({0, 1, 2});
+        if (d(1) % d(2) != 0) throw bad("groupnorm needs C % groups == 0");
+        need = {d(0) * d(1), d(1), d(1)}; need_out = d(0) * d(1); break;
+    case XTTS_COND_GEGLU:            // rows, F
+        pos({0, 1}); need = {d(0) * 2 * d(1)}; need_out = d(0) * d(1); break;
+    case XTTS_COND_RMSNORM_ACCUM:    // rows, C
+        pos({0, 1}); need = {d(0) * d(1), d(1)}; need_out = d(0) * d(1); break;
+    case XTTS_COND_CONV2D: {         // Cin, Cout, Hin, Win, k, stride, relu_before_bn, has_bias, has_bn
+        pos({0, 1, 2, 3, 4, 5});
+        if (d(4) % 2 == 0) throw bad("conv2d needs an odd k");
+        if (d(6) > 1 || d(7) > 1 || d(8) > 1) throw bad("conv2d flags must be 0 or 1");
+        if (conv2d_smem(dims[0], dims[4]) > kSmemLimit) throw bad("conv2d weight slice exceeds 48 KB of shared memory");
+        const int64_t Ho = conv_out(dims[2], dims[4], dims[5]), Wo = conv_out(dims[3], dims[4], dims[5]);
+        if (Ho < 1 || Wo < 1) throw bad("conv2d output is empty");
+        need = {d(0) * d(2) * d(3), d(1) * d(0) * d(4) * d(4)};
+        if (d(7)) need.push_back(d(1));
+        if (d(8)) { need.push_back(d(1)); need.push_back(d(1)); }
+        need_out = d(1) * Ho * Wo; break;
+    }
+    case XTTS_COND_CHANNEL_MEAN:     // C, HW
+        pos({0, 1}); need = {d(0) * d(1)}; need_out = d(0); break;
+    case XTTS_COND_SE_GATE:          // C, R
+        pos({0, 1});
+        if ((size_t)d(1) * sizeof(float) > kSmemLimit) throw bad("se_gate hidden layer exceeds 48 KB of shared memory");
+        need = {d(0), d(1) * d(0), d(1), d(0) * d(1), d(0)}; need_out = d(0); break;
+    case XTTS_COND_SE_APPLY:         // C, HW
+        pos({0, 1}); need = {d(0) * d(1), d(0), d(0) * d(1)}; need_out = d(0) * d(1); break;
+    case XTTS_COND_TRANSPOSE:        // R, Cc
+        pos({0, 1}); need = {d(0) * d(1)}; need_out = d(0) * d(1); break;
+    case XTTS_COND_RELU_BN_ROWS:     // rows, C
+        pos({0, 1}); need = {d(1), d(1)}; need_out = d(0) * d(1); break;
+    case XTTS_COND_ASP:              // T, C
+        pos({0, 1}); need = {d(0) * d(1), d(1) * d(0)}; need_out = 2 * d(1); break;
+    case XTTS_COND_L2NORM:           // n
+        pos({0}); need = {}; need_out = d(0); break;
+    case XTTS_COND_GEMV:             // rows, cols, has_bias
+        pos({0, 1});
+        if (d(2) > 1) throw bad("gemv has_bias must be 0 or 1");
+        need = {d(0) * d(1), d(1)};
+        if (d(2)) need.push_back(d(0));
+        need_out = d(0); break;
+    case XTTS_COND_MEL22:            // n
+    case XTTS_COND_MEL16:
+        if (!cnd) throw bad("the checkpoint has no conditioning weights");
+        if (op == XTTS_COND_MEL22 && d(0) < 2) throw bad("mel22 needs n >= 2");
+        if (op == XTTS_COND_MEL16 && d(0) < 400) throw bad("mel16 needs n >= 400");
+        need = {d(0)};
+        need_out = op == XTTS_COND_MEL22 ? (1 + d(0) / 256) * cnd->n_mels() : (int64_t)cnd->spk_mels() * (1 + d(0) / 160);
+        break;
+    }
+    if (n_in != (int)need.size()) throw bad("op " + std::to_string(op) + " takes " + std::to_string(need.size()) + " inputs");
+    for (int i = 0; i < n_in; ++i) {
+        if (in_len[i] != need[i])
+            throw bad("input " + std::to_string(i) + " has " + std::to_string(in_len[i]) + " floats, expected " + std::to_string(need[i]));
+        if (!in[i]) throw bad("input " + std::to_string(i) + " is NULL");
+    }
+    if (out_len < 1 || out_len != need_out) throw bad("out has " + std::to_string(out_len) + " floats, expected " + std::to_string(need_out));
+
+    std::vector<std::unique_ptr<Dev<float>>> din;
+    std::vector<const float*> ip(n_in);
+    for (int i = 0; i < n_in; ++i) {
+        din.emplace_back(new Dev<float>());
+        din.back()->up(std::vector<float>(in[i], in[i] + in_len[i]), st);
+        ip[i] = din.back()->p;
+    }
+    // out with kGuardWords sentinel words on each side; its incoming contents are uploaded (in-place kernels read them)
+    std::vector<uint32_t> h((size_t)out_len + 2 * kGuardWords, kGuardBits);
+    std::memcpy(h.data() + kGuardWords, out, (size_t)out_len * sizeof(float));
+    Dev<float> dout;
+    dout.alloc(h.size());
+    CUDA_CHECK(cudaMemcpyAsync(dout.p, h.data(), h.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    float* o = dout.p + kGuardWords;
+    const float* const* I = ip.data();
+    const int* D = dims;
+    int Ho = 0, Wo = 0;
+    switch (op) {
+    case XTTS_COND_FRAME_WINDOW:
+        launch_frame_window(I[0], D[0], I[1], D[1], D[2], D[3], D[4], D[5], o, D[6], D[7], st); break;
+    case XTTS_COND_POWER: launch_power(I[0], o, D[0], D[1], st); break;
+    case XTTS_COND_MEL_LOG: launch_mel_log(o, D[2] == 0 ? I[0] : nullptr, (size_t)D[0], D[1], D[2], st); break;
+    case XTTS_COND_PREEMPHASIS: launch_preemphasis(I[0], o, D[0], scal[0], st); break;
+    case XTTS_COND_INSTNORM_T: launch_instnorm_t(I[0], o, D[0], D[1], scal[0], st); break;
+    case XTTS_COND_GROUPNORM: launch_groupnorm(I[0], I[1], I[2], o, D[0], D[1], D[2], scal[0], st); break;
+    case XTTS_COND_GEGLU: launch_geglu(I[0], o, D[0], D[1], st); break;
+    case XTTS_COND_RMSNORM_ACCUM: launch_rmsnorm_accum(I[0], I[1], o, D[0], D[1], scal[0], st); break;
+    case XTTS_COND_CONV2D: {
+        const float* bias = D[7] ? I[2] : nullptr;
+        const float* sc = D[8] ? I[2 + D[7]] : nullptr;
+        const float* sh = D[8] ? I[3 + D[7]] : nullptr;
+        launch_conv2d(I[0], I[1], bias, sc, sh, o, (size_t)out_len, D[0], D[1], D[2], D[3], D[4], D[5], D[6], Ho, Wo, st);
+        break;
+    }
+    case XTTS_COND_CHANNEL_MEAN: launch_channel_mean(I[0], o, D[0], D[1], st); break;
+    case XTTS_COND_SE_GATE: launch_se_gate(I[0], I[1], I[2], I[3], I[4], o, D[0], D[1], st); break;
+    case XTTS_COND_SE_APPLY: launch_se_apply(I[0], I[1], I[2], o, D[1], (size_t)D[0] * D[1], st); break;
+    case XTTS_COND_TRANSPOSE: launch_transpose(I[0], o, D[0], D[1], st); break;
+    case XTTS_COND_RELU_BN_ROWS: launch_relu_bn_rows(o, I[0], I[1], (size_t)D[0] * D[1], D[1], st); break;
+    case XTTS_COND_ASP: launch_asp(I[0], I[1], o, D[0], D[1], st); break;
+    case XTTS_COND_L2NORM: launch_l2norm(o, D[0], st); break;
+    case XTTS_COND_GEMV: launch_gemv(I[0], D[2] ? I[2] : nullptr, I[1], o, D[0], D[1], st); break;
+    case XTTS_COND_MEL22:
+    case XTTS_COND_MEL16: cnd->frontend(op, I[0], D[0], o, (size_t)out_len); break;
+    }
+    CUDA_CHECK(cudaMemcpyAsync(h.data(), dout.p, h.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    for (int i = 0; i < kGuardWords; ++i)
+        if (h[i] != kGuardBits || h[kGuardWords + out_len + i] != kGuardBits)
+            throw bad("op " + std::to_string(op) + " wrote outside its output");
+    std::memcpy(out, h.data() + kGuardWords, (size_t)out_len * sizeof(float));
 }
 
 }  // namespace xtts

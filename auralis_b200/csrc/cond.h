@@ -62,14 +62,22 @@ public:
     // writes cond [n_cond*H] and g [spk_proj] (device pointers)
     void run(const float* wav22k_host, int64_t n22, const float* wav16k_host, int64_t n16, int cond_len_s,
              int chunk_len_s, float* cond_dev, float* g_dev);
-    // stage taps for parity tests (host copies of the last run)
-    std::vector<float> last_mel;       // [frames,80] of the first piece
-    int last_mel_frames = 0;
+    // one front-end on device data, as run() applies it (xtts_debug_cond): op XTTS_COND_MEL22, x [n] -> [1 + n/256][n_mels];
+    // XTTS_COND_MEL16, x [n] -> [spk_mels][1 + n/160].  Throws before any launch when the output exceeds cap floats.
+    void frontend(int op, const float* x_dev, int n, float* out_dev, size_t cap);
+    int n_mels() const;
+    int spk_mels() const;
 
 private:
     struct Impl;
     std::unique_ptr<Impl> impl;
 };
+
+// xtts_debug_cond (include/xtts_b200.h): one conditioning kernel (or front-end, through `cnd`, which may be NULL for the
+// single-kernel ops) on host data, with the launch Conditioner::run uses.  Throws before any launch on a bad argument, and
+// after it when the kernel wrote into the guard words around `out`.
+void cond_debug(Conditioner* cnd, int op, const int32_t* dims, int n_dims, const float* scal, int n_scal, const float* const* in,
+                const int64_t* in_len, int n_in, float* out, int64_t out_len, cudaStream_t st);
 
 // Reference-audio enhancer (enhance.cu): the reference's EnhancedAudioProcessor.process followed by a 16-bit PCM
 // write/read, on the GPU.  Needs no weights; its STFT basis and mel filterbanks are built on first use.

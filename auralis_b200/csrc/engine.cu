@@ -214,6 +214,8 @@ public:
     void debug_conv_tc(int up, int Cin, int Cout, int K, int dil, int batch, int L, const int32_t* item_len, const float* w,
                        const float* bias, const float* cbias, int cbias_stride, const float* x, const float* resid, int mode,
                        float slope_out, float scale16, int max_ctas, float* out32, float* out16);
+    void debug_cond(int op, const int32_t* dims, int n_dims, const float* scal, int n_scal, const float* const* in,
+                    const int64_t* in_len, int n_in, float* out, int64_t out_len);
 
 private:
     KernelCtx kctx_;
@@ -2863,6 +2865,15 @@ void Engine::debug_conv_tc(int up, int Cin, int Cout, int K, int dil, int batch,
     if (out16) widen16(r16, true, out16);
 }
 
+// One conditioning kernel or front-end (cond_debug in cond.cu) on the engine's stream
+void Engine::debug_cond(int op, const int32_t* dims, int n_dims, const float* scal, int n_scal, const float* const* in,
+                        const int64_t* in_len, int n_in, float* out, int64_t out_len) {
+    ApiLock lk(this);
+    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
+    CUDA_CHECK(cudaSetDevice(cfg.device));
+    cond_debug(conditioner.get(), op, dims, n_dims, scal, n_scal, in, in_len, n_in, out, out_len, st);
+}
+
 }  // namespace xtts
 
 // ================================================================================================
@@ -3043,6 +3054,10 @@ int xtts_debug_conv_tc(xtts_engine* e, int32_t up, int32_t Cin, int32_t Cout, in
                        float* out32, float* out16) {
     XTTS_TRY(e->impl->debug_conv_tc(up, Cin, Cout, K, dil, batch, L, item_len, w, bias, cbias, cbias_stride, x, resid, mode,
                                     slope_out, scale16, max_ctas, out32, out16))
+}
+int xtts_debug_cond(xtts_engine* e, int32_t op, const int32_t* dims, int32_t n_dims, const float* scal, int32_t n_scal,
+                    const float* const* in, const int64_t* in_len, int32_t n_in, float* out, int64_t out_len) {
+    XTTS_TRY(e->impl->debug_cond(op, dims, n_dims, scal, n_scal, in, in_len, n_in, out, out_len))
 }
 
 }  // extern "C"

@@ -116,10 +116,16 @@ ABI_SYMBOLS = [
     "xtts_debug_gemm", "xtts_debug_sample_slots", "xtts_debug_trace",
     "xtts_debug_attn_decode", "xtts_debug_attn_prefill", "xtts_debug_splitk_ln", "xtts_debug_conv_tc",
     "xtts_debug_ln_gemm", "xtts_debug_norms", "xtts_debug_kv_write", "xtts_debug_build_rows", "xtts_debug_build_decode_rows",
+    "xtts_debug_cond",
 ]
 
 # flag bits of xtts_debug_gemm / xtts_debug_ln_gemm (include/xtts_b200.h)
 GEMM_GELU, GEMM_OUT16, GEMM_INPLACE, GEMM_PDL = 1, 2, 4, 8
+
+# op codes of xtts_debug_cond (XTTS_COND_* in include/xtts_b200.h)
+COND_OPS = ("FRAME_WINDOW", "POWER", "MEL_LOG", "PREEMPHASIS", "INSTNORM_T", "GROUPNORM", "GEGLU", "RMSNORM_ACCUM", "CONV2D",
+            "CHANNEL_MEAN", "SE_GATE", "SE_APPLY", "TRANSPOSE", "RELU_BN_ROWS", "ASP", "L2NORM", "GEMV", "MEL22", "MEL16")
+COND_OP = {name: i for i, name in enumerate(COND_OPS)}
 
 _lib = None
 
@@ -180,6 +186,7 @@ def load_library(path: Optional[str] = None):
     lib.xtts_debug_kv_write.argtypes = [vp, i32, i32, i32, f32p, i32p, i32p, i32, i32p, i32p, i32, i32, vp, vp]
     lib.xtts_debug_build_rows.argtypes = [vp, i32, i32, f32p, i32, f32p, i32, f32p, i32, f32p, i32, f32p, i32, i32p, i32, f32p]
     lib.xtts_debug_build_decode_rows.argtypes = [vp, i32, f32p, i32, f32p, i32, i32, i32p, i32, i32p, i32p, f32p, u32p, i32, i32]
+    lib.xtts_debug_cond.argtypes = [vp, i32, i32p, i32, f32p, i32, C.POINTER(f32p), C.POINTER(i64), i32, f32p, i64]
     for s in ABI_SYMBOLS:
         if s not in ("xtts_last_error", "xtts_version"):
             getattr(lib, s).restype = C.c_int
@@ -764,3 +771,17 @@ class NativeEngine:
                                               cb.shape[1] if cb is not None else 0, _fp(x), _fp(r), mode, slope_out,
                                               scale16, max_ctas, _fp(o32), _fp(o16)), "debug_conv_tc")
         return o32, o16
+
+    def debug_cond(self, op, dims, inputs=(), out=None, out_len: Optional[int] = None, scal=()):
+        """One conditioning kernel (xtts_debug_cond).  op: a name of COND_OPS or its code; inputs: arrays, flattened to fp32;
+        out: the incoming contents (the base of the in-place ops), else out_len floats of NaN.  -> out after, flat fp32."""
+        code = COND_OP[op] if isinstance(op, str) else int(op)
+        d = _i32(dims).reshape(-1)
+        s = _f32(scal).reshape(-1)
+        ins = [_f32(a).reshape(-1) for a in inputs]
+        o = _f32(out).reshape(-1).copy() if out is not None else np.full(int(out_len), np.nan, np.float32)
+        ptrs = (C.POINTER(C.c_float) * max(len(ins), 1))(*[_fp(a) for a in ins])
+        lens = (C.c_int64 * max(len(ins), 1))(*[a.size for a in ins])
+        self._chk(self.lib.xtts_debug_cond(self.h, code, _ip(d), d.size, _fp(s) if s.size else None, s.size, ptrs, lens,
+                                           len(ins), _fp(o), o.size), "debug_cond")
+        return o

@@ -401,6 +401,64 @@ int xtts_debug_conv_tc(xtts_engine* e, int32_t up, int32_t Cin, int32_t Cout, in
                        const int32_t* item_len, const float* w, const float* bias, const float* cbias, int32_t cbias_stride,
                        const float* x, const float* resid, int32_t mode, float slope_out, float scale16, int32_t max_ctas,
                        float* out32, float* out16);
+/* one speaker-conditioning kernel (csrc/cond.cu) on caller data, launched with the grid, block size and shared memory
+ * xtts_condition uses.  dims [n_dims] and scal [n_scal] are the op's parameters; in [n_in] its fp32 inputs of in_len[i]
+ * floats each; out [out_len] is in/out: uploaded before the launch (the base of the in-place ops, and what an element the
+ * kernel does not write comes back as) and downloaded after it.  The device copy of out has 256 sentinel words on each
+ * side; a kernel that writes one of them is an error.  Rejected before any launch: an unknown op, a wrong n_dims / n_scal
+ * / n_in, a dim out of range, any in_len or out_len other than the one the dims imply, a NULL pointer.  Layouts are
+ * row-major; per op, "dims; scal; inputs -> out":
+ *   FRAME_WINDOW   n, wlen, hop, off, pad, pad_mode (0 reflect, 1 zero), frames, threads (128 or 256); -; x [n], win [wlen]
+ *                  -> F [frames][wlen], F[t][i] = win[i] * xp[t*hop + off + i], xp = x padded by `pad` on each side
+ *                  (reflect; or zero with NaN / inf samples read as 0)
+ *   POWER          frames, nb; -; D [frames][2*nb] (re | im) -> P [frames][nb] = re^2 + im^2
+ *   MEL_LOG        n, C, mode; -; mode 0: stats [C], mode 1: none -> out [n] in place: mode 0 log(max(v, 1e-5)) / stats[i % C],
+ *                  mode 1 log(v + 1e-6)
+ *   PREEMPHASIS    n (>= 2); coef; x [n] -> y [n] = x[i] - coef * x[i-1], x[-1] = x[1]
+ *   INSTNORM_T     T, C; eps; x [T][C] -> y [C][T], each channel normalised over time (biased variance)
+ *   GROUPNORM      T, C, groups (C % groups == 0); eps; x [T][C], w [C], b [C] -> y [T][C]
+ *   GEGLU          rows, F; -; h [rows][2F] -> y [rows][F] = h[:, :F] * gelu_erf(h[:, F:])
+ *   RMSNORM_ACCUM  rows, C; scale; x [rows][C], gamma [C] -> acc [rows][C] in place:
+ *                  acc += x / max(|x|, 1e-12) * sqrt(C) * gamma * scale
+ *   CONV2D         Cin, Cout, Hin, Win, k (odd), stride, relu_before_bn, has_bias, has_bn; -; x [Cin][Hin][Win],
+ *                  w [Cout][Cin][k][k], then bias [Cout] if has_bias, then bn_scale [Cout], bn_shift [Cout] if has_bn
+ *                  -> y [Cout][Hout][Wout], padding k/2, Hout = (Hin - 1) / stride + 1 (Wout alike);
+ *                  y = bn(relu?(conv + bias)).  Rejected too: a weight slice 4 * Cin * k * k floats above 48 KB
+ *   CHANNEL_MEAN   C, HW; -; x [C][HW] -> m [C]
+ *   SE_GATE        C, R; -; m [C], w1 [R][C], b1 [R], w2 [C][R], b2 [C] -> s [C] = sigmoid(w2 relu(w1 m + b1) + b2)
+ *   SE_APPLY       C, HW; -; x [C][HW], gate [C], resid [C][HW] -> y [C][HW] = relu(x * gate + resid)
+ *   TRANSPOSE      R, Cc; -; x [R][Cc] -> y [Cc][R]
+ *   RELU_BN_ROWS   rows, C; -; scale [C], shift [C] -> x [rows][C] in place: relu(x) * scale + shift
+ *   ASP            T, C; -; logits [T][C], x [C][T] -> [2][C]: mu = sum softmax_t * x, sqrt(max(sum softmax_t * x^2 - mu^2, 1e-5))
+ *   L2NORM         n; -; none -> x [n] in place: x / max(|x|, 1e-12)
+ *   GEMV           rows, cols, has_bias; -; W [rows][cols], g [cols], then b [rows] if has_bias -> y [rows] = W g + b
+ *   MEL22          n (>= 2); -; wav [n] at 22.05 kHz -> [1 + n/256][n_mels]: the engine's Hann window, DFT basis, power,
+ *                  slaney mel filterbank, log(max(., 1e-5)) / mel_stats (the GPT conditioning front-end)
+ *   MEL16          n (>= 400); -; wav [n] at 16 kHz -> [spk_mels][1 + n/160]: pre-emphasis 0.97, the engine's Hamming window,
+ *                  DFT basis, power, mel filterbank, log(. + 1e-6), InstanceNorm over time (the speaker encoder front-end)
+ * MEL22 / MEL16 need a checkpoint with the conditioning weights. */
+#define XTTS_COND_FRAME_WINDOW 0
+#define XTTS_COND_POWER 1
+#define XTTS_COND_MEL_LOG 2
+#define XTTS_COND_PREEMPHASIS 3
+#define XTTS_COND_INSTNORM_T 4
+#define XTTS_COND_GROUPNORM 5
+#define XTTS_COND_GEGLU 6
+#define XTTS_COND_RMSNORM_ACCUM 7
+#define XTTS_COND_CONV2D 8
+#define XTTS_COND_CHANNEL_MEAN 9
+#define XTTS_COND_SE_GATE 10
+#define XTTS_COND_SE_APPLY 11
+#define XTTS_COND_TRANSPOSE 12
+#define XTTS_COND_RELU_BN_ROWS 13
+#define XTTS_COND_ASP 14
+#define XTTS_COND_L2NORM 15
+#define XTTS_COND_GEMV 16
+#define XTTS_COND_MEL22 17
+#define XTTS_COND_MEL16 18
+#define XTTS_COND_N_OPS 19
+int xtts_debug_cond(xtts_engine* e, int32_t op, const int32_t* dims, int32_t n_dims, const float* scal, int32_t n_scal,
+                    const float* const* in, const int64_t* in_len, int32_t n_in, float* out, int64_t out_len);
 
 #ifdef __cplusplus
 }

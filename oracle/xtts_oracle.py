@@ -425,14 +425,14 @@ def mel_cloning(wav: torch.Tensor, mel_stats: torch.Tensor, n_mels: int = 80) ->
     (common/utilities.py:53-70 with the args of XTTSv2.py:374-386)."""
     from auralis_b200.weights import mel_filterbank
     n_fft, hop, win = 2048, 256, 1024
-    window = torch.hann_window(win)
+    window = torch.hann_window(win, dtype=wav.dtype)
     spec = torch.stft(wav, n_fft, hop, win, window=window, center=True, pad_mode="reflect",
                       normalized=False, onesided=True, return_complex=True)
     power = spec.real ** 2 + spec.imag ** 2                   # [1025, frames]
-    fb = mel_filterbank(n_fft // 2 + 1, 0.0, 8000.0, n_mels, 22050, "slaney")  # [1025, n_mels]
+    fb = mel_filterbank(n_fft // 2 + 1, 0.0, 8000.0, n_mels, 22050, "slaney").to(wav.dtype)  # [1025, n_mels]
     mel = (power.t() @ fb).t()
     mel = torch.log(torch.clamp(mel, min=1e-5))
-    return mel / mel_stats[:, None]
+    return mel / mel_stats.to(wav.dtype)[:, None]
 
 
 def cond_encoder(mel: torch.Tensor, core: State, dims) -> torch.Tensor:
@@ -513,21 +513,27 @@ def gpt_cond_latents(wav22k: torch.Tensor, core: State, dims, length: int = 30, 
     return torch.stack(embs).mean(dim=0)
 
 
+def speaker_frontend(wav16k: torch.Tensor, core: State) -> torch.Tensor:
+    """wav [N] @16k -> InstanceNorm'd log-mel [1, 64, frames] in wav's dtype (hifigan_decoder.py:452-482, 602-613)."""
+    s = "hifigan_decoder.speaker_encoder."
+    dt = wav16k.dtype
+    x = wav16k[None]
+    x = F.pad(x[:, None], (1, 0), mode="reflect")
+    x = F.conv1d(x, core[s + "torch_spec.0.filter"].to(dt))[:, 0]
+    spec = torch.stft(x[0], 512, 160, 400, window=core[s + "torch_spec.1.spectrogram.window"].to(dt),
+                      center=True, pad_mode="reflect", normalized=False, onesided=True,
+                      return_complex=True)
+    power = spec.real ** 2 + spec.imag ** 2                     # [257, frames]
+    mel = (power.t() @ core[s + "torch_spec.1.mel_scale.fb"].to(dt)).t()[None]   # [1,64,frames]
+    mel = torch.log(mel + 1e-6)
+    return F.instance_norm(mel)                                  # nn.InstanceNorm1d(64), no affine
+
+
 def speaker_embedding(wav16k: torch.Tensor, core: State, dims) -> torch.Tensor:
     """wav [N] @16k -> L2-normalised d-vector [proj]  (hifigan_decoder.py:452-482, 602-646)."""
     c = dims.cond
     s = "hifigan_decoder.speaker_encoder."
-    x = wav16k[None]
-    x = F.pad(x[:, None], (1, 0), mode="reflect")
-    x = F.conv1d(x, core[s + "torch_spec.0.filter"])[:, 0]
-    spec = torch.stft(x[0], 512, 160, 400, window=core[s + "torch_spec.1.spectrogram.window"],
-                      center=True, pad_mode="reflect", normalized=False, onesided=True,
-                      return_complex=True)
-    power = spec.real ** 2 + spec.imag ** 2                     # [257, frames]
-    mel = (power.t() @ core[s + "torch_spec.1.mel_scale.fb"]).t()[None]   # [1,64,frames]
-    mel = torch.log(mel + 1e-6)
-    mel = F.instance_norm(mel)                                   # nn.InstanceNorm1d(64), no affine
-    x = mel[:, None]
+    x = speaker_frontend(wav16k, core)[:, None]
 
     def bn(x, pfx):
         return F.batch_norm(x, core[pfx + ".running_mean"], core[pfx + ".running_var"],

@@ -32,15 +32,33 @@ def test_condition_matches_reference_golden(name, request):
     assert abs(np.linalg.norm(g) - 1.0) < 1e-4
 
 
+def _check_against_oracle(eng, dims, state, w22, w16, slot):
+    eng.condition(slot, w22, w16, 30, 4)
+    cond, g = eng.get_speaker(slot)
+    rc, rg = _ref(dims, state[1], w22, w16)
+    print("oracle", dims.gpt.hidden, len(w16), "cond err", np.abs(cond - rc).max(), "max", np.abs(rc).max(),
+          "dvec err", np.abs(g - rg).max())
+    assert np.abs(cond - rc).max() < 2e-3 * max(1.0, np.abs(rc).max()), np.abs(cond - rc).max()
+    assert np.abs(g - rg).max() < 2e-4, np.abs(g - rg).max()
+
+
 def test_condition_multi_piece_small(engine_small, dims_small, state_small):
     """6 s reference cut into 4 s pieces (one 4 s + one 2 s), averaged (XTTSv2.py:361-391)."""
     w22 = O.synthetic_reference_wav(6.0, 22050, 140.0, 3).numpy()
     w16 = O.synthetic_reference_wav(6.0, 16000, 140.0, 3).numpy()
-    engine_small.condition(5, w22, w16, 30, 4)
-    cond, g = engine_small.get_speaker(5)
-    rc, rg = _ref(dims_small, state_small[1], w22, w16)
-    assert np.abs(cond - rc).max() < 2e-3 * max(1.0, np.abs(rc).max()), np.abs(cond - rc).max()
-    assert np.abs(g - rg).max() < 2e-4, np.abs(g - rg).max()
+    _check_against_oracle(engine_small, dims_small, state_small, w22, w16, 5)
+
+
+# 16 kHz lengths: T = 1 + N/160 frames is odd at 1.00 s (101) and 10.5 s (1051), even at 1.01 s (102).  An odd T leaves
+# the stride-2 layers an odd width to round up (the downsample branch writes ceil(T/2) columns), and 10.5 s makes layer
+# 4 132 columns wide, more than one 128-wide conv2d block.  The 6 s case above has T = 601.
+@pytest.mark.parametrize("name,sec16", [("small", 1.0), ("small", 1.01), ("full", 1.0), ("full", 1.01), ("small", 10.5)])
+def test_condition_dvector_lengths_match_oracle(name, sec16, request):
+    """The d-vector of a 16 kHz reference of sec16 seconds (and the latents of the same 6 s 22.05 kHz reference)."""
+    eng = request.getfixturevalue(f"engine_{name}")
+    w22 = O.synthetic_reference_wav(6.0, 22050, 140.0, 3).numpy()
+    w16 = O.synthetic_reference_wav(sec16, 16000, 140.0, 3).numpy()
+    _check_against_oracle(eng, request.getfixturevalue(f"dims_{name}"), request.getfixturevalue(f"state_{name}"), w22, w16, 5)
 
 
 def test_condition_truncation_and_short_tail(engine_small, dims_small, state_small):
