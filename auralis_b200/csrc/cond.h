@@ -115,6 +115,26 @@ private:
     std::unique_ptr<Impl> impl;
 };
 
+// Resampler (resample.cu): torchaudio.functional.resample with its defaults (sinc_interp_hann, lowpass_filter_width 6,
+// rolloff 0.99) on float32 mono audio, for speaker references, conditioning and TTSOutput.resample.  Needs no weights.
+// Evaluates only the taps inside the filter's window, from a band table cached for the last rate pair, and works in
+// passes of at most `block_samples` outputs, so its workspace does not grow with the input.
+class Resampler {
+public:
+    explicit Resampler(cudaStream_t st);
+    ~Resampler();
+    // ceil(M n / L) (n when orig == new_sr); 0 for a rate outside 1 .. 2^20 - 1 or n outside 0 .. 2^40.
+    static int64_t out_len(int64_t n, int orig, int new_sr);
+    // wav: host, n samples at orig Hz.  Writes out_len(n, orig, new_sr) samples at new_sr Hz to `out` (host).  Throws
+    // std::invalid_argument for a rate out of range, n < 0, a NULL pointer, cap too small or a non-finite sample
+    // (orig == new_sr copies the samples as they are).  The result does not depend on block_samples.
+    int64_t run(const float* wav, int64_t n, int orig, int new_sr, float* out, int64_t cap, int block_samples);
+
+private:
+    struct Impl;
+    std::unique_ptr<Impl> impl;
+};
+
 // FLAC encoder (flac.cu): mono 16-bit PCM -> a complete lossless FLAC stream (RFC 9639), for TTSOutput.to_bytes("flac").
 // Needs no weights.  Works in batches of at most `batch_frames` 4096-sample frames, so its device memory does not grow
 // with the input; only the host holds the whole input and stream.

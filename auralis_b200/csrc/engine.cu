@@ -159,6 +159,7 @@ public:
     void condition(int slot, const float* w22, int64_t n22, const float* w16, int64_t n16, int cond_len, int chunk_len);
     int64_t enhance(const float* wav, int64_t n, const xtts_enhance_config& c, float* out, int64_t cap);
     int64_t change_speed(const float* wav, int64_t n, double rate, float* out, int64_t cap);
+    int64_t resample(const float* wav, int64_t n, int orig_sr, int new_sr, float* out, int64_t cap);
     int64_t encode_flac(const int16_t* pcm, int64_t n, int sample_rate, const uint8_t* md5, uint8_t* out, int64_t cap,
                         int64_t* n_out);
     int64_t decode_flac(const uint8_t* data, int64_t n, int32_t* out, int64_t cap, xtts_flac_info* info);
@@ -257,6 +258,8 @@ private:
     std::unique_ptr<Enhancer> enhancer;          // built on the first xtts_enhance
     std::unique_ptr<PhaseVocoder> pvoc;          // built on the first xtts_change_speed
     int pvoc_block_frames = 4096;                // option "pvoc_block_frames"
+    std::unique_ptr<Resampler> resampler;        // built on the first xtts_resample
+    int resample_block_samples = 1 << 22;        // option "resample_block_samples"
     std::unique_ptr<FlacEncoder> flac;           // built on the first xtts_encode_flac
     std::unique_ptr<FlacDecoder> flac_dec;       // built on the first xtts_decode_flac
     int flac_batch_frames = 8192;                // option "flac_batch_frames" (encoder and decoder)
@@ -884,6 +887,17 @@ int64_t Engine::change_speed(const float* wav, int64_t n, double rate, float* ou
     const double t0 = now_s();
     if (!pvoc) pvoc.reset(new PhaseVocoder(st));
     const int64_t n_out = pvoc->run(wav, n, rate, out, cap, pvoc_block_frames);
+    st_cond_ms += (now_s() - t0) * 1e3;
+    return n_out;
+}
+
+// torchaudio.functional.resample (common/utilities.py:94, XTTSv2.py:322,362, TTSOutput.resample), on the conditioning stream
+int64_t Engine::resample(const float* wav, int64_t n, int orig_sr, int new_sr, float* out, int64_t cap) {
+    ApiLock lk(this);
+    CUDA_CHECK(cudaSetDevice(cfg.device));
+    const double t0 = now_s();
+    if (!resampler) resampler.reset(new Resampler(st));
+    const int64_t n_out = resampler->run(wav, n, orig_sr, new_sr, out, cap, resample_block_samples);
     st_cond_ms += (now_s() - t0) * 1e3;
     return n_out;
 }
@@ -2028,6 +2042,10 @@ void Engine::set_option(const std::string& k, int64_t v) {
         if (v < 1 || v > (1 << 20)) throw std::runtime_error("pvoc_block_frames: 1 .. 2^20 output frames");
         pvoc_block_frames = (int)v;
     }
+    else if (k == "resample_block_samples") {
+        if (v < 1 || v > (1 << 26)) throw std::runtime_error("resample_block_samples: 1 .. 2^26 output samples");
+        resample_block_samples = (int)v;
+    }
     else if (k == "flac_batch_frames") {
         if (v < 1 || v > (1 << 20)) throw std::runtime_error("flac_batch_frames: 1 .. 2^20 frames");
         flac_batch_frames = (int)v;
@@ -2932,6 +2950,12 @@ int xtts_change_speed(xtts_engine* e, const float* wav, int64_t n, double rate, 
     if (!n_out) { xtts::set_error("null argument"); return XTTS_ERR_INVALID; }
     *n_out = xtts::PhaseVocoder::out_len(n, rate);
     XTTS_TRY(*n_out = e->impl->change_speed(wav, n, rate, out, cap))
+}
+int xtts_resample(xtts_engine* e, const float* wav, int64_t n, int32_t orig_sr, int32_t new_sr, float* out, int64_t cap,
+                  int64_t* n_out) {
+    if (!n_out) { xtts::set_error("null argument"); return XTTS_ERR_INVALID; }
+    *n_out = xtts::Resampler::out_len(n, orig_sr, new_sr);
+    XTTS_TRY(*n_out = e->impl->resample(wav, n, orig_sr, new_sr, out, cap))
 }
 int xtts_encode_flac(xtts_engine* e, const int16_t* pcm, int64_t n, int32_t sample_rate, const uint8_t* md5,
                      uint8_t* out, int64_t cap, int64_t* n_out) {

@@ -66,12 +66,13 @@ class ChunkOutput:
 
 
 def load_audio(source: Union[str, Path, bytes], sampling_rate: int) -> np.ndarray:
-    """Mono float32 in [-1,1] at `sampling_rate` (common/utilities.py:72-97: mean over channels, torchaudio sinc resampling,
-    clip).  RIFF/WAV — integer PCM and IEEE float — is decoded here (torchaudio.load needs a codec backend this image does
-    not ship).  FLAC (optionally behind an ID3v2 tag) is decoded losslessly on the GPU while an `XTTSv2Engine` is alive
-    and scaled v / 2^(bits - 1) into the same [frames, channels] float32 array an integer WAV gives, so a FLAC
-    reference conditions exactly like the same PCM in a WAV; a corrupt stream raises ValueError.  Any other container,
-    and FLAC with no engine alive, goes through torchaudio.load when it can."""
+    """Mono float32 in [-1,1] at `sampling_rate` (common/utilities.py:72-97: mean over channels, torchaudio's sinc
+    resampler — on the GPU while an `XTTSv2Engine` is alive, see `_resample` — and clip).  RIFF/WAV — integer PCM and
+    IEEE float — is decoded here (torchaudio.load needs a codec backend this image does not ship).  FLAC (optionally
+    behind an ID3v2 tag) is decoded losslessly on the GPU while an `XTTSv2Engine` is alive and scaled v / 2^(bits - 1)
+    into the same [frames, channels] float32 array an integer WAV gives, so a FLAC reference conditions exactly like the
+    same PCM in a WAV; a corrupt stream raises ValueError.  Any other container, and FLAC with no engine alive, goes
+    through torchaudio.load when it can."""
     from .output import _parse_flac, _parse_riff_wav
     if isinstance(source, (bytes, bytearray)):
         blob = bytes(source)
@@ -157,7 +158,7 @@ class XTTSv2Engine(BaseAsyncTTSEngine):
         self._pollers = [threading.Thread(target=self._poll_loop, args=(i,), name=f"xtts-poll-{i}", daemon=True)
                          for i in range(len(self.natives))]
         [t.start() for t in self._pollers]
-        _output.register_gpu_provider(self)             # change_speed and FLAC output / input run here while it lives
+        _output.register_gpu_provider(self)             # change_speed, FLAC in / out and resampling run here while it lives
 
     # ---- plugin API -------------------------------------------------------------------------
     @classmethod
@@ -478,6 +479,22 @@ class XTTSv2Engine(BaseAsyncTTSEngine):
                 raise ValueError(str(e)) from e
             raise
 
+    def resample(self, array, orig_sr: int, new_sr: int) -> np.ndarray:
+        """`TTSOutput.resample` and speaker-reference resampling on the first GPU (``xtts_resample``):
+        torchaudio.functional.resample(array, orig_sr, new_sr) with its defaults, float32 [..., N] -> float32
+        [..., ceil(new' N / orig')] (the rates over their gcd), each row on its own.  A rate outside 1 .. 1048575 or a
+        non-finite sample raises ValueError."""
+        a = np.ascontiguousarray(array, np.float32)
+        if a.ndim == 0 or 0 in a.shape[:-1]:
+            raise ValueError("resample needs at least one row of samples")
+        try:
+            rows = [self.native.resample(r, orig_sr, new_sr) for r in a.reshape(-1, a.shape[-1])]
+        except native.NativeError as e:
+            if e.code == native.ERR_INVALID:
+                raise ValueError(str(e)) from e
+            raise
+        return np.stack(rows).reshape(a.shape[:-1] + rows[0].shape)
+
     def encode_flac(self, pcm_i16, sample_rate: int, md5: Optional[bytes] = None) -> bytes:
         """`TTSOutput.to_bytes("flac")` on the first GPU (``xtts_encode_flac``): a lossless FLAC stream of mono int16
         samples, with `md5` (16 bytes, or None for zeros) in its STREAMINFO.  A sample rate outside 1 .. 1048575 raises
@@ -577,10 +594,14 @@ class _SpeakerArray(np.ndarray):
 
 
 def _resample(a: np.ndarray, sr: int, new_sr: int) -> np.ndarray:
-    """torchaudio.functional.resample (the reference's resampler, XTTSv2.py:323,360) when importable,
-    scipy polyphase otherwise.  Host-side preprocessing of the reference wav, not part of the hot path."""
+    """torchaudio.functional.resample (the reference's resampler, XTTSv2.py:323,360): on the GPU of a live engine
+    (`output.gpu_resample`), else torchaudio on the host when importable, scipy polyphase otherwise.  Every resample of a
+    speaker reference goes through here."""
     if sr == new_sr:
         return a
+    y = _output.gpu_resample(a, sr, new_sr)
+    if y is not None:
+        return y
     try:
         import torch
         import torchaudio

@@ -110,7 +110,7 @@ class XttsKernelProfile(C.Structure):
 # every symbol include/xtts_b200.h declares (checked by tests/test_abi.py against the header text)
 ABI_SYMBOLS = [
     "xtts_last_error", "xtts_version", "xtts_create", "xtts_destroy", "xtts_load_weight", "xtts_finalize_weights",
-    "xtts_set_speaker", "xtts_get_speaker", "xtts_condition", "xtts_enhance", "xtts_change_speed", "xtts_encode_flac", "xtts_decode_flac", "xtts_submit", "xtts_submit_speed", "xtts_cancel", "xtts_poll",
+    "xtts_set_speaker", "xtts_get_speaker", "xtts_condition", "xtts_enhance", "xtts_change_speed", "xtts_resample", "xtts_encode_flac", "xtts_decode_flac", "xtts_submit", "xtts_submit_speed", "xtts_cancel", "xtts_poll",
     "xtts_fetch", "xtts_set_option", "xtts_get_stats", "xtts_sync", "xtts_get_kernel_profile", "xtts_device_timer", "xtts_vocode",
     "xtts_vocode_window", "xtts_vocode_speed", "xtts_gpt_prefill", "xtts_gpt_teacher_forced",
     "xtts_debug_gemm", "xtts_debug_sample_slots", "xtts_debug_trace",
@@ -151,6 +151,7 @@ def load_library(path: Optional[str] = None):
     lib.xtts_condition.argtypes = [vp, i32, f32p, i64, f32p, i64, i32, i32]
     lib.xtts_enhance.argtypes = [vp, f32p, i64, C.POINTER(XttsEnhanceConfig), f32p, i64, C.POINTER(i64)]
     lib.xtts_change_speed.argtypes = [vp, f32p, i64, C.c_double, f32p, i64, C.POINTER(i64)]
+    lib.xtts_resample.argtypes = [vp, f32p, i64, i32, i32, f32p, i64, C.POINTER(i64)]
     u8p = C.POINTER(C.c_uint8)
     lib.xtts_encode_flac.argtypes = [vp, C.POINTER(C.c_int16), i64, i32, u8p, u8p, i64, C.POINTER(i64)]
     lib.xtts_decode_flac.argtypes = [vp, u8p, i64, i32p, i64, C.POINTER(XttsFlacInfo)]
@@ -352,6 +353,21 @@ class NativeEngine:
         cap = 512 * (frames - 1) if frames <= 1 << 22 else 0          # longer results are rejected by the call
         out = np.empty((max(cap, 1),), np.float32)
         self._chk(self.lib.xtts_change_speed(self.h, _fp(a), a.size, rate, _fp(out), cap, C.byref(n_out)), "change_speed")
+        return out[: n_out.value]
+
+    def resample(self, wav, orig_sr: int, new_sr: int) -> np.ndarray:
+        """xtts_resample: torchaudio.functional.resample(wav, orig_sr, new_sr) with its defaults, on the GPU, for mono
+        float32 audio -> float32 [ceil(new' n / orig')] (the rates over their gcd).  orig_sr == new_sr returns the samples
+        unchanged.  Raises NativeError with code ERR_INVALID for a rate outside 1 .. 1048575 or a non-finite sample."""
+        a = _f32(wav).reshape(-1)
+        orig_sr, new_sr = int(orig_sr), int(new_sr)
+        cap = 0                                                           # bad rates are rejected by the call
+        if 0 < orig_sr < 1 << 20 and 0 < new_sr < 1 << 20:
+            g = math.gcd(orig_sr, new_sr)
+            cap = -(-(new_sr // g) * a.size // (orig_sr // g))
+        out = np.empty((max(cap, 1),), np.float32)
+        n_out = C.c_int64(0)
+        self._chk(self.lib.xtts_resample(self.h, _fp(a), a.size, orig_sr, new_sr, _fp(out), cap, C.byref(n_out)), "resample")
         return out[: n_out.value]
 
     def encode_flac(self, pcm_i16, sample_rate: int, md5: Optional[bytes] = None) -> bytes:

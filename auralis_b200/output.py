@@ -3,8 +3,9 @@
 Mirrors `/root/reference/src/auralis/common/definitions/output.py:17-38,95-111` for the fields and
 ``combine_outputs``.  ``change_speed`` (the reference's librosa phase vocoder + peak normalisation), 16-bit FLAC
 (``to_bytes("flac")``, a lossless LPC + partitioned-Rice encoder) and FLAC input (``from_file``, a lossless RFC 9639
-decoder) run on the GPU of a live `XTTSv2Engine` (``register_gpu_provider``), and on librosa / torchaudio when no
-engine is alive.  The other audio utilities (mp3/opus/aac
+decoder) and ``resample`` (torchaudio's windowed-sinc resampler, also used for speaker references) run on the GPU of a
+live `XTTSv2Engine` (``register_gpu_provider``), and on librosa / torchaudio when no engine is alive.  The other audio
+utilities (mp3/opus/aac
 encoders, playback) are CPU post-processing outside the hot path (SURVEY.md §2.1 #3): wav/pcm paths are provided with the
 standard library, the rest raise with a clear message when their optional dependency is absent.
 """
@@ -110,11 +111,12 @@ _providers_lock = threading.Lock()
 
 def register_gpu_provider(engine) -> None:
     """Route `TTSOutput.change_speed` to `engine.change_speed(array, speed_factor) -> np.ndarray`, 16-bit
-    `TTSOutput.to_bytes("flac")` to `engine.encode_flac(pcm_i16, sample_rate, md5) -> bytes`, and FLAC input
+    `TTSOutput.to_bytes("flac")` to `engine.encode_flac(pcm_i16, sample_rate, md5) -> bytes`, FLAC input
     (`TTSOutput.from_file`, `engine.load_audio`) to `engine.decode_flac(blob) -> (int32 [C, N], sample_rate,
-    bits_per_sample)`, each when the engine has that method, while the engine is alive (`XTTSv2Engine` registers itself
-    when it is built).  Held through a weak reference, so the registry never keeps an engine alive; the most recently
-    registered live engine serves."""
+    bits_per_sample)`, and every resample (`TTSOutput.resample`, speaker references and conditioning through
+    `engine._resample`) to `engine.resample(array [..., N], orig_sr, new_sr) -> float32 [..., N']`, each when the engine
+    has that method, while the engine is alive (`XTTSv2Engine` registers itself when it is built).  Held through a weak
+    reference, so the registry never keeps an engine alive; the most recently registered live engine serves."""
     with _providers_lock:
         _providers[:] = [r for r in _providers if r() is not None and r() is not engine]
         _providers.append(weakref.ref(engine))
@@ -127,13 +129,38 @@ def unregister_gpu_provider(engine) -> None:
 
 
 def gpu_provider():
-    """The engine `TTSOutput.change_speed`, `TTSOutput.to_bytes("flac")` and FLAC input run on, or None."""
+    """The engine `TTSOutput.change_speed`, `TTSOutput.to_bytes("flac")`, FLAC input and resampling run on, or None."""
     with _providers_lock:
         for r in reversed(_providers):
             e = r()
             if e is not None:
                 return e
     return None
+
+
+def _is_rate(r) -> bool:
+    """A positive integer sample rate: an int, or a float with an integral value."""
+    if isinstance(r, (bool, np.bool_)):
+        return False
+    if isinstance(r, (int, np.integer)):
+        return r > 0
+    return isinstance(r, (float, np.floating)) and float(r).is_integer() and r > 0
+
+
+def gpu_resample(a, orig_sr, new_sr) -> Optional[np.ndarray]:
+    """float32 `a` [..., N] at `orig_sr` -> float32 [..., N'] at `new_sr`, computed by the live engine's `resample`
+    (torchaudio's windowed-sinc resampler on the GPU, with torchaudio's numbers up to fp32 rounding).  None when there is
+    no live engine with `resample`, `a` is not float32, a rate is not a positive integer, or the engine rejects the call
+    (a non-finite sample, a rate above 1048575): the caller then resamples on the host, as without an engine.  The one
+    place `TTSOutput.resample` and `engine._resample` choose between the GPU and the host."""
+    gpu = gpu_provider()
+    a = np.asarray(a)
+    if gpu is None or not hasattr(gpu, "resample") or a.dtype != np.float32 or not (_is_rate(orig_sr) and _is_rate(new_sr)):
+        return None
+    try:
+        return gpu.resample(a, int(orig_sr), int(new_sr))
+    except ValueError:
+        return None
 
 
 @dataclass
@@ -258,8 +285,14 @@ class TTSOutput:
             f.write(data)
 
     def resample(self, new_sample_rate: int) -> "TTSOutput":
-        """output.py:224-246: torchaudio's windowed-sinc resampler, like the reference; scipy's polyphase filter only when
-        torchaudio cannot be imported."""
+        """output.py:224-246: torchaudio's windowed-sinc resampler, like the reference.  While an `XTTSv2Engine` is alive
+        it runs on its first GPU (`xtts_resample`, torchaudio's float32 coefficients over the taps inside the filter's
+        window), one row at a time for [C, N]; otherwise, and for input the GPU call rejects (a non-finite sample, a
+        rate above 1048575), torchaudio on the host, and scipy's polyphase filter only when torchaudio cannot be
+        imported.  The result is float32 and squeezed like torchaudio's: [N] -> [N'], [C, N] -> [C, N']."""
+        y = gpu_resample(np.ascontiguousarray(self.array, np.float32), self.sample_rate, new_sample_rate)
+        if y is not None:
+            return TTSOutput(array=np.squeeze(y), sample_rate=new_sample_rate)
         try:
             import torch
             import torchaudio

@@ -10,8 +10,8 @@ each behind its ``audio_config`` flag), but on the GPU (``xtts_enhance``) and on
 like the reference.  Where the reference would fail (audio too short for a VAD frame or a 400 ms loudness block, a
 non-finite result) the original file is used, with a warning.  Unlike the reference, ``speaker_files`` is not rewritten to
 enhanced temporary files: the request keeps its paths, and the engine enhances while it conditions (the speaker cache
-key includes ``audio_config``).  The audio is loaded at ``audio_config.sample_rate`` with torchaudio's sinc resampler,
-not librosa's soxr.
+key includes ``audio_config``).  The audio is loaded at ``audio_config.sample_rate`` with torchaudio's sinc resampler
+(computed on the GPU, ``xtts_resample``), not librosa's soxr.
 
 Additions (not in the reference): ``seed`` (reproducible sampling) and ``speed``, the speaking rate in [0.25, 4.0] (> 1 is
 faster; the reference offers speed only in its OpenAI server, as a CPU phase vocoder on the finished waveform).  Here it

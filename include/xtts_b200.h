@@ -154,6 +154,22 @@ int xtts_enhance(xtts_engine* e, const float* wav, int64_t n, const xtts_enhance
  * Runs on the conditioning stream; its time counts in xtts_stats.cond_ms. */
 int xtts_change_speed(xtts_engine* e, const float* wav, int64_t n, double rate, float* out, int64_t cap, int64_t* n_out);
 
+/* torchaudio.functional.resample(wav, orig_sr, new_sr) with its defaults (sinc_interp_hann, lowpass_filter_width 6,
+ * rolloff 0.99), the reference's resampler for speaker files, conditioning and TTSOutput.resample (common/utilities.py:94,
+ * models/base.py:220, XTTSv2.py:322,362), on the GPU: wav n mono float32 samples at orig_sr Hz -> *n_out = ceil(M n / L)
+ * samples at new_sr Hz (L, M = the rates over their gcd).  Coefficients are torchaudio's float32 kernel, built with its
+ * operation order; only the taps whose scaled argument lies strictly inside the window (-6, 6) are evaluated (at most
+ * 2 width + 2 per output, width = ceil(6 L / (0.99 min(L, M)))).  The taps torchaudio also evaluates have the clamped
+ * argument +-6 and coefficients below 5e-24.  Each output is an fp32 FMA chain in a fixed tap order, so it does not
+ * depend on the launch shape.  Input outside [0, n) reads as 0.  orig_sr == new_sr copies the samples; n == 0 gives 0.
+ * Workspace: a band table of about M (2 width + 2) floats, cached for the last rate pair, and passes of at most
+ * "resample_block_samples" outputs with the input they read (2 x that many + 2 width + L floats); bit-identical for
+ * every value.  *n_out is always set (0 for an invalid rate or length); cap < *n_out fails.  XTTS_ERR_INVALID: a rate
+ * outside 1 .. 1048575, n < 0, a NULL pointer with n > 0, cap < *n_out, a non-finite sample (checked on the device).
+ * Runs on the conditioning stream; its time counts in xtts_stats.cond_ms. */
+int xtts_resample(xtts_engine* e, const float* wav, int64_t n, int32_t orig_sr, int32_t new_sr, float* out, int64_t cap,
+                  int64_t* n_out);
+
 /* TTSOutput.to_bytes("flac") (output.py:119-187): a complete, lossless FLAC stream (RFC 9639) of n mono 16-bit samples
  * at sample_rate Hz, encoded on the GPU.  "fLaC", one STREAMINFO block (min/max block size 4096, the real min/max frame
  * sizes, total samples n, the 16-byte md5 the caller passes or zeros for NULL = "not computed"), then fixed blocks of
@@ -242,6 +258,9 @@ int xtts_fetch(xtts_engine* e, uint64_t seq_id, int32_t* tokens, float* wav, flo
  *                         many x 4096 samples, all channels together (one larger frame is a batch alone); about 4 B
  *                         per sample (12 B at 32 bits) beside the compressed stream, which is whole on the device.
  *                         Identical samples for every value.
+ *   "resample_block_samples"   xtts_resample's pass: at most this many output samples, and the input they read (at most
+ *                         this many + 2 width + L samples) per pass, 1 .. 2^26, default 2^22 (about 32 MB of device memory
+ *                         at the default, whatever the input length).  Bit-identical results for every value.
  *   "tc_epilogue"         epilogue of the fast-mode vocoder's tensor-core Conv1d: 1 (default) = staged through shared
  *                         memory (residual prefetched by a loader warp, outputs drained by bulk copies while the next
  *                         tile's MMAs run), 0 = straight from the accumulators.  Bit-identical results either way.
