@@ -85,6 +85,7 @@ class VocoderDims:
 
 
 SPEED_MIN, SPEED_MAX = 0.25, 4.0     # speaking-rate range (that of OpenAI's /v1/audio/speech)
+NUM_BEAMS_MAX = 8                   # beams per chunk (TTSRequest.num_beams, xtts_submit_beams)
 
 
 def speed_scale(speed: float) -> float:

@@ -90,6 +90,8 @@ struct Sequence {
     int speaker = 0;
     xtts_sampling sp{};
     float speed = 1.f;            // speaking rate (xtts_submit_speed): time-scales the latents before the vocoder
+    xtts_beam beam{1, 1.f, 0};    // xtts_submit_beams: num_beams > 1 decodes the chunk as a beam-search group
+    std::vector<int> beam_slots;  // the group's slots, beam j in beam_slots[j]; beam_slots[0] == slot (the primary)
     int slot = -1;
     int n_prompt = 0;
     int max_tok = 0;              // min(sp.max_tokens, max_audio_tokens)
@@ -163,7 +165,8 @@ public:
     int64_t encode_flac(const int16_t* pcm, int64_t n, int sample_rate, const uint8_t* md5, uint8_t* out, int64_t cap,
                         int64_t* n_out);
     int64_t decode_flac(const uint8_t* data, int64_t n, int32_t* out, int64_t cap, xtts_flac_info* info);
-    void submit(uint64_t id, const int32_t* text, int n_text, int speaker, const xtts_sampling& sp, float speed);
+    void submit(uint64_t id, const int32_t* text, int n_text, int speaker, const xtts_sampling& sp, float speed,
+                const xtts_beam* beam = nullptr);
     void cancel(uint64_t id);
     int poll(xtts_result* out, int timeout_ms);
     void fetch(uint64_t id, int32_t* tokens, float* wav, float* latents);
@@ -215,6 +218,10 @@ public:
     void debug_conv_tc(int up, int Cin, int Cout, int K, int dil, int batch, int L, const int32_t* item_len, const float* w,
                        const float* bias, const float* cbias, int cbias_stride, const float* x, const float* resid, int mode,
                        float slope_out, float scale16, int max_ctas, float* out32, float* out16);
+    void debug_beam_step(int kv_type, int heads, int layers, int Vn, const xtts_sampling& sp, const xtts_beam& bm, int first,
+                         int advance, const float* logits, int32_t* n_gen, int32_t* ctx_len, int32_t* last_tok, uint32_t* seen,
+                         int mp, int32_t* block_tables, int n_pages, int32_t* pool, int cap, int32_t* hist,
+                         xtts_beam_state* state, void* kpool, void* vpool, float* scores);
     void debug_cond(int op, const int32_t* dims, int n_dims, const float* scal, int n_scal, const float* const* in,
                     const int64_t* in_len, int n_in, float* out, int64_t out_len);
 
@@ -276,6 +283,18 @@ private:
     DBuf<unsigned> d_seen;
     DBuf<float> d_temp, d_top_p, d_pen;
     DBuf<unsigned long long> d_seed;
+    DBuf<int> d_beam_flag;        // [NSLOT] SampleState::beam
+    // beam search (beam.cu): per-group state, history and page pool indexed by the primary slot, scores per slot
+    DBuf<BeamState> d_beam_state;
+    DBuf<int2> d_beam_hist;
+    DBuf<int> d_beam_pool;
+    DBuf<float> d_beam_scores;
+    DBuf<BeamDesc> d_beam_desc;
+    BeamDesc* h_beam_desc = nullptr;               // pinned [NSLOT]
+    BeamState* h_beam_init = nullptr;              // pinned [NSLOT]: initial state of the groups of an admission wave
+    int* h_beam_pool = nullptr;                    // pinned [NSLOT][beam_pool_cap]: their page pools
+    DBuf<void*> d_kv_ptrs;                          // [2][L] K then V pool of each layer
+    int beam_pool_cap = 0;
     DBuf<float> d_latents;
     DBuf<RowDesc> d_rows;
     DBuf<AttnSeq> d_attnseq;
@@ -408,6 +427,7 @@ private:
     int build_prefill(const std::vector<Sequence*>& seqs, const std::vector<std::vector<int32_t>>& audio,
                       std::vector<int>& last_rows, int& max_nq);
     void prefill(const std::vector<Sequence*>& seqs);
+    void beam_step(const std::vector<Sequence*>& groups, const std::vector<int>& rows0, bool first);
     void decode_step(const std::vector<int>& active);
     void run_vocoder(const VocItem* it, int nb, float* wav_dev_out, const char* stage, float* stage_out, int64_t stage_cap);
     int samples_for(int T, float speed = 1.f) const;
@@ -501,6 +521,14 @@ Engine::Engine(const xtts_config& c) : cfg(c) {
     d_seen.alloc((size_t)NSLOT * SEENW);
     d_block_tables.alloc((size_t)NSLOT * max_pages);
     d_active.alloc(NSLOT);
+    d_beam_flag.alloc(NSLOT); d_beam_flag.zero(st);
+    beam_pool_cap = kMaxBeams * max_pages;
+    d_beam_state.alloc(NSLOT); d_beam_hist.alloc((size_t)NSLOT * CAP * kMaxBeams); d_beam_pool.alloc((size_t)NSLOT * beam_pool_cap);
+    d_beam_desc.alloc(NSLOT);
+    CUDA_CHECK(cudaMallocHost(&h_beam_desc, NSLOT * sizeof(BeamDesc)));
+    CUDA_CHECK(cudaMallocHost(&h_beam_init, NSLOT * sizeof(BeamState)));
+    CUDA_CHECK(cudaMallocHost(&h_beam_pool, (size_t)NSLOT * beam_pool_cap * sizeof(int)));
+    beam_init_device();
     d_latents.alloc((size_t)NSLOT * CAP * H);
     d_finished.zero(st); d_n_gen.zero(st); d_ctx_len.zero(st); d_last_tok.zero(st);
     CUDA_CHECK(cudaMallocHost(&h_finished, 2 * NSLOT * sizeof(int)));
@@ -516,6 +544,7 @@ Engine::Engine(const xtts_config& c) : cfg(c) {
     d_attnseq.alloc(NSLOT);
     const size_t Mmax = (size_t)std::max(prefill_rows_cap, NSLOT);
     wX.alloc(Mmax * H); wQKV.alloc(Mmax * 3 * H); wLOG.alloc((size_t)std::max(NSLOT, CAP + 1) * Vpad);
+    d_beam_scores.alloc((size_t)NSLOT * Vpad);
     if (bf16) wPART.alloc((size_t)8 * NSLOT * H);
     d_chain_sync.alloc(64); d_chain_sync.zero(st);
     d_dep.alloc((size_t)kMaxMicro * L * 7); d_dep.zero(st);
@@ -533,6 +562,15 @@ Engine::Engine(const xtts_config& c) : cfg(c) {
             k32.emplace_back(new DBuf<float>()); v32.emplace_back(new DBuf<float>());
             k32.back()->alloc(total_pages * page_elems); v32.back()->alloc(total_pages * page_elems);
         }
+    }
+    {
+        std::vector<void*> kv(2 * L);
+        for (int l = 0; l < L; ++l) {
+            kv[l] = bf16 ? (void*)k16[l]->p : (void*)k32[l]->p;
+            kv[L + l] = bf16 ? (void*)v16[l]->p : (void*)v32[l]->p;
+        }
+        d_kv_ptrs.alloc(2 * L); d_kv_ptrs.upload(kv.data(), 2 * L, st);
+        CUDA_CHECK(cudaStreamSynchronize(st));
     }
     for (int p = total_pages - 1; p >= 0; --p) free_pages.push_back(p);
     for (int s = B - 1; s >= 0; --s) free_slots.push_back(s);
@@ -606,6 +644,9 @@ Engine::~Engine() {
     if (h_finished) cudaFreeHost(h_finished);
     if (h_slot_init) cudaFreeHost(h_slot_init);
     if (h_slot_pages) cudaFreeHost(h_slot_pages);
+    if (h_beam_desc) cudaFreeHost(h_beam_desc);
+    if (h_beam_init) cudaFreeHost(h_beam_init);
+    if (h_beam_pool) cudaFreeHost(h_beam_pool);
     for (int i = 1; i < kMaxMicro; ++i) { if (st_mb[i]) cudaStreamDestroy(st_mb[i]); if (ev_join[i]) cudaEventDestroy(ev_join[i]); }
     if (ev_fork) cudaEventDestroy(ev_fork);
     if (ev_vjoin) cudaEventDestroy(ev_vjoin);
@@ -944,6 +985,7 @@ SampleState Engine::sample_state() const {
     s.tokens = d_tokens.p; s.sampled = d_sampled.p; s.forced = use_forced ? d_forced.p : nullptr;
     s.seen = d_seen.p; s.temperature = d_temp.p; s.top_p = d_top_p.p; s.top_k = d_top_k.p; s.penalty = d_pen.p;
     s.max_tokens = d_max_tokens.p; s.stop_token = d_stop.p; s.seed = d_seed.p; s.seq_seed = d_seq_seed.p;
+    s.beam = d_beam_flag.p;
     s.tokens_cap = CAP; s.seen_words = SEENW;
     return s;
 }
@@ -1027,22 +1069,32 @@ void Engine::head_and_sample(int M, const int* row_index, const int* slots_dev, 
 // Slot state of an admission wave: KV pages are taken here, everything the device needs goes up in one staged copy and
 // one kernel (launch_init_slots).  `forced` (debug entry points, one sequence): teacher-forced token ids.
 void Engine::init_slots(const std::vector<Sequence*>& seqs, const int32_t* forced, int n_forced) {
-    const int n = (int)seqs.size();
-    if (n == 0) return;
+    if (seqs.empty()) return;
+    int n = 0;
+    for (auto* sq : seqs) n += std::max(1, (int)sq->beam_slots.size());
     if (n > NSLOT) throw std::runtime_error("init_slots: wave larger than the slot count");
-    for (int i = 0; i < n; ++i) {
+    std::vector<std::pair<Sequence*, int>> groups;      // beam groups of the wave and their prompt pages
+    for (int i = 0, r = 0; i < (int)seqs.size(); ++i) {
         Sequence& s = *seqs[i];
         s.n_prompt = cfg.n_cond_latents + (int)s.text_ids.size() + 1;
         s.max_tok = std::min<int>(s.sp.max_tokens > 0 ? s.sp.max_tokens : CAP, CAP);
         const int need_pages = ceil_div(s.n_prompt + s.max_tok, kPageTokens);
-        if ((int)free_pages.size() < need_pages) throw std::runtime_error("out of KV pages");
+        const int nb = std::max(1, (int)s.beam_slots.size());
+        // a beam group takes nb x need_pages at once: beam 0 starts with the prompt's pages, the rest form the group's pool
+        const int n_pages = nb == 1 ? need_pages : ceil_div(s.n_prompt, kPageTokens);
+        if ((int)free_pages.size() < nb * need_pages) throw std::runtime_error("out of KV pages");
         s.pages.clear();
-        int* pg = h_slot_pages + (size_t)i * max_pages;
-        for (int k = 0; k < need_pages; ++k) { pg[k] = free_pages.back(); free_pages.pop_back(); s.pages.push_back(pg[k]); }
-        SlotInit& d = h_slot_init[i];
-        d.slot = s.slot; d.ctx_len = s.n_prompt; d.top_k = s.sp.top_k; d.max_tokens = s.max_tok; d.stop_token = s.sp.stop_token;
-        d.seq_seed = s.sp.seq_seed; d.start_token = cfg.start_audio_token; d.n_pages = need_pages;
-        d.temperature = s.sp.temperature; d.top_p = s.sp.top_p; d.penalty = s.sp.repetition_penalty; d.seed = s.sp.seed;
+        for (int k = 0; k < nb * need_pages; ++k) { s.pages.push_back(free_pages.back()); free_pages.pop_back(); }
+        if (nb > 1) groups.emplace_back(&s, n_pages);
+        for (int b = 0; b < nb; ++b, ++r) {
+            int* pg = h_slot_pages + (size_t)r * max_pages;
+            SlotInit& d = h_slot_init[r];
+            d.slot = nb == 1 ? s.slot : s.beam_slots[b]; d.ctx_len = s.n_prompt; d.top_k = s.sp.top_k; d.max_tokens = s.max_tok;
+            d.stop_token = s.sp.stop_token; d.seq_seed = s.sp.seq_seed; d.start_token = cfg.start_audio_token;
+            d.n_pages = b == 0 ? n_pages : 0; d.beam = nb > 1;
+            for (int k = 0; k < d.n_pages; ++k) pg[k] = s.pages[k];
+            d.temperature = s.sp.temperature; d.top_p = s.sp.top_p; d.penalty = s.sp.repetition_penalty; d.seed = s.sp.seed;
+        }
     }
     d_slot_init.upload(h_slot_init, n, st);
     d_slot_pages.upload(h_slot_pages, (size_t)n * max_pages, st);
@@ -1050,8 +1102,23 @@ void Engine::init_slots(const std::vector<Sequence*>& seqs, const int32_t* force
     a.last_tok = d_last_tok.p; a.n_gen = d_n_gen.p; a.ctx_len = d_ctx_len.p; a.finished = d_finished.p; a.seen = d_seen.p;
     a.temperature = d_temp.p; a.top_p = d_top_p.p; a.top_k = d_top_k.p; a.penalty = d_pen.p; a.max_tokens = d_max_tokens.p;
     a.stop_token = d_stop.p; a.seed = d_seed.p; a.seq_seed = d_seq_seed.p; a.block_tables = d_block_tables.p;
+    a.beam = d_beam_flag.p;
     a.seen_words = SEENW; a.max_pages = max_pages;
     launch_init_slots(d_slot_init.p, d_slot_pages.p, n, a, st);
+    for (size_t gi = 0; gi < groups.size(); ++gi) {
+        // group state as transformers initialises it: no finished hypothesis (-1e9), heuristic unsatisfied
+        Sequence& s = *groups[gi].first;
+        BeamState& bs = h_beam_init[gi];
+        bs = BeamState{};
+        for (int j = 0; j < kMaxBeams; ++j) bs.fin_score[j] = -1e9f;
+        bs.heur_unsat = 1;
+        bs.n_pages[0] = groups[gi].second;
+        bs.n_free = (int)s.pages.size() - groups[gi].second;
+        int* pool = h_beam_pool + gi * beam_pool_cap;
+        std::copy(s.pages.begin() + groups[gi].second, s.pages.end(), pool);
+        d_beam_state.upload(&bs, 1, st, (size_t)s.slot);
+        d_beam_pool.upload(pool, bs.n_free, st, (size_t)s.slot * beam_pool_cap);
+    }
     if (forced) {
         std::vector<int> f(CAP, -1);
         for (int i = 0; i < std::min(n_forced, CAP); ++i) f[i] = forced[i];
@@ -1068,8 +1135,32 @@ void Engine::release_pages(Sequence& s) {
 
 void Engine::release_slot(Sequence& s) {
     release_pages(s);
+    for (size_t b = 1; b < s.beam_slots.size(); ++b) free_slots.push_back(s.beam_slots[b]);
+    if (s.beam_slots.size() > 1) s.beam_slots.resize(1);
     if (s.slot >= 0 && s.slot < B) free_slots.push_back(s.slot);
     s.slot = -1;
+}
+
+// The beam kernels of one step for `groups` (running beam groups), after the prefill (first: every beam reads the
+// group's prefill row rows0[g]) or after a decode step (beam j reads the row of its slot in d_active)
+void Engine::beam_step(const std::vector<Sequence*>& groups, const std::vector<int>& rows0, bool first) {
+    if (groups.empty()) return;
+    for (size_t g = 0; g < groups.size(); ++g) {
+        const Sequence& s = *groups[g];
+        BeamDesc& d = h_beam_desc[g];
+        d.primary = s.slot; d.nb = (int)s.beam_slots.size(); d.first = first; d.advance = first ? 0 : 1;
+        d.do_sample = s.beam.do_sample != 0; d.length_penalty = s.beam.length_penalty;
+        for (int j = 0; j < kMaxBeams; ++j) {
+            d.slot[j] = j < d.nb ? s.beam_slots[j] : -1;
+            d.row[j] = j < d.nb ? (first ? rows0[g] : rows0[g] + j) : 0;
+        }
+    }
+    d_beam_desc.upload(h_beam_desc, groups.size(), st);
+    BeamArgs a{};
+    a.desc = d_beam_desc.p; a.n_groups = (int)groups.size(); a.state = d_beam_state.p; a.hist = d_beam_hist.p;
+    a.pool = d_beam_pool.p; a.pool_cap = beam_pool_cap; a.scores = d_beam_scores.p; a.block_tables = d_block_tables.p;
+    a.max_pages = max_pages; a.latents = d_latents.p; a.H = H;
+    launch_beam_step(wLOG.p, Vpad, V, sample_state(), a, d_kv_ptrs.p, d_kv_ptrs.p + L, L, NH, bf16 ? 2 : 4, st);
 }
 
 // builds row descriptors for [prompt ; optional forced audio rows] of each sequence; returns total rows
@@ -1587,8 +1678,19 @@ void Engine::dev_put(float* p, size_t cap) { std::lock_guard<std::mutex> lk(pin_
 
 void Engine::pinned_put(float* p, size_t cap) { std::lock_guard<std::mutex> lk(pin_mu); pinned_pool.emplace_back(p, cap); }
 
-void Engine::submit(uint64_t id, const int32_t* text, int n_text, int speaker, const xtts_sampling& sp, float speed) {
+void Engine::submit(uint64_t id, const int32_t* text, int n_text, int speaker, const xtts_sampling& sp, float speed,
+                    const xtts_beam* beam) {
     if (!(speed >= 0.25f && speed <= 4.0f)) throw std::runtime_error("speed out of range (0.25..4)");   // NaN included
+    if (beam) {
+        if (beam->num_beams < 1 || beam->num_beams > kMaxBeams || beam->num_beams > B)
+            throw std::runtime_error("num_beams out of range (1..8, <= max_batch)");
+        if (beam->num_beams > 1 && sp.early_tokens != 0) throw std::runtime_error("a beam-search chunk cannot stream (early_tokens must be 0)");
+        if (beam->num_beams > 1 && !std::isfinite(beam->length_penalty)) throw std::runtime_error("length_penalty must be finite");
+        if (beam->num_beams > 1 && beam->do_sample && !(sp.temperature > 0.f))
+            throw std::runtime_error("beam sampling needs a temperature > 0 (transformers rejects it too)");
+        if (beam->num_beams > 1 && !beam_supported(V, max_pages, CAP))
+            throw std::runtime_error("beam search: this engine's geometry exceeds the beam kernels' limits");
+    }
     if (n_text <= 0 || n_text > cfg.max_text_tokens + 2) throw std::runtime_error("n_text out of range (1..max_text_tokens+2)");
     if (speaker < 0 || speaker >= S) throw std::runtime_error("speaker slot out of range");
     // ids are checked here so that a bad id fails this call alone, not the batched step it would have joined
@@ -1596,6 +1698,7 @@ void Engine::submit(uint64_t id, const int32_t* text, int n_text, int speaker, c
         if (text[i] < 0 || text[i] >= cfg.n_text_tokens) throw std::runtime_error("text token id out of range");
     std::shared_ptr<Sequence> s(new Sequence());
     s->id = id; s->text_ids.assign(text, text + n_text); s->speaker = speaker; s->sp = sp; s->speed = speed; s->t_submit = now_s();
+    if (beam && beam->num_beams > 1) s->beam = *beam;
     require_finalized();
     if (!spk_valid[speaker]) throw std::runtime_error("speaker slot not set");
     {
@@ -1654,6 +1757,9 @@ void Engine::fail_unadmitted(std::shared_ptr<Sequence> s, int code, const char* 
 // the slot — whose latent ring and token row the remaining vocoder work reads — when the final job has completed.
 void Engine::on_finished(std::shared_ptr<Sequence> s, int n_tokens, int fail_status) {
     release_pages(*s);
+    // a beam group: the hypothesis is in the primary slot now (beam_gather_kernel); the other slots go back
+    for (size_t b = 1; b < s->beam_slots.size(); ++b) free_slots.push_back(s->beam_slots[b]);
+    if (s->beam_slots.size() > 1) s->beam_slots.resize(1);
     s->n_tokens = std::max(0, std::min(n_tokens, CAP));
     st_tokens += s->n_tokens;
     VocJob j;
@@ -1914,9 +2020,16 @@ void Engine::loop() {
                 auto s = waiting.front();
                 const int p = cfg.n_cond_latents + (int)s->text_ids.size() + 1;
                 if (!fresh.empty() && rows + p > prefill_rows_cap) break;
+                // a beam group takes its num_beams slots at once (only beam 0's prompt is prefilled); one that does not
+                // fit stops the wave, as the row budget does
+                if ((int)free_slots.size() < s->beam.num_beams) break;
                 waiting.pop_front();                          // (KV pages cannot run out: the pool holds max_pages per slot)
                 if (!spk_valid[s->speaker]) { fail_unadmitted(s, XTTS_ERR_STATE, "speaker slot not set"); continue; }
                 s->slot = free_slots.back(); free_slots.pop_back();
+                if (s->beam.num_beams > 1) {
+                    s->beam_slots.assign(1, s->slot);
+                    for (int b = 1; b < s->beam.num_beams; ++b) { s->beam_slots.push_back(free_slots.back()); free_slots.pop_back(); }
+                }
                 rows += p;
                 fresh.push_back(s.get()); fresh_sp.push_back(s);
             }
@@ -1927,11 +2040,18 @@ void Engine::loop() {
                 for (auto& s : fresh_sp) {
                     // vocoder windows: the first cut after early_tokens (streaming chunks) or voc_segment tokens, then every
                     // voc_segment; 0 = the chunk is vocoded whole when it ends
-                    s->stream_pieces = s->sp.early_tokens > 0 && s->sp.vocode;
-                    s->seg_next = s->sp.vocode ? voc_segment : 0;
+                    // (a beam chunk's hypothesis is known only when its group ends: no windows, no pieces)
+                    const bool beams = s->beam.num_beams > 1;
+                    s->stream_pieces = s->sp.early_tokens > 0 && s->sp.vocode && !beams;
+                    s->seg_next = s->sp.vocode && !beams ? voc_segment : 0;
                     s->next_boundary = s->stream_pieces ? s->sp.early_tokens : s->seg_next;
                 }
                 prefill(fresh);
+                std::vector<Sequence*> groups;
+                std::vector<int> rows0;
+                for (size_t i = 0; i < fresh.size(); ++i)
+                    if (fresh[i]->beam.num_beams > 1) { groups.push_back(fresh[i]); rows0.push_back((int)i); }
+                beam_step(groups, rows0, true);
                 for (auto& s : fresh_sp) running.push_back(s);
                 fresh_sp.clear();
                 // a sequence may already be finished after its first token (max_tokens == 1 / instant stop)
@@ -1941,12 +2061,21 @@ void Engine::loop() {
             }
             if (!running.empty()) {
                 std::vector<int> active;
+                std::vector<Sequence*> groups;
+                std::vector<int> rows0;
                 double ctx_sum = 0;
-                for (auto& s : running) if (!h_finished[s->slot]) { active.push_back(s->slot); ctx_sum += s->n_prompt + s->steps + 1; ++s->steps; }
+                for (auto& s : running) {
+                    if (h_finished[s->slot]) continue;
+                    if (s->beam.num_beams > 1) { groups.push_back(s.get()); rows0.push_back((int)active.size()); }
+                    const int nb = std::max(1, (int)s->beam_slots.size());
+                    for (int b = 0; b < nb; ++b) { active.push_back(nb == 1 ? s->slot : s->beam_slots[b]); ctx_sum += s->n_prompt + s->steps + 1; }
+                    ++s->steps;
+                }
                 if (!active.empty()) {
                     gpt_work = true;
                     decode_ctx_sum = ctx_sum;
                     decode_step(active);
+                    beam_step(groups, rows0, false);     // eager on st, ahead of the read-back: no extra host sync
                     d_finished.download(h_finished, NSLOT, st);
                     d_n_gen.download(h_finished + NSLOT, NSLOT, st);
                     CUDA_CHECK(cudaStreamSynchronize(st));
@@ -2435,7 +2564,7 @@ void Engine::debug_sample_slots(int Vn, int M, const int32_t* active, int n_slot
     S.last_tok = dlast.p; S.n_gen = dng.p; S.ctx_len = dctx.p; S.finished = dfin.p;
     S.tokens = dtok.p; S.sampled = dsmp.p; S.forced = forced ? dfor.p : nullptr;
     S.seen = dseen.p; S.temperature = dT.p; S.top_p = dtp.p; S.top_k = dtk.p; S.penalty = dpen.p;
-    S.max_tokens = dmt.p; S.stop_token = dstp.p; S.seed = dseed.p; S.seq_seed = dss.p;
+    S.max_tokens = dmt.p; S.stop_token = dstp.p; S.seed = dseed.p; S.seq_seed = dss.p; S.beam = nullptr;
     S.tokens_cap = cap; S.seen_words = sw;
     launch_sample(dlg.p, ld, dact.p, M, Vn, S, advance_ctx, st);
     dng.download(n_gen, n_slots, st); dctx.download(ctx_len, n_slots, st); dfin.download(finished, n_slots, st);
@@ -2503,6 +2632,92 @@ void Engine::debug_attn_decode(int kv_type, int heads, int M, const int32_t* act
         CUDA_CHECK(cudaStreamSynchronize(st));
         widen16(o, kv_type == 2, out);
     }
+}
+
+// One beam step on caller arrays for one group of nb beams in slots 0..nb-1: logprob, select, reorder and the partial-page
+// copy (launch_beam_step without the gather), every input and output on the host (include/xtts_b200.h)
+void Engine::debug_beam_step(int kv_type, int heads, int layers, int Vn, const xtts_sampling& sp, const xtts_beam& bm, int first,
+                             int advance, const float* logits, int32_t* n_gen, int32_t* ctx_len, int32_t* last_tok,
+                             uint32_t* seen, int mp, int32_t* block_tables, int n_pages, int32_t* pool, int cap, int32_t* hist,
+                             xtts_beam_state* state, void* kpool, void* vpool, float* scores) {
+    static_assert(sizeof(xtts_beam_state) == sizeof(BeamState), "xtts_beam_state mirrors BeamState");
+    ApiLock lk(this);
+    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
+    const int nb = bm.num_beams;
+    auto bad = [](const char* m) { throw std::runtime_error(std::string("debug_beam_step: ") + m); };
+    if (kv_type < 0 || kv_type > 2) bad("kv_type 0 (fp32), 1 (bf16) or 2 (fp16)");
+    if (nb < 2 || nb > kMaxBeams) bad("num_beams 2..8");
+    if (heads < 1 || layers < 1 || Vn < 2 * nb || n_pages < 1 || cap < 1 || mp < 1) bad("empty problem");
+    if (!beam_supported(Vn, mp, cap)) bad("geometry outside the beam kernels' limits");
+    const int W = ceil_div(Vn, 32), pool_cap = nb * mp;
+    BeamState bs;
+    std::memcpy(&bs, state, sizeof(bs));
+    if (bs.n_free < nb || bs.n_free > pool_cap) bad("the pool must hold nb .. nb * max_pages pages");
+    for (int i = 0; i < bs.n_free; ++i) if (pool[i] < 0 || pool[i] >= n_pages) bad("pool page outside the pool");
+    // every beam that owns pages holds exactly those of its KV positions [0, L), L = ctx_len + advance; the pool and the
+    // tables together never exceed nb * max_pages entries
+    const int L = ctx_len[0] + advance;
+    if (L < 1 || L / kPageTokens >= mp) bad("the next position must lie inside the block table");
+    int held = 0;
+    for (int j = 0; j < nb; ++j) {
+        if (n_gen[j] != n_gen[0] || ctx_len[j] != ctx_len[0]) bad("the beams of a group share n_gen and ctx_len");
+        const int np = first && j > 0 ? 0 : bs.n_pages[j];
+        if (np != (first && j > 0 ? 0 : ceil_div(L, kPageTokens))) bad("n_pages must cover the KV positions [0, ctx_len + advance)");
+        for (int k = 0; k < np; ++k)
+            if (block_tables[(size_t)j * mp + k] < 0 || block_tables[(size_t)j * mp + k] >= n_pages) bad("page id outside the pool");
+        held += np;
+    }
+    if (held + bs.n_free > pool_cap) bad("pool and tables exceed nb * max_pages pages");
+    if (n_gen[0] < 0 || n_gen[0] >= cap) bad("n_gen outside the history");
+    CUDA_CHECK(cudaSetDevice(cfg.device));
+    const size_t esz = kv_type == 0 ? 4 : 2;
+    const size_t page_bytes = (size_t)heads * kPageTokens * kHeadDim * esz, pool_bytes = (size_t)layers * n_pages * page_bytes;
+    DBuf<int> dng, dctx, dlast, dfin, dtok, dtk, dmt, dstop, dss, dbt, dpool;
+    DBuf<float> dT, dtp, dpen, dlog, dsc;
+    DBuf<unsigned long long> dseed;
+    DBuf<unsigned> dseen;
+    DBuf<BeamState> dstate;
+    DBuf<BeamDesc> ddesc;
+    DBuf<int2> dhist;
+    DBuf<uint8_t> dk, dv;
+    DBuf<void*> dptr;
+    dng.alloc(nb); dctx.alloc(nb); dlast.alloc(nb); dfin.alloc(nb); dtok.alloc((size_t)nb * cap); dtk.alloc(nb); dmt.alloc(nb);
+    dstop.alloc(nb); dss.alloc(nb); dbt.alloc((size_t)nb * mp); dpool.alloc(pool_cap); dT.alloc(nb); dtp.alloc(nb); dpen.alloc(nb);
+    dlog.alloc((size_t)nb * Vn); dsc.alloc((size_t)nb * Vn); dseed.alloc(nb); dseen.alloc((size_t)nb * W); dstate.alloc(1);
+    ddesc.alloc(1); dhist.alloc((size_t)cap * kMaxBeams); dk.alloc(pool_bytes); dv.alloc(pool_bytes); dptr.alloc(2 * layers);
+    std::vector<int> v_tk(nb, sp.top_k), v_mt(nb, sp.max_tokens), v_stop(nb, sp.stop_token), v_ss(nb, sp.seq_seed);
+    std::vector<float> v_T(nb, sp.temperature), v_tp(nb, sp.top_p), v_pen(nb, sp.repetition_penalty);
+    std::vector<unsigned long long> v_seed(nb, sp.seed);
+    std::vector<void*> ptr(2 * layers);
+    for (int l = 0; l < layers; ++l) { ptr[l] = dk.p + l * n_pages * page_bytes; ptr[layers + l] = dv.p + l * n_pages * page_bytes; }
+    BeamDesc d{};
+    d.primary = 0; d.nb = nb; d.first = first != 0; d.advance = advance; d.do_sample = bm.do_sample != 0;
+    d.length_penalty = bm.length_penalty;
+    for (int j = 0; j < kMaxBeams; ++j) { d.slot[j] = j < nb ? j : -1; d.row[j] = j < nb ? (first ? 0 : j) : 0; }
+    dng.upload(n_gen, nb, st); dctx.upload(ctx_len, nb, st); dfin.zero(st); dtok.zero(st);
+    dtk.upload(v_tk.data(), nb, st); dmt.upload(v_mt.data(), nb, st); dstop.upload(v_stop.data(), nb, st); dss.upload(v_ss.data(), nb, st);
+    dT.upload(v_T.data(), nb, st); dtp.upload(v_tp.data(), nb, st); dpen.upload(v_pen.data(), nb, st); dseed.upload(v_seed.data(), nb, st);
+    dseen.upload(seen, (size_t)nb * W, st); dbt.upload(block_tables, (size_t)nb * mp, st); dpool.upload(pool, pool_cap, st);
+    dlog.upload(logits, (size_t)(first ? 1 : nb) * Vn, st); dstate.upload(&bs, 1, st); ddesc.upload(&d, 1, st);
+    dhist.upload(reinterpret_cast<const int2*>(hist), (size_t)cap * kMaxBeams, st);
+    dk.upload(static_cast<const uint8_t*>(kpool), pool_bytes, st); dv.upload(static_cast<const uint8_t*>(vpool), pool_bytes, st);
+    dptr.upload(ptr.data(), 2 * layers, st);
+    SampleState S{};
+    S.last_tok = dlast.p; S.n_gen = dng.p; S.ctx_len = dctx.p; S.finished = dfin.p; S.tokens = dtok.p; S.sampled = nullptr;
+    S.forced = nullptr; S.seen = dseen.p; S.temperature = dT.p; S.top_p = dtp.p; S.top_k = dtk.p; S.penalty = dpen.p;
+    S.max_tokens = dmt.p; S.stop_token = dstop.p; S.seed = dseed.p; S.seq_seed = dss.p; S.beam = nullptr;
+    S.tokens_cap = cap; S.seen_words = W;
+    BeamArgs a{};
+    a.desc = ddesc.p; a.n_groups = 1; a.state = dstate.p; a.hist = dhist.p; a.pool = dpool.p; a.pool_cap = pool_cap;
+    a.scores = dsc.p; a.block_tables = dbt.p; a.max_pages = mp; a.latents = nullptr; a.H = 0;
+    launch_beam_step(dlog.p, Vn, Vn, S, a, dptr.p, dptr.p + layers, layers, heads, (int)esz, st, false);
+    dng.download(n_gen, nb, st); dctx.download(ctx_len, nb, st); dlast.download(last_tok, nb, st);
+    dseen.download(seen, (size_t)nb * W, st); dbt.download(block_tables, (size_t)nb * mp, st); dpool.download(pool, pool_cap, st);
+    dstate.download(&bs, 1, st); dhist.download(reinterpret_cast<int2*>(hist), (size_t)cap * kMaxBeams, st);
+    dk.download(static_cast<uint8_t*>(kpool), pool_bytes, st); dv.download(static_cast<uint8_t*>(vpool), pool_bytes, st);
+    dsc.download(scores, (size_t)nb * Vn, st);
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    std::memcpy(state, &bs, sizeof(bs));
 }
 
 // One launch of the prefill / encoder attention (launch_attn_generic).  q rows and k / v rows are addressed with the given
@@ -2976,6 +3191,21 @@ int xtts_submit(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, int32_
 int xtts_submit_speed(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
                       const xtts_sampling* sp, float speed) {
     XTTS_TRY(e->impl->submit(seq_id, text_ids, n_text, speaker_slot, *sp, speed))
+}
+int xtts_submit_beams(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
+                      const xtts_sampling* sp, float speed, const xtts_beam* beam) {
+    if (!sp || !beam) { xtts::set_error("null argument"); return XTTS_ERR_INVALID; }
+    XTTS_TRY(e->impl->submit(seq_id, text_ids, n_text, speaker_slot, *sp, speed, beam))
+}
+int xtts_debug_beam_step(xtts_engine* e, int32_t kv_type, int32_t heads, int32_t layers, int32_t V, const xtts_sampling* sp,
+                         const xtts_beam* beam, int32_t first, int32_t advance, const float* logits, int32_t* n_gen,
+                         int32_t* ctx_len, int32_t* last_tok, uint32_t* seen, int32_t max_pages, int32_t* block_tables,
+                         int32_t n_pages, int32_t* pool, int32_t cap, int32_t* hist, xtts_beam_state* state, void* kpool,
+                         void* vpool, float* scores) {
+    if (!sp || !beam || !logits || !n_gen || !ctx_len || !last_tok || !seen || !block_tables || !pool || !hist || !state ||
+        !kpool || !vpool || !scores) { xtts::set_error("null argument"); return XTTS_ERR_INVALID; }
+    XTTS_TRY(e->impl->debug_beam_step(kv_type, heads, layers, V, *sp, *beam, first, advance, logits, n_gen, ctx_len, last_tok,
+                                      seen, max_pages, block_tables, n_pages, pool, cap, hist, state, kpool, vpool, scores))
 }
 int xtts_cancel(xtts_engine* e, uint64_t seq_id) { XTTS_TRY(e->impl->cancel(seq_id)) }
 int xtts_poll(xtts_engine* e, xtts_result* out, int32_t timeout_ms) {

@@ -68,6 +68,7 @@ init_slots_kernel(const SlotInit* __restrict__ init, const int* __restrict__ pag
         a.last_tok[slot] = d.start_token; a.n_gen[slot] = 0; a.ctx_len[slot] = d.ctx_len; a.finished[slot] = 0;
         a.temperature[slot] = d.temperature; a.top_p[slot] = d.top_p; a.top_k[slot] = d.top_k; a.penalty[slot] = d.penalty;
         a.max_tokens[slot] = d.max_tokens; a.stop_token[slot] = d.stop_token; a.seed[slot] = d.seed; a.seq_seed[slot] = d.seq_seed;
+        a.beam[slot] = d.beam;
     }
     // penalty set seed: the prompt ids are [1]*(32+Lt)+[start]  (vllm_mm_gpt.py:325, App. B.7)
     for (int w = threadIdx.x; w < a.seen_words; w += blockDim.x) {
@@ -787,20 +788,6 @@ attn_generic_kernel(AttnLayout L, const AttnSeq* __restrict__ seqs, TOut* __rest
 // ------------------------------------------------------------------------------------------------
 constexpr int SV = 2048;
 
-__device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0,
-                                              uint32_t k1, uint32_t out[4]) {
-    const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u, W0 = 0x9E3779B9u, W1 = 0xBB67AE85u;
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        const uint32_t hi0 = __umulhi(M0, c0), lo0 = M0 * c0;
-        const uint32_t hi1 = __umulhi(M1, c2), lo1 = M1 * c2;
-        const uint32_t n0 = hi1 ^ c1 ^ k0, n1 = lo1, n2 = hi0 ^ c3 ^ k1, n3 = lo0;
-        c0 = n0; c1 = n1; c2 = n2; c3 = n3;
-        k0 += W0; k1 += W1;
-    }
-    out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
-}
-
 struct KeyIdx { float v; int i; };
 __device__ __forceinline__ bool key_less(const KeyIdx& a, const KeyIdx& b) {
     return (a.v < b.v) || (a.v == b.v && a.i < b.i);
@@ -818,6 +805,7 @@ sample_kernel(const float* __restrict__ logits, int ld, const int* __restrict__ 
     trace_pt(TR_SAMPLE, 0); pdl_trigger(); pdl_wait(); trace_pt(TR_SAMPLE, 1);
     const int tid = threadIdx.x;
     const int slot = active[blockIdx.x];
+    if (S.beam && S.beam[slot]) return;                 // a beam: the beam kernels choose its token (beam.cu)
     const int n = S.n_gen[slot];
     const float* z = logits + (size_t)blockIdx.x * ld;
     const float pen = S.penalty[slot];

@@ -140,10 +140,58 @@ struct SampleState {      // per-slot arrays (device)
     unsigned* seen;       // [slot][seen_words] bitmap of ids in prompt ∪ generated
     const float* temperature; const float* top_p; const int* top_k; const float* penalty;
     const int* max_tokens; const int* stop_token; const unsigned long long* seed; const int* seq_seed;
+    const int* beam;      // [slot] != 0: the slot is a beam of a beam-search group, chosen by the beam kernels (or nullptr)
     int tokens_cap, seen_words;
 };
 void launch_sample(const float* logits, int ld_logits, const int* active, int M, int V, SampleState s,
                    int advance_ctx, cudaStream_t st, bool pdl = false);
+
+// ------------------------------------------------------------------------------------------
+// beam search (beam.cu): transformers 5.5 `_beam_search` for one batch item per group, num_return_sequences 1,
+// early_stopping unset.  A group of nb <= 8 beams lives in nb slots; beam j is slot[j] for the group's whole life.
+// ------------------------------------------------------------------------------------------
+constexpr int kMaxBeams = 8;
+struct BeamDesc {         // one running group, uploaded every step
+    int primary;          // slot of beam 0: indexes the group's persistent state
+    int nb;
+    int slot[kMaxBeams];
+    int row[kMaxBeams];   // logits row of each beam this step (all = the prefill row on the first step)
+    int first;            // first selection: B copies of the prefill logits, running scores [0, -1e9, ...]
+    int advance;          // KV positions appended by the step just run (0 after the prefill, 1 after a decode step)
+    int do_sample;
+    float length_penalty;
+};
+struct BeamState {        // persistent per group, indexed by the primary slot
+    float run_score[kMaxBeams];
+    float fin_score[kMaxBeams];
+    int fin_valid[kMaxBeams];                    // is_sent_finished
+    int fin_step[kMaxBeams], fin_beam[kMaxBeams], fin_tok[kMaxBeams];
+    int heur_unsat;                              // is_early_stop_heuristic_unsatisfied
+    int done;
+    int sel_parent[kMaxBeams], sel_tok[kMaxBeams];   // this step's running beams: parent beam, token
+    int n_copy;                                  // partial pages to copy this step
+    int copy_src[kMaxBeams], copy_dst[kMaxBeams], copy_ntok[kMaxBeams];
+    int n_free;                                  // pages in the group's free list
+    int n_pages[kMaxBeams];                      // table entries of each beam
+};
+struct BeamArgs {
+    const BeamDesc* desc; int n_groups;
+    BeamState* state;     // [NSLOT]
+    int2* hist;           // [NSLOT][tokens_cap][kMaxBeams]: (parent beam, token) of each running beam, per step
+    int* pool;            // [NSLOT][pool_cap] free pages of each group
+    int pool_cap;
+    float* scores;        // [NSLOT][ld] processed, accumulated scores of each beam slot
+    int* block_tables; int max_pages;
+    float* latents; int H;                       // latent ring [NSLOT][tokens_cap][H]
+};
+// logprob -> select -> reorder (block tables, slot state) -> partial-page copy -> gather of finished groups (`gather`)
+// kpool / vpool: device arrays of the `layers` per-layer pool base pointers; elem = bytes per KV element
+void launch_beam_step(const float* logits, int ld_logits, int V, SampleState s, BeamArgs a, void* const* kpool,
+                      void* const* vpool, int layers, int heads, int elem, cudaStream_t st, bool gather = true);
+// the geometry the beam kernels take: V <= 2048, <= 128 KV pages per sequence, the gather's token list in shared memory
+bool beam_supported(int V, int max_pages, int tokens_cap);
+// per device (the current one): the beam kernels' dynamic shared memory limits
+void beam_init_device();
 
 // ------------------------------------------------------------------------------------------
 // Vocoder kernels (fp32, channel-major activations [C][L])
@@ -213,13 +261,14 @@ void launch_conv_post(const float* x, const float* w, float* wav, int Cin, int L
 // dozen small copies per sequence).
 struct SlotInit {
     int slot, ctx_len, top_k, max_tokens, stop_token, seq_seed, start_token, n_pages;
+    int beam;             // the slot is a beam of a beam-search group (SampleState::beam)
     float temperature, top_p, penalty;
     unsigned long long seed;
 };
 struct SlotArrays {       // per-slot device arrays (mutable view of SampleState + block tables)
     int* last_tok; int* n_gen; int* ctx_len; int* finished; unsigned* seen;
     float* temperature; float* top_p; int* top_k; float* penalty; int* max_tokens; int* stop_token;
-    unsigned long long* seed; int* seq_seed; int* block_tables;
+    unsigned long long* seed; int* seq_seed; int* block_tables; int* beam;
     int seen_words, max_pages;
 };
 // pages: [n][max_pages] page ids of each sequence (first n_pages valid)

@@ -359,13 +359,20 @@ class XTTSv2Engine(BaseAsyncTTSEngine):
         token_lists = self.prepare_text_tokens(request.text, request.language)
         generators, request_ids = [], []
         base_seed = request.seed if getattr(request, "seed", None) is not None else int.from_bytes(hashlib.sha256(request.request_id.encode()).digest()[:6], "little")
+        num_beams = getattr(request, "num_beams", 1)
+        if num_beams > 1 and num_beams > self.max_concurrency:
+            raise ValueError(f"num_beams {num_beams} exceeds the engine's {self.max_concurrency} batch slots")
         for seq_index, ids in enumerate(token_lists):
+            # a beam chunk (num_beams > 1) is delivered whole: its best hypothesis is known only when its group ends
+            stream_first = request.stream and seq_index == 0 and num_beams == 1
             sp = native.Sampling(temperature=request.temperature, top_p=request.top_p, top_k=request.top_k,
                                  repetition_penalty=request.repetition_penalty,
                                  max_tokens=self.dims.gpt.max_audio_tokens, stop_token=self.mel_eos_token_id,
                                  seed=base_seed, seq_seed=seq_index, vocode=True, priority=seq_index,
-                                 early_tokens=self.early_emit_tokens if (request.stream and seq_index == 0) else 0,
-                                 speed=getattr(request, "speed", 1.0))     # (the reference's own TTSRequest has none)
+                                 early_tokens=self.early_emit_tokens if stream_first else 0,
+                                 speed=getattr(request, "speed", 1.0),     # (the reference's own TTSRequest has none)
+                                 num_beams=num_beams, length_penalty=getattr(request, "length_penalty", 1.0),
+                                 do_sample=getattr(request, "do_sample", True))
             rid = f"{request.request_id}_{seq_index}"
             generators.append(self._chunk_generator(rid, ids, gpt_cond_latent, speaker_embeddings, sp))
             request_ids.append(rid)
@@ -379,7 +386,7 @@ class XTTSv2Engine(BaseAsyncTTSEngine):
         box: asyncio.Queue = asyncio.Queue()            # completions of this chunk: partial pieces, then the final one
         natives = getattr(self, "natives", None) or [self.native]
         spks = getattr(self, "_spks", None) or [self._spk]
-        work = len(ids)
+        work = len(ids) * max(1, getattr(sp, "num_beams", 1))     # a beam group decodes num_beams rows per step
         with self._wlock:                               # data parallelism: the GPU with the least work in flight takes it
             load = getattr(self, "_load", None)
             if load is None:

@@ -51,6 +51,18 @@ class XttsConfig(C.Structure):
     ]
 
 
+class XttsBeam(C.Structure):
+    _fields_ = [("num_beams", C.c_int32), ("length_penalty", C.c_float), ("do_sample", C.c_int32)]
+
+
+class XttsBeamState(C.Structure):
+    _fields_ = [("run_score", C.c_float * 8), ("fin_score", C.c_float * 8), ("fin_valid", C.c_int32 * 8),
+                ("fin_step", C.c_int32 * 8), ("fin_beam", C.c_int32 * 8), ("fin_tok", C.c_int32 * 8),
+                ("heur_unsat", C.c_int32), ("done", C.c_int32), ("sel_parent", C.c_int32 * 8), ("sel_tok", C.c_int32 * 8),
+                ("n_copy", C.c_int32), ("copy_src", C.c_int32 * 8), ("copy_dst", C.c_int32 * 8), ("copy_ntok", C.c_int32 * 8),
+                ("n_free", C.c_int32), ("n_pages", C.c_int32 * 8)]
+
+
 class XttsSampling(C.Structure):
     _fields_ = [("temperature", C.c_float), ("top_p", C.c_float), ("repetition_penalty", C.c_float),
                 ("top_k", C.c_int32), ("max_tokens", C.c_int32), ("stop_token", C.c_int32),
@@ -110,7 +122,7 @@ class XttsKernelProfile(C.Structure):
 # every symbol include/xtts_b200.h declares (checked by tests/test_abi.py against the header text)
 ABI_SYMBOLS = [
     "xtts_last_error", "xtts_version", "xtts_create", "xtts_destroy", "xtts_load_weight", "xtts_finalize_weights",
-    "xtts_set_speaker", "xtts_get_speaker", "xtts_condition", "xtts_enhance", "xtts_change_speed", "xtts_resample", "xtts_encode_flac", "xtts_decode_flac", "xtts_submit", "xtts_submit_speed", "xtts_cancel", "xtts_poll",
+    "xtts_set_speaker", "xtts_get_speaker", "xtts_condition", "xtts_enhance", "xtts_change_speed", "xtts_resample", "xtts_encode_flac", "xtts_decode_flac", "xtts_submit", "xtts_submit_speed", "xtts_submit_beams", "xtts_debug_beam_step", "xtts_cancel", "xtts_poll",
     "xtts_fetch", "xtts_set_option", "xtts_get_stats", "xtts_sync", "xtts_get_kernel_profile", "xtts_device_timer", "xtts_vocode",
     "xtts_vocode_window", "xtts_vocode_speed", "xtts_gpt_prefill", "xtts_gpt_teacher_forced",
     "xtts_debug_gemm", "xtts_debug_sample_slots", "xtts_debug_trace",
@@ -157,6 +169,7 @@ def load_library(path: Optional[str] = None):
     lib.xtts_decode_flac.argtypes = [vp, u8p, i64, i32p, i64, C.POINTER(XttsFlacInfo)]
     lib.xtts_submit.argtypes = [vp, C.c_uint64, i32p, i32, i32, C.POINTER(XttsSampling)]
     lib.xtts_submit_speed.argtypes = [vp, C.c_uint64, i32p, i32, i32, C.POINTER(XttsSampling), C.c_float]
+    lib.xtts_submit_beams.argtypes = [vp, C.c_uint64, i32p, i32, i32, C.POINTER(XttsSampling), C.c_float, C.POINTER(XttsBeam)]
     lib.xtts_cancel.argtypes = [vp, C.c_uint64]
     lib.xtts_poll.argtypes = [vp, C.POINTER(XttsResult), i32]
     lib.xtts_fetch.argtypes = [vp, C.c_uint64, i32p, f32p, f32p]
@@ -187,6 +200,9 @@ def load_library(path: Optional[str] = None):
     lib.xtts_debug_kv_write.argtypes = [vp, i32, i32, i32, f32p, i32p, i32p, i32, i32p, i32p, i32, i32, vp, vp]
     lib.xtts_debug_build_rows.argtypes = [vp, i32, i32, f32p, i32, f32p, i32, f32p, i32, f32p, i32, f32p, i32, i32p, i32, f32p]
     lib.xtts_debug_build_decode_rows.argtypes = [vp, i32, f32p, i32, f32p, i32, i32, i32p, i32, i32p, i32p, f32p, u32p, i32, i32]
+    lib.xtts_debug_beam_step.argtypes = [vp, i32, i32, i32, i32, C.POINTER(XttsSampling), C.POINTER(XttsBeam), i32, i32, f32p,
+                                         i32p, i32p, i32p, u32p, i32, i32p, i32, i32p, i32, i32p, C.POINTER(XttsBeamState),
+                                         vp, vp, f32p]
     lib.xtts_debug_cond.argtypes = [vp, i32, i32p, i32, f32p, i32, C.POINTER(f32p), C.POINTER(i64), i32, f32p, i64]
     for s in ABI_SYMBOLS:
         if s not in ("xtts_last_error", "xtts_version"):
@@ -260,6 +276,9 @@ class Sampling:
     priority: int = 0
     early_tokens: int = 0          # > 0: stream the chunk's audio as partial results, first piece after n tokens (include/xtts_b200.h)
     speed: float = 1.0             # speaking rate in [0.25, 4] (xtts_submit_speed; passed beside the struct, which cannot grow)
+    num_beams: int = 1             # > 1: beam search over this many beams (xtts_submit_beams), with the two fields below
+    length_penalty: float = 1.0
+    do_sample: bool = True
 
     def c(self) -> XttsSampling:
         s = XttsSampling()
@@ -413,8 +432,39 @@ class NativeEngine:
     def submit(self, seq_id: int, text_ids, speaker_slot: int, sp: Sampling):
         t = _i32(text_ids)
         cs = sp.c()
+        nb = int(getattr(sp, "num_beams", 1))
+        if nb > 1:
+            bm = XttsBeam(nb, float(sp.length_penalty), 1 if sp.do_sample else 0)
+            self._chk(self.lib.xtts_submit_beams(self.h, seq_id, _ip(t), t.size, speaker_slot, C.byref(cs),
+                                                 float(getattr(sp, "speed", 1.0)), C.byref(bm)), "submit")
+            return
         self._chk(self.lib.xtts_submit_speed(self.h, seq_id, _ip(t), t.size, speaker_slot, C.byref(cs),
                                              float(getattr(sp, "speed", 1.0))), "submit")
+
+    def debug_beam_step(self, kv_type: int, heads: int, layers: int, sp: Sampling, first: bool, advance: int, logits,
+                        n_gen, ctx_len, seen, block_tables, pool, hist, state: XttsBeamState, kpool, vpool):
+        """xtts_debug_beam_step: one beam step (logprob, select, reorder, partial-page copy) on caller arrays, updated in
+        place: n_gen, ctx_len int32 [nb]; seen uint32 [nb][ceil(V/32)]; block_tables int32 [nb][max_pages]; pool int32
+        [nb * max_pages]; hist int32 [cap][8][2]; state; kpool / vpool raw bytes [layers][n_pages][page].  Returns
+        (last_tok [nb], scores [nb][V])."""
+        nb = int(sp.num_beams)
+        lg = _f32(logits)
+        V = lg.shape[-1]
+        for a, dt in ((n_gen, np.int32), (ctx_len, np.int32), (seen, np.uint32), (block_tables, np.int32), (pool, np.int32),
+                      (hist, np.int32)):
+            assert a.dtype == dt and a.flags.c_contiguous
+        last = np.zeros(nb, np.int32)
+        scores = np.zeros((nb, V), np.float32)
+        page = heads * 32 * 64 * (4 if kv_type == 0 else 2)
+        n_pages = kpool.nbytes // (layers * page)
+        bm = XttsBeam(nb, float(sp.length_penalty), 1 if sp.do_sample else 0)
+        cs = sp.c()
+        self._chk(self.lib.xtts_debug_beam_step(
+            self.h, kv_type, heads, layers, V, C.byref(cs), C.byref(bm), int(first), advance, _fp(lg), _ip(n_gen), _ip(ctx_len),
+            _ip(last), seen.ctypes.data_as(C.POINTER(C.c_uint32)), block_tables.shape[1], _ip(block_tables), n_pages, _ip(pool),
+            hist.shape[0], _ip(hist), C.byref(state), kpool.ctypes.data_as(C.c_void_p), vpool.ctypes.data_as(C.c_void_p),
+            _fp(scores)), "debug_beam_step")
+        return last, scores
 
     def cancel(self, seq_id: int):
         self._chk(self.lib.xtts_cancel(self.h, seq_id), "cancel")

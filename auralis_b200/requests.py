@@ -20,6 +20,11 @@ stays; the tokens are the same at every speed.  The reference's own tool for a f
 ``TTSOutput.change_speed`` (what its OpenAI server applies), is there too and also runs on the GPU while an engine is
 alive; it stretches any audio after the fact (a combined book, a file read with ``TTSOutput.from_file``) and
 peak-normalises it.
+
+``num_beams`` (1..8, default 1) is the third addition: above 1 each text chunk is decoded by beam search on the GPU, with
+``length_penalty`` and ``do_sample`` consumed as Coqui's ``Xtts.inference`` hands them to transformers' ``generate``
+(``do_sample`` chooses beam sampling over beam search).  At one beam nothing changes and those two fields stay unused,
+as in the reference.  A beam chunk is delivered whole, also with ``stream=True``.
 """
 from __future__ import annotations
 
@@ -29,7 +34,7 @@ from dataclasses import dataclass, field
 from functools import lru_cache
 from typing import AsyncGenerator, Callable, List, Optional, Union
 
-from .config import SPEED_MAX, SPEED_MIN
+from .config import NUM_BEAMS_MAX, SPEED_MAX, SPEED_MIN
 
 SUPPORTED_LANGUAGES = ("en", "es", "fr", "de", "it", "pt", "pl", "tr", "ru", "nl", "cs", "ar", "zh-cn", "hu", "ko",
                        "ja", "hi", "auto", "")
@@ -96,13 +101,16 @@ class TTSRequest:
     top_p: float = 0.85
     top_k: int = 50
     repetition_penalty: float = 5.0
-    length_penalty: float = 1.0     # carried, not consumed by the engine (SURVEY App. A.3)
-    do_sample: bool = True          # carried, not consumed by the engine
-    # additions (not in the reference): reproducible sampling, speaking rate
+    length_penalty: float = 1.0     # consumed only by beam search (num_beams > 1), as transformers' generate does
+    do_sample: bool = True          # num_beams > 1: beam sampling (True) or beam search (False); unused at one beam
+    # additions (not in the reference): reproducible sampling, speaking rate, beam search
     seed: Optional[int] = None
     speed: float = 1.0
+    num_beams: int = 1              # 1..8; > 1 decodes each chunk by beam search (Coqui Xtts.inference(num_beams=...))
 
     def __post_init__(self):
+        if isinstance(self.num_beams, bool) or not isinstance(self.num_beams, int) or not (1 <= self.num_beams <= NUM_BEAMS_MAX):
+            raise ValueError(f"num_beams {self.num_beams!r} must be an int in [1, {NUM_BEAMS_MAX}]")
         if not (SPEED_MIN <= self.speed <= SPEED_MAX):                 # NaN fails the comparison too
             raise ValueError(f"speed {self.speed} out of range [{SPEED_MIN}, {SPEED_MAX}]")
         if self.language == "auto" and len(self.text) > 0:
@@ -122,5 +130,5 @@ class TTSRequest:
         fields = {k: getattr(self, k) for k in (
             "text", "speaker_files", "enhance_speech", "audio_config", "language", "request_id", "load_sample_rate",
             "sound_norm_refs", "max_ref_length", "gpt_cond_len", "gpt_cond_chunk_len", "stream", "temperature", "top_p",
-            "top_k", "repetition_penalty", "length_penalty", "do_sample", "seed", "speed")}
+            "top_k", "repetition_penalty", "length_penalty", "do_sample", "seed", "speed", "num_beams")}
         return TTSRequest(**fields)

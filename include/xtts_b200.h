@@ -225,6 +225,50 @@ int xtts_submit(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, int32_
  * speed; a finished chunk longer than one vocoder window is vocoded in several, none of them a partial result. */
 int xtts_submit_speed(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
                       const xtts_sampling* sp, float speed);
+/* Beam-search decoding of one chunk (Coqui Xtts.inference(num_beams, length_penalty, do_sample) -> transformers'
+ * generate): transformers 5.5 _beam_search for one batch item, num_return_sequences 1, early_stopping unset.  Each step
+ * takes log_softmax of the mel-head logits in fp32, applies the repetition penalty over the prompt ids and the beam's own
+ * hypothesis (s < 0 ? s * p : s / p) and, with do_sample, temperature, top-k and top-p (min_tokens_to_keep 2), adds the
+ * beam's running score and picks 2 num_beams candidates over num_beams x V: the top ones (ties: the lower
+ * beam * V + token), or with do_sample draws without replacement by an Exp(1) race on the sampler's Philox stream
+ * (key = seed, counter = ((beam * V + token) / 4, step, seq_seed, 0)).  Finished candidates (stop token, or max_tokens)
+ * are scored score / gen_len ^ length_penalty into the best-num_beams finished set; the group stops by transformers'
+ * default heuristic.  The result is the best finished hypothesis: its tokens (stop token included), and latents and
+ * samples exactly as xtts_submit_speed would give for those token ids.  num_beams beams take num_beams batch slots and
+ * KV pages for num_beams full-length chunks; they share the prompt's pages and fork each other's pages every step.
+ * num_beams in 1 .. 8 and <= max_batch, early_tokens 0 when num_beams > 1 (no partial results: the hypothesis is known
+ * only at the end), a finite length_penalty, temperature > 0 with do_sample (transformers rejects it too), and an engine
+ * geometry the beam kernels take (<= 128 KV pages per chunk); otherwise XTTS_ERR_INVALID.  num_beams == 1 is xtts_submit_speed. */
+typedef struct xtts_beam {
+    int32_t num_beams;
+    float length_penalty;
+    int32_t do_sample;         /* 0: beam search, non-zero: beam sampling */
+} xtts_beam;
+int xtts_submit_beams(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, int32_t n_text, int32_t speaker_slot,
+                      const xtts_sampling* sp, float speed, const xtts_beam* beam);
+/* One beam step on caller arrays, for the isolation tests: logprob, select, reorder and partial-page copy of the engine's
+ * beam kernels, on one group of num_beams = nb (2..8) beams in slots 0..nb-1, without the final gather.  V <= 2048 tokens;
+ * sp: repetition_penalty, temperature / top_k / top_p (do_sample), max_tokens, stop_token, seed, seq_seed.  first: the
+ * group's first selection (row 0 of logits for every beam, running scores [0, -1e9, ...], only beam 0 owns pages);
+ * advance: KV positions the step appended (0 after the prefill, 1 after a decode step).  In / out: n_gen, ctx_len [nb]
+ * (equal across beams), seen [nb][ceil(V / 32)] bitmaps, block_tables [nb][max_pages] (max_pages <= 128), pool [nb *
+ * max_pages] (the first state->n_free entries are free page ids, n_free >= nb), hist [cap][8][2] (parent, token) rows,
+ * *state (the group state, transformers' beam-search tensors; sel_* / copy_* are this step's outputs), kpool / vpool
+ * [layers][n_pages pages] in the layout of xtts_debug_attn_decode, kv_type 0 fp32, 1 bf16, 2 fp16.  Out: last_tok [nb],
+ * scores [nb][V] (the processed, accumulated scores the selection ranked).  logits: [1][V] when first, else [nb][V]. */
+typedef struct xtts_beam_state {
+    float run_score[8], fin_score[8];
+    int32_t fin_valid[8], fin_step[8], fin_beam[8], fin_tok[8];
+    int32_t heur_unsat, done;
+    int32_t sel_parent[8], sel_tok[8];
+    int32_t n_copy, copy_src[8], copy_dst[8], copy_ntok[8];
+    int32_t n_free, n_pages[8];
+} xtts_beam_state;
+int xtts_debug_beam_step(xtts_engine* e, int32_t kv_type, int32_t heads, int32_t layers, int32_t V, const xtts_sampling* sp,
+                         const xtts_beam* beam, int32_t first, int32_t advance, const float* logits, int32_t* n_gen,
+                         int32_t* ctx_len, int32_t* last_tok, uint32_t* seen, int32_t max_pages, int32_t* block_tables,
+                         int32_t n_pages, int32_t* pool, int32_t cap, int32_t* hist, xtts_beam_state* state, void* kpool,
+                         void* vpool, float* scores);
 /* Aborts a chunk (the reference aborts the vLLM request when its generator is dropped).  A queued chunk is dropped, a
  * decoding one stops at the scheduler's next iteration and returns its batch slot and KV pages; either way exactly one
  * final result with status XTTS_ERR_CANCELLED is delivered.  Unknown / already finished ids are ignored. */
