@@ -40,7 +40,7 @@ inline KernelCtx& kctx() { return t_kctx ? *t_kctx : kctx_default(); }
 // Off by default; when on, every launcher records an event pair and its algorithmic FLOPs / bytes.
 enum KernelFamily : int {
     KF_GEMM_TC = 0, KF_GEMM_F32, KF_ATTN_DECODE, KF_ATTN_PREFILL, KF_NORM, KF_SAMPLE, KF_KV_WRITE, KF_EMBED,
-    KF_CONV1D, KF_CONVT, KF_CONV_POST, KF_INTERP, KF_COND, KF_MISC, KF_CONV1D_TC, KF_DECODE_CHAIN, KF_COUNT
+    KF_CONV1D, KF_CONVT, KF_CONV_POST, KF_INTERP, KF_COND, KF_MISC, KF_CONV1D_TC, KF_COUNT
 };
 struct KernelProfiler {
     bool enabled = false;
@@ -95,13 +95,6 @@ struct KernelCtx {
     int conv_tc_epilogue = 1;     // tensor-core Conv1d epilogue: 1 staged through shared memory + bulk copies, 0 direct
     int attn_ctas_per_sm = 0;     // 0 = uncapped decode-attention grid; > 0: at most this many CTAs per SM
     int gemm_decode_bn = 0;       // 0 = heuristic; 32/64/128 forces the tile width of decode-shaped tensor-core GEMMs
-    int attn_warps = 4;           // warps per (row, head) item of the bf16 decode attention (4, or 8: measured slower, run 7)
-    int attn_bulk = 0;            // > 0: 16-bit decode attention streams cache pages with cp.async.bulk, this many CTAs per SM
-    int attn_stages = 8;          // ring depth of that kernel (8 KB per stage)
-    int attn_l2_pages = 0;        // register-load decode attention: every warp prefetches the page this many of its pages ahead into L2
-    int attn_l2_ahead = 1;        // that kernel prefetches the next item's pages into L2 (cp.async.bulk.prefetch.L2)
-    int gemm_deep_ring = 0;       // decode-shaped unsplit GEMMs use a ring that fills the SM (BN 32: 10 stages, BN 64: 8) instead of 5 / 4
-    int gemm_l2_prefetch = 0;     // one-tile GEMM: weight tiles beyond the first ring pass are prefetched into L2 before the dependency wait
     int gemm_wide = 4;            // large shapes (M >= 256) go to the persistent wide-tile kernel (gemm_wgmma_wide.cu) with this ring depth (2-4); 0: off
 };
 #define g_prof (::xtts::kctx().prof)
@@ -111,13 +104,6 @@ struct KernelCtx {
 #define g_attn_ctas_per_sm (::xtts::kctx().attn_ctas_per_sm)
 #define g_gemm_decode_bn (::xtts::kctx().gemm_decode_bn)
 #define g_gemm_wide (::xtts::kctx().gemm_wide)
-#define g_attn_warps (::xtts::kctx().attn_warps)
-#define g_gemm_l2_prefetch (::xtts::kctx().gemm_l2_prefetch)
-#define g_gemm_deep_ring (::xtts::kctx().gemm_deep_ring)
-#define g_attn_bulk (::xtts::kctx().attn_bulk)
-#define g_attn_stages (::xtts::kctx().attn_stages)
-#define g_attn_l2_ahead (::xtts::kctx().attn_l2_ahead)
-#define g_attn_l2_pages (::xtts::kctx().attn_l2_pages)
 
 // true the first time it is called with the current CUDA device for this flag set (function attributes are per device)
 inline bool first_on_device(bool (&done)[64]) {
@@ -167,7 +153,7 @@ struct ProfScope {
 inline const char* kernel_family_name(int f) {
     static const char* n[KF_COUNT] = {"gemm_bf16_wgmma", "gemm_f32", "attn_decode_paged", "attn_prefill", "layernorm",
                                       "sample", "kv_write", "embed", "conv1d", "conv_transpose1d", "conv_post_tanh",
-                                      "interp", "conditioning", "misc", "conv1d_tc_f16_wgmma", "decode_chain_wgmma"};
+                                      "interp", "conditioning", "misc", "conv1d_tc_f16_wgmma"};
     return (f >= 0 && f < KF_COUNT) ? n[f] : "?";
 }
 
@@ -200,37 +186,6 @@ __device__ __forceinline__ void trace_pt(int id, int phase) {
 // init, weight-tile prefetch) and only blocks at griddepcontrol.wait before touching N's outputs.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-
-// ---- fine-grained dependencies along the decode chain.  `griddepcontrol.wait` resolves only when the whole prerequisite
-// grid has drained and flushed (measured: 1.2-5 us after its last CTA's exit, tools/trace_step.py).  With a DepFlag the
-// consumer instead polls a counter that every producer CTA bumps (release) right after its own stores: ~1 us.  The consumer
-// kernel is still launched with the PDL attribute (so it is resident early) but never executes griddepcontrol.wait; ordering
-// with everything older follows transitively, because its producer waited on ITS producer's flag before finishing.
-// wait == nullptr: fall back to griddepcontrol.wait.  One thread of the CTA calls dep_wait, then the CTA synchronises.
-struct DepFlag {
-    const unsigned* wait = nullptr;     // counter of the producer kernel (device)
-    unsigned target = 0;                // its value once every producer CTA has arrived
-    unsigned* arrive = nullptr;         // this kernel's own counter (nullptr: nobody polls it)
-};
-__device__ __forceinline__ void dep_wait(const DepFlag& d) {
-    if (d.wait == nullptr) { pdl_wait(); return; }
-    const long long t0 = clock64();
-    int polls = 0;
-    unsigned v;
-    while (true) {
-        asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(d.wait) : "memory");
-        if (v >= d.target) break;
-        __nanosleep(polls < 8 ? 100 : 400);          // hundreds of CTAs poll one line that the producers are also adding to
-        if ((++polls & 255) == 0 && clock64() - t0 > 4000000000LL) __trap();     // watchdog (no printf: see hopper.cuh)
-    }
-}
-// every thread that stored results calls this; `leader` (one thread, after a CTA barrier) publishes the CTA's arrival
-__device__ __forceinline__ void dep_arrive(const DepFlag& d, bool leader) {
-    if (d.arrive == nullptr) return;
-    __threadfence();
-    __syncthreads();
-    if (leader) asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(d.arrive) : "memory");
-}
 
 template <typename... KArgs, typename... Args>
 inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, Args&&... args) {

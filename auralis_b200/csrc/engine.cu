@@ -188,8 +188,7 @@ public:
     void debug_gemm(int mode, const float* A, const float* W, const float* bias, const float* resid, float* out, int M,
                     int N, int K, int dflags, int iters, float* ms);
     void debug_ln_gemm(int mode, int launch, int M, int N, int K, const float* X, const float* ln_w, const float* ln_b,
-                       const float* W, const float* bias, const float* resid, int dflags, float* Y, float* out, int32_t* n_ctas,
-                       uint32_t* counters);
+                       const float* W, const float* bias, const float* resid, int dflags, float* Y, float* out);
     void debug_norms(int out_type, int M, int H, const float* X, int x_rows, const int32_t* row_index, const float* w1,
                      const float* b1, const float* w2, const float* b2, float* Y, float* latents, int n_slots, int lat_rows,
                      const int32_t* slots, const int32_t* lat_pos, const int32_t* n_gen);
@@ -200,8 +199,7 @@ public:
                           const float* wte, int n_audio, const float* wpe, int n_wpe, const float* spk, int n_spk,
                           const int32_t* rows, int n_rows, float* X);
     void debug_build_decode_rows(int H, const float* wte, int n_audio, const float* wpe, int n_wpe, int M, const int32_t* active,
-                                 int n_slots, const int32_t* last_tok, const int32_t* n_gen, float* X, uint32_t* counters,
-                                 int n_flags, int n_words);
+                                 int n_slots, const int32_t* last_tok, const int32_t* n_gen, float* X);
     void debug_sample_slots(int V, int M, const int32_t* active, int n_slots, const float* logits, int ld,
                             const xtts_sampling* sp, int cap, int advance_ctx, const int32_t* forced, int32_t* n_gen,
                             int32_t* ctx_len, int32_t* finished, int32_t* last_tok, uint8_t* seen, int32_t* tokens,
@@ -362,15 +360,9 @@ private:
     std::map<int, std::pair<cudaGraphExec_t, KernelProfiler::GraphRecs*>> prof_graphs;   // decode graphs with event-record nodes (option "profile")
     KernelProfiler::GraphRecs* last_prof = nullptr;     // recs of the profiled graph launched by the current step
     void drop_graphs();
-    bool use_chain = false;       // option "decode_chain": fused persistent per-layer GEMM/LayerNorm chain kernel (measured slower, see DESIGN.md)
-    DBuf<unsigned> d_chain_sync;  // device-wide barrier words of the chain kernel
     DBuf<unsigned long long> d_trace; DBuf<unsigned> d_trace_n;      // debug timeline (xtts_debug_trace)
     int n_micro = 2;              // option "microbatches": decode rows are split into this many concurrent branches
     int micro_min_rows = 48;      // option "microbatch_min_rows": below this many active rows the step stays single-branch
-    int stagger_us = 0;           // option "branch_stagger_us": branch i starts i * this many microseconds late
-    bool use_dep_flags = false;   // option "dep_flags": counter dependencies along the decode chain instead of grid-wide waits
-                                  // (parity-tested; measured SLOWER than griddepcontrol.wait, runs 6-7: kept as an experiment)
-    DBuf<unsigned> d_dep;         // [kMaxMicro][layers][7] dependency counters (zeroed by the first kernel of every step)
     int eager_steps_done = 0;
     std::map<int, cudaGraphExec_t> decode_graphs;
     std::map<int, unsigned long long> graph_kernels;
@@ -411,14 +403,13 @@ private:
     void layers_forward(int M, bool prefill, int nseq, int max_nq);
     void head_and_sample(int M, const int* row_index, const int* slots_dev, const int* lat_pos, int advance_ctx, bool do_sample,
                          bool pdl_first = true);
-    void decode_layers_rows(int r0, int Mi, cudaStream_t s, bool pdl_first, double ctx_sum, int branch);
+    void decode_layers_rows(int r0, int Mi, cudaStream_t s, bool pdl_first, double ctx_sum);
     // split-K reduction + bias + residual + LayerNorm into the 16-bit operand buffer, in the engine's 16-bit format
     void reduce_ln16(float* X, const float* part, int splits, const float* bias, const float* w, const float* b, __nv_bfloat16* Y, int M,
-                     cudaStream_t s, bool pdl, DepFlag dep) {
-        if (f16) launch_residual_reduce_layernorm<__half>(X, part, splits, bias, w, b, reinterpret_cast<__half*>(Y), M, H, cfg.ln_eps, s, pdl, dep);
-        else launch_residual_reduce_layernorm<__nv_bfloat16>(X, part, splits, bias, w, b, Y, M, H, cfg.ln_eps, s, pdl, dep);
+                     cudaStream_t s, bool pdl) {
+        if (f16) launch_residual_reduce_layernorm<__half>(X, part, splits, bias, w, b, reinterpret_cast<__half*>(Y), M, H, cfg.ln_eps, s, pdl);
+        else launch_residual_reduce_layernorm<__nv_bfloat16>(X, part, splits, bias, w, b, Y, M, H, cfg.ln_eps, s, pdl);
     }
-    void decode_layers_chain(int M);
     void init_slots(const std::vector<Sequence*>& seqs, const int32_t* forced, int n_forced);
     void release_pages(Sequence& s);
     void release_slot(Sequence& s);
@@ -546,8 +537,6 @@ Engine::Engine(const xtts_config& c) : cfg(c) {
     wX.alloc(Mmax * H); wQKV.alloc(Mmax * 3 * H); wLOG.alloc((size_t)std::max(NSLOT, CAP + 1) * Vpad);
     d_beam_scores.alloc((size_t)NSLOT * Vpad);
     if (bf16) wPART.alloc((size_t)8 * NSLOT * H);
-    d_chain_sync.alloc(64); d_chain_sync.zero(st);
-    d_dep.alloc((size_t)kMaxMicro * L * 7); d_dep.zero(st);
     if (bf16) { wXn16.alloc(Mmax * H); wATT16.alloc(Mmax * H); wFF16.alloc(Mmax * FF); wY16.alloc((size_t)std::max(NSLOT, CAP + 1) * H); }
     else { wXn32.alloc(Mmax * H); wATT32.alloc(Mmax * H); wFF32.alloc(Mmax * FF); wY32.alloc((size_t)std::max(NSLOT, CAP + 1) * H); }
 
@@ -1038,13 +1027,13 @@ void Engine::layers_forward(int M, bool prefill, int nseq, int max_nq) {
             else launch_attn_decode<float, float>(wQKV.p, d_active.p, M, d_ctx_len.p, d_block_tables.p, max_pages, k32[l]->p, v32[l]->p, wATT32.p, NH, st, decode_ctx_sum, pdl);
         }
         if (splitk) {
-            launch_gemm_bf16_tc_splitk(wATT16.p, ly.o.w16.p, wPART.p, M, H, H, 4, st, pdl, DepFlag(), gflag);
-            reduce_ln16(wX.p, wPART.p, 4, ly.o.b.p, ly.ln2w.p, ly.ln2b.p, wXn16.p, M, st, pdl, DepFlag());
+            launch_gemm_bf16_tc_splitk(wATT16.p, ly.o.w16.p, wPART.p, M, H, H, 4, st, pdl, gflag);
+            reduce_ln16(wX.p, wPART.p, 4, ly.o.b.p, ly.ln2w.p, ly.ln2b.p, wXn16.p, M, st, pdl);
             gemm(Xn, ly.fc, nullptr, FFb, M, GEMM_GELU | oflag, pdl);
-            launch_gemm_bf16_tc_splitk(wFF16.p, ly.proj.w16.p, wPART.p, M, H, FF, 8, st, pdl, DepFlag(), gflag);
+            launch_gemm_bf16_tc_splitk(wFF16.p, ly.proj.w16.p, wPART.p, M, H, FF, 8, st, pdl, gflag);
             const bool last = (l + 1 == L);
             reduce_ln16(wX.p, wPART.p, 8, ly.proj.b.p, last ? nullptr : layers[l + 1]->ln1w.p,
-                        last ? nullptr : layers[l + 1]->ln1b.p, last ? nullptr : wXn16.p, M, st, pdl, DepFlag());
+                        last ? nullptr : layers[l + 1]->ln1b.p, last ? nullptr : wXn16.p, M, st, pdl);
         } else {
             gemm(ATT, ly.o, wX.p, wX.p, M, GEMM_RESID, pdl);
             ln(ly.ln2w.p, ly.ln2b.p);
@@ -1220,7 +1209,7 @@ void Engine::prefill(const std::vector<Sequence*>& seqs) {
 // Fast-mode decode layers for rows [r0, r0 + Mi) of the step on stream `s`.  Every work buffer is row-major and the
 // KV cache is per slot, so disjoint row ranges are independent: decode_step runs several of these as concurrent
 // branches (micro-batches), which lets one branch's HBM-bound attention overlap another's latency-bound GEMM chain.
-void Engine::decode_layers_rows(int r0, int Mi, cudaStream_t s, bool pdl_first, double ctx_sum, int branch) {
+void Engine::decode_layers_rows(int r0, int Mi, cudaStream_t s, bool pdl_first, double ctx_sum) {
     float* X = wX.p + (size_t)r0 * H;
     __nv_bfloat16* Xn = wXn16.p + (size_t)r0 * H;
     float* QKV = wQKV.p + (size_t)r0 * 3 * H;
@@ -1229,64 +1218,24 @@ void Engine::decode_layers_rows(int r0, int Mi, cudaStream_t s, bool pdl_first, 
     float* PART = wPART.p + (size_t)r0 * 8 * H;          // [splits <= 8][Mi][H] inside this branch's own region
     const int* act = d_active.p + r0;
     const bool pdl = use_pdl;
-    // Dependency counters of this branch (option "dep_flags"): 7 per layer — ln1, qkv, attn, o-proj, ln2, fc, down-proj done.
-    // Every kernel polls its producer's counter instead of waiting for that whole grid to drain (common.cuh: DepFlag);
-    // build_decode_rows zeroed them at the start of the step.
-    const bool flags = use_dep_flags && d_dep.p != nullptr;
-    unsigned* F = flags ? d_dep.p + (size_t)branch * L * 7 : nullptr;
-    auto dep = [&](int l_wait, int e_wait, unsigned target, int l_arr, int e_arr) {
-        DepFlag d;
-        if (flags) { d.wait = F + l_wait * 7 + e_wait; d.target = target; d.arrive = F + l_arr * 7 + e_arr; }
-        return d;
-    };
-    DepFlag d0;
-    if (flags) d0.arrive = F + 0;                        // the step's first LayerNorm: full wait (the row build), then counts in
-    if (f16) launch_layernorm<__half>(X, layers[0]->ln1w.p, layers[0]->ln1b.p, reinterpret_cast<__half*>(Xn), Mi, H, cfg.ln_eps, s, pdl && pdl_first, d0);
-    else launch_layernorm<__nv_bfloat16>(X, layers[0]->ln1w.p, layers[0]->ln1b.p, Xn, Mi, H, cfg.ln_eps, s, pdl && pdl_first, d0);
-    unsigned n_ln1 = (unsigned)Mi;
+    if (f16) launch_layernorm<__half>(X, layers[0]->ln1w.p, layers[0]->ln1b.p, reinterpret_cast<__half*>(Xn), Mi, H, cfg.ln_eps, s, pdl && pdl_first);
+    else launch_layernorm<__nv_bfloat16>(X, layers[0]->ln1w.p, layers[0]->ln1b.p, Xn, Mi, H, cfg.ln_eps, s, pdl && pdl_first);
     for (int l = 0; l < L; ++l) {
         Layer& ly = *layers[l];
-        const unsigned n_qkv = (unsigned)launch_gemm_bf16_tc(Xn, ly.qkv.w16.p, ly.qkv.b.p, nullptr, QKV, Mi, ly.qkv.N, ly.qkv.K, gflag, s, pdl,
-                                                             dep(l, 0, n_ln1, l, 1));
-        const unsigned n_att = f16
-            ? (unsigned)launch_attn_decode<__half, __half>(QKV, act, Mi, d_ctx_len.p, d_block_tables.p, max_pages, reinterpret_cast<__half*>(k16[l]->p),
-                                                           reinterpret_cast<__half*>(v16[l]->p), reinterpret_cast<__half*>(ATT), NH, s, ctx_sum, pdl,
-                                                           dep(l, 1, n_qkv, l, 2))
-            : (unsigned)launch_attn_decode<__nv_bfloat16, __nv_bfloat16>(QKV, act, Mi, d_ctx_len.p, d_block_tables.p, max_pages, k16[l]->p, v16[l]->p,
-                                                                         ATT, NH, s, ctx_sum, pdl, dep(l, 1, n_qkv, l, 2));
-        const unsigned n_o = (unsigned)launch_gemm_bf16_tc_splitk(ATT, ly.o.w16.p, PART, Mi, H, H, 4, s, pdl, dep(l, 2, n_att, l, 3), gflag);
-        reduce_ln16(X, PART, 4, ly.o.b.p, ly.ln2w.p, ly.ln2b.p, Xn, Mi, s, pdl, dep(l, 3, n_o, l, 4));
-        const unsigned n_fc = (unsigned)launch_gemm_bf16_tc(Xn, ly.fc.w16.p, ly.fc.b.p, nullptr, FFb, Mi, ly.fc.N, ly.fc.K,
-                                                            GEMM_GELU | GEMM_OUT_BF16 | gflag, s, pdl, dep(l, 4, (unsigned)Mi, l, 5));
-        const unsigned n_pr = (unsigned)launch_gemm_bf16_tc_splitk(FFb, ly.proj.w16.p, PART, Mi, H, FF, 8, s, pdl, dep(l, 5, n_fc, l, 6), gflag);
+        launch_gemm_bf16_tc(Xn, ly.qkv.w16.p, ly.qkv.b.p, nullptr, QKV, Mi, ly.qkv.N, ly.qkv.K, gflag, s, pdl);
+        if (f16)
+            launch_attn_decode<__half, __half>(QKV, act, Mi, d_ctx_len.p, d_block_tables.p, max_pages, reinterpret_cast<__half*>(k16[l]->p),
+                                               reinterpret_cast<__half*>(v16[l]->p), reinterpret_cast<__half*>(ATT), NH, s, ctx_sum, pdl);
+        else
+            launch_attn_decode<__nv_bfloat16, __nv_bfloat16>(QKV, act, Mi, d_ctx_len.p, d_block_tables.p, max_pages, k16[l]->p, v16[l]->p,
+                                                             ATT, NH, s, ctx_sum, pdl);
+        launch_gemm_bf16_tc_splitk(ATT, ly.o.w16.p, PART, Mi, H, H, 4, s, pdl, gflag);
+        reduce_ln16(X, PART, 4, ly.o.b.p, ly.ln2w.p, ly.ln2b.p, Xn, Mi, s, pdl);
+        launch_gemm_bf16_tc(Xn, ly.fc.w16.p, ly.fc.b.p, nullptr, FFb, Mi, ly.fc.N, ly.fc.K, GEMM_GELU | GEMM_OUT_BF16 | gflag, s, pdl);
+        launch_gemm_bf16_tc_splitk(FFb, ly.proj.w16.p, PART, Mi, H, FF, 8, s, pdl, gflag);
         const bool last = (l + 1 == L);
-        DepFlag dl = dep(l, 6, n_pr, last ? l : l + 1, 0);
-        if (last) dl.arrive = nullptr;                   // the head kernel behind it takes a full dependency
         reduce_ln16(X, PART, 8, ly.proj.b.p, last ? nullptr : layers[l + 1]->ln1w.p, last ? nullptr : layers[l + 1]->ln1b.p,
-                    last ? nullptr : Xn, Mi, s, pdl, dl);
-        n_ln1 = (unsigned)Mi;
-    }
-}
-
-// Fast-mode decode layers with the fused chain kernel: per layer one attention launch and one persistent launch that
-// runs out-proj, residual+LN2, fc+gelu, down-proj, residual+LN1(next) and the next layer's QKV projection.
-void Engine::decode_layers_chain(int M) {
-    const bool pdl = use_pdl;
-    launch_layernorm<__nv_bfloat16>(wX.p, layers[0]->ln1w.p, layers[0]->ln1b.p, wXn16.p, M, H, cfg.ln_eps, st, pdl);
-    launch_gemm_bf16_tc(wXn16.p, layers[0]->qkv.w16.p, layers[0]->qkv.b.p, nullptr, wQKV.p, M, layers[0]->qkv.N, layers[0]->qkv.K, 0, st, pdl);
-    for (int l = 0; l < L; ++l) {
-        Layer& ly = *layers[l];
-        Layer* nx = (l + 1 < L) ? layers[l + 1].get() : nullptr;
-        launch_attn_decode<__nv_bfloat16, __nv_bfloat16>(wQKV.p, d_active.p, M, d_ctx_len.p, d_block_tables.p, max_pages, k16[l]->p, v16[l]->p,
-                                                         wATT16.p, NH, st, decode_ctx_sum, pdl);
-        DecodeChainArgs a{};
-        a.phases = DC_PROJ | DC_LN2 | DC_FC | DC_FC2 | DC_LN1 | (nx ? DC_QKV : 0);
-        a.M = M; a.H = H; a.FF = FF; a.eps = cfg.ln_eps;
-        a.ATT = wATT16.p; a.Wo = ly.o.w16.p; a.Wfc = ly.fc.w16.p; a.Wproj = ly.proj.w16.p; a.Wqkv = nx ? nx->qkv.w16.p : nullptr;
-        a.proj_bias = ly.o.b.p; a.ln2_w = ly.ln2w.p; a.ln2_b = ly.ln2b.p; a.fc_bias = ly.fc.b.p; a.fc2_bias = ly.proj.b.p;
-        a.ln1_w = nx ? nx->ln1w.p : nullptr; a.ln1_b = nx ? nx->ln1b.p : nullptr; a.qkv_bias = nx ? nx->qkv.b.p : nullptr;
-        a.X = wX.p; a.Xn = wXn16.p; a.FFb = wFF16.p; a.QKV = wQKV.p; a.PART = wPART.p; a.sync = d_chain_sync.p;
-        launch_decode_chain(a, st, pdl);
+                    last ? nullptr : Xn, Mi, s, pdl);
     }
 }
 
@@ -1306,19 +1255,16 @@ void Engine::decode_step(const std::vector<int>& active) {
     const int M = (int)active.size();
     d_active.upload(active.data(), M, st);
     const bool fast = bf16 && use_splitk && M <= NSLOT && (H / 64) % 4 == 0 && (FF / 64) % 8 == 0;
-    const bool chain = fast && use_chain && !f16 && decode_chain_supported(M, H, FF);
-    const int nmb = (fast && !chain && n_micro > 1 && M >= micro_min_rows) ? std::min(n_micro, (int)kMaxMicro) : 1;
+    const int nmb = (fast && n_micro > 1 && M >= micro_min_rows) ? std::min(n_micro, (int)kMaxMicro) : 1;
     auto enqueue = [&] {
-        launch_build_decode_rows(d_active.p, M, d_last_tok.p, d_n_gen.p, tables(), wX.p, st, use_pdl,
-                                 (fast && use_dep_flags) ? d_dep.p : nullptr, kMaxMicro * L * 7);
+        launch_build_decode_rows(d_active.p, M, d_last_tok.p, d_n_gen.p, tables(), wX.p, st, use_pdl);
         if (nmb > 1) {
             // fork: every branch starts after the row build; join: head + sampler run once over all rows
             CUDA_CHECK(cudaEventRecord(ev_fork, st));
             for (int i = 1; i < nmb; ++i) CUDA_CHECK(cudaStreamWaitEvent(st_mb[i], ev_fork, 0));
             for (int i = 0, r0 = 0; i < nmb; ++i) {
                 const int Mi = M / nmb + (i < M % nmb ? 1 : 0);
-                if (i > 0 && stagger_us > 0) launch_stream_delay((unsigned)(i * stagger_us) * 1000u, st_mb[i], false);
-                decode_layers_rows(r0, Mi, st_mb[i], i == 0, decode_ctx_sum * (double)Mi / (double)M, i);
+                decode_layers_rows(r0, Mi, st_mb[i], i == 0, decode_ctx_sum * (double)Mi / (double)M);
                 r0 += Mi;
             }
             for (int i = 1; i < nmb; ++i) {
@@ -1327,8 +1273,7 @@ void Engine::decode_step(const std::vector<int>& active) {
             }
             head_and_sample(M, nullptr, d_active.p, nullptr, 1, true, false);
         } else {
-            if (chain) decode_layers_chain(M);
-            else if (fast) decode_layers_rows(0, M, st, true, decode_ctx_sum, 0);
+            if (fast) decode_layers_rows(0, M, st, true, decode_ctx_sum);
             else layers_forward(M, false, 0, 0);
             head_and_sample(M, nullptr, d_active.p, nullptr, 1, true);
         }
@@ -2184,19 +2129,12 @@ void Engine::set_option(const std::string& k, int64_t v) {
         if (v != 0 && (v < 2 || v > 4)) throw std::runtime_error("gemm_wide: 0 (off) or a ring depth of 2, 3 or 4");
         g_gemm_wide = (int)v;
     }
-    else if (k == "attn_bulk") { g_attn_bulk = (int)std::max<int64_t>(0, std::min<int64_t>(v, 4)); drop_graphs(); }
-    else if (k == "gemm_deep_ring") { g_gemm_deep_ring = v ? 1 : 0; drop_graphs(); }
-    else if (k == "gemm_l2_prefetch") { g_gemm_l2_prefetch = v ? 1 : 0; drop_graphs(); }
-    else if (k == "attn_l2_pages") { g_attn_l2_pages = (int)std::max<int64_t>(0, std::min<int64_t>(v, 8)); drop_graphs(); }
-    else if (k == "attn_l2_ahead") { g_attn_l2_ahead = v ? 1 : 0; drop_graphs(); }
-    else if (k == "attn_stages") { g_attn_stages = (int)std::max<int64_t>(4, std::min<int64_t>(v, 24)); drop_graphs(); }
-    else if (k == "attn_warps") { g_attn_warps = (v == 1 || v == 2 || v == 8 || v == 16) ? (int)v : 4; drop_graphs(); }
     else if (k == "cuda_graphs") use_graphs = v != 0;
     else if (k == "pdl") { use_pdl = v != 0; drop_graphs(); }
     else if (k == "splitk") { use_splitk = v != 0; drop_graphs(); }
-    else if (k == "decode_chain") { use_chain = v != 0; drop_graphs(); }
-    else if (k == "dep_flags") { use_dep_flags = v != 0; drop_graphs(); }
-    else if (k == "branch_stagger_us") { stagger_us = (int)std::max<int64_t>(0, std::min<int64_t>(v, 1000)); drop_graphs(); }
+    else if (k == "decode_chain") {                               // still accepted so that callers passing 0 keep working
+        if (v != 0) throw std::runtime_error("decode_chain: the fused decode chain kernel was removed; only 0 is accepted");
+    }
     else if (k == "microbatches" || k == "microbatch_min_rows") {
         if (k == "microbatches") n_micro = std::max<int>(1, std::min<int64_t>(v, kMaxMicro)); else micro_min_rows = (int)std::max<int64_t>(2, v);
         drop_graphs();
@@ -2798,7 +2736,7 @@ void Engine::debug_splitk_ln(int mode, int M, int N, int K, int splits, const fl
         launch_f32_to_f16(dA.p, reinterpret_cast<__half*>(hA.p), (size_t)M * K, st);
         launch_f32_to_f16(dW.p, reinterpret_cast<__half*>(hW.p), (size_t)N * K, st);
     }
-    launch_gemm_bf16_tc_splitk(hA.p, hW.p, dpart.p, M, N, K, splits, st, false, DepFlag(), mode == 2 ? GEMM_F16 : 0);
+    launch_gemm_bf16_tc_splitk(hA.p, hW.p, dpart.p, M, N, K, splits, st, false, mode == 2 ? GEMM_F16 : 0);
     if (mode == 2)
         launch_residual_reduce_layernorm<__half>(dX.p, dpart.p, splits, db.p, dlw.p, dlb.p, reinterpret_cast<__half*>(dY.p), M, N,
                                                  cfg.ln_eps, st);
@@ -2812,51 +2750,40 @@ void Engine::debug_splitk_ln(int mode, int M, int N, int K, int splits, const fl
 }
 
 // The decode step's LayerNorm -> GEMM pair as decode_layers_rows launches it: the 16-bit LayerNorm into the operand buffer,
-// then the one-tile GEMM on it.  launch 0: plain launches; 1: both with PDL; 2: PDL plus dependency counters (the LN waits
-// for its predecessor in full and counts its CTAs into counter 0, the GEMM polls counter 0 for M arrivals instead of
-// griddepcontrol.wait and counts its CTAs into counter 1).
+// then the one-tile GEMM on it.  launch 0: plain launches; 1: both with PDL.
 void Engine::debug_ln_gemm(int mode, int launch, int M, int N, int K, const float* X, const float* ln_w, const float* ln_b,
-                           const float* W, const float* bias, const float* resid, int dflags, float* Y, float* out,
-                           int32_t* n_ctas, uint32_t* counters) {
+                           const float* W, const float* bias, const float* resid, int dflags, float* Y, float* out) {
     ApiLock lk(this);
     if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
     if (mode != 1 && mode != 2) throw std::runtime_error("debug_ln_gemm: mode 1 (bf16) or 2 (fp16)");
-    if (launch < 0 || launch > 2) throw std::runtime_error("debug_ln_gemm: launch 0 (plain), 1 (PDL) or 2 (PDL + counters)");
+    if (launch < 0 || launch > 1) throw std::runtime_error("debug_ln_gemm: launch 0 (plain) or 1 (PDL)");
     if (M < 1 || N < 32 || N % 32 != 0 || K < 64 || K % 64 != 0 || K > 8192) throw std::runtime_error("debug_ln_gemm: need M >= 1, N % 32 == 0, K % 64 == 0 (<= 8192)");
     if (dflags & ~(XTTS_DEBUG_GEMM_GELU | XTTS_DEBUG_GEMM_OUT16)) throw std::runtime_error("debug_ln_gemm: flags GELU / OUT16 only");
-    if (!X || !ln_w || !ln_b || !W || !Y || !out || !n_ctas || !counters) throw std::runtime_error("debug_ln_gemm: only bias and resid may be NULL");
+    if (!X || !ln_w || !ln_b || !W || !Y || !out) throw std::runtime_error("debug_ln_gemm: only bias and resid may be NULL");
     if (resid && (dflags & XTTS_DEBUG_GEMM_OUT16)) throw std::runtime_error("debug_ln_gemm: a residual needs fp32 output");
-    // (launch_gemm_bf16_tc refuses it too, but only after the LayerNorm has been enqueued)
-    if (resid && launch == 2) throw std::runtime_error("debug_ln_gemm: a counter dependency cannot order a residual read");
     CUDA_CHECK(cudaSetDevice(cfg.device));
     std::string err;
     if (!gemm_tc_init(&err)) throw std::runtime_error(err);
     const bool out16 = dflags & XTTS_DEBUG_GEMM_OUT16;
     DBuf<float> dX, dlw, dlb, dW, db, dr, dout;
     DBuf<__nv_bfloat16> hW, dY, dout16;
-    DBuf<unsigned> dcnt;
     dX.alloc((size_t)M * K); dlw.alloc(K); dlb.alloc(K); dW.alloc((size_t)N * K); hW.alloc((size_t)N * K); dY.alloc((size_t)M * K);
-    dcnt.alloc(2);
     if (out16) dout16.alloc((size_t)M * N); else dout.alloc((size_t)M * N);
     dX.upload(X, (size_t)M * K, st); dlw.upload(ln_w, K, st); dlb.upload(ln_b, K, st); dW.upload(W, (size_t)N * K, st);
     if (bias) { db.alloc(N); db.upload(bias, N, st); }
     if (resid) { dr.alloc((size_t)M * N); dr.upload(resid, (size_t)M * N, st); }
     to16(mode, dW.p, hW.p, (size_t)N * K, st);
-    CUDA_CHECK(cudaMemsetAsync(dcnt.p, 0, 2 * sizeof(unsigned), st));
     CUDA_CHECK(cudaStreamSynchronize(st));
-    const bool pdl = launch >= 1;
-    DepFlag dln, dg;
-    if (launch == 2) { dln.arrive = dcnt.p; dg.wait = dcnt.p; dg.target = (unsigned)M; dg.arrive = dcnt.p + 1; }
-    if (mode == 2) launch_layernorm<__half>(dX.p, dlw.p, dlb.p, reinterpret_cast<__half*>(dY.p), M, K, cfg.ln_eps, st, pdl, dln);
-    else launch_layernorm<__nv_bfloat16>(dX.p, dlw.p, dlb.p, dY.p, M, K, cfg.ln_eps, st, pdl, dln);
+    const bool pdl = launch == 1;
+    if (mode == 2) launch_layernorm<__half>(dX.p, dlw.p, dlb.p, reinterpret_cast<__half*>(dY.p), M, K, cfg.ln_eps, st, pdl);
+    else launch_layernorm<__nv_bfloat16>(dX.p, dlw.p, dlb.p, dY.p, M, K, cfg.ln_eps, st, pdl);
     const int flags = ((dflags & XTTS_DEBUG_GEMM_GELU) ? GEMM_GELU : 0) | (out16 ? GEMM_OUT_BF16 : 0) | (resid ? GEMM_RESID : 0) |
                       (mode == 2 ? GEMM_F16 : 0);
-    *n_ctas = launch_gemm_bf16_tc(dY.p, hW.p, db.p, dr.p, out16 ? (void*)dout16.p : (void*)dout.p, M, N, K, flags, st, pdl, dg);
+    launch_gemm_bf16_tc(dY.p, hW.p, db.p, dr.p, out16 ? (void*)dout16.p : (void*)dout.p, M, N, K, flags, st, pdl);
     std::vector<uint16_t> y((size_t)M * K), o16(out16 ? (size_t)M * N : 0);
     dY.download(reinterpret_cast<__nv_bfloat16*>(y.data()), y.size(), st);
     if (out16) dout16.download(reinterpret_cast<__nv_bfloat16*>(o16.data()), o16.size(), st);
     else dout.download(out, (size_t)M * N, st);
-    dcnt.download(counters, 2, st);
     CUDA_CHECK(cudaStreamSynchronize(st));
     widen16(y, mode == 2, Y);
     if (out16) widen16(o16, mode == 2, out);
@@ -2990,16 +2917,13 @@ void Engine::debug_build_rows(int Hd, int n_cond, const float* text_emb, int n_t
     CUDA_CHECK(cudaStreamSynchronize(st));
 }
 
-// launch_build_decode_rows over private tables and slot arrays; counters [n_words] in/out, the first n_flags of them are the
-// step's dependency counters the kernel zeroes (the rest are guard words it must not touch)
+// launch_build_decode_rows over private tables and slot arrays
 void Engine::debug_build_decode_rows(int Hd, const float* wte_h, int n_audio, const float* wpe_h, int n_wpe, int M,
-                                     const int32_t* active, int n_slots, const int32_t* last_tok, const int32_t* n_gen, float* X,
-                                     uint32_t* counters, int n_flags, int n_words) {
+                                     const int32_t* active, int n_slots, const int32_t* last_tok, const int32_t* n_gen, float* X) {
     ApiLock lk(this);
     if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
     if (Hd < 4 || Hd % 4 != 0 || M < 1 || n_slots < 1 || n_audio < 1 || n_wpe < 1) throw std::runtime_error("debug_build_decode_rows: need H % 4 == 0, M >= 1 and non-empty tables");
     if (!wte_h || !wpe_h || !active || !last_tok || !n_gen || !X) throw std::runtime_error("debug_build_decode_rows: NULL argument");
-    if (n_flags < 0 || n_words < n_flags || (n_words > 0 && !counters)) throw std::runtime_error("debug_build_decode_rows: need 0 <= n_flags <= n_words and the counters");
     for (int i = 0; i < M; ++i) {
         const int s = active[i];
         if (s < 0 || s >= n_slots) throw std::runtime_error("debug_build_decode_rows: active slot outside n_slots");
@@ -3009,16 +2933,13 @@ void Engine::debug_build_decode_rows(int Hd, const float* wte_h, int n_audio, co
     CUDA_CHECK(cudaSetDevice(cfg.device));
     DBuf<float> dwte, dwpe, dX;
     DBuf<int> dact, dlast, dng;
-    DBuf<unsigned> dcnt;
     dwte.alloc((size_t)n_audio * Hd); dwpe.alloc((size_t)n_wpe * Hd); dX.alloc((size_t)M * Hd);
     dact.alloc(M); dlast.alloc(n_slots); dng.alloc(n_slots);
     dwte.upload(wte_h, (size_t)n_audio * Hd, st); dwpe.upload(wpe_h, (size_t)n_wpe * Hd, st);
     dact.upload(active, M, st); dlast.upload(last_tok, n_slots, st); dng.upload(n_gen, n_slots, st);
-    if (n_words > 0) { dcnt.alloc(n_words); dcnt.upload(counters, n_words, st); }
     GptTables t{}; t.wte = dwte.p; t.wpe = dwpe.p; t.H = Hd;
-    launch_build_decode_rows(dact.p, M, dlast.p, dng.p, t, dX.p, st, use_pdl, n_flags > 0 ? dcnt.p : nullptr, n_flags);
+    launch_build_decode_rows(dact.p, M, dlast.p, dng.p, t, dX.p, st, use_pdl);
     dX.download(X, (size_t)M * Hd, st);
-    if (n_words > 0) dcnt.download(counters, n_words, st);
     CUDA_CHECK(cudaStreamSynchronize(st));
 }
 
@@ -3250,8 +3171,8 @@ int xtts_debug_gemm(xtts_engine* e, int32_t mode, const float* A, const float* W
 }
 int xtts_debug_ln_gemm(xtts_engine* e, int32_t mode, int32_t launch, int32_t M, int32_t N, int32_t K, const float* X,
                        const float* ln_w, const float* ln_b, const float* W, const float* bias, const float* resid, int32_t flags,
-                       float* Y, float* out, int32_t* n_ctas, uint32_t* counters) {
-    XTTS_TRY(e->impl->debug_ln_gemm(mode, launch, M, N, K, X, ln_w, ln_b, W, bias, resid, flags, Y, out, n_ctas, counters))
+                       float* Y, float* out) {
+    XTTS_TRY(e->impl->debug_ln_gemm(mode, launch, M, N, K, X, ln_w, ln_b, W, bias, resid, flags, Y, out))
 }
 int xtts_debug_norms(xtts_engine* e, int32_t out_type, int32_t M, int32_t H, const float* X, int32_t x_rows,
                      const int32_t* row_index, const float* w1, const float* b1, const float* w2, const float* b2, float* Y,
@@ -3274,9 +3195,8 @@ int xtts_debug_build_rows(xtts_engine* e, int32_t H, int32_t n_cond, const float
 }
 int xtts_debug_build_decode_rows(xtts_engine* e, int32_t H, const float* wte, int32_t n_audio, const float* wpe, int32_t n_wpe,
                                  int32_t M, const int32_t* active, int32_t n_slots, const int32_t* last_tok, const int32_t* n_gen,
-                                 float* X, uint32_t* counters, int32_t n_flags, int32_t n_words) {
-    XTTS_TRY(e->impl->debug_build_decode_rows(H, wte, n_audio, wpe, n_wpe, M, active, n_slots, last_tok, n_gen, X, counters, n_flags,
-                                              n_words))
+                                 float* X) {
+    XTTS_TRY(e->impl->debug_build_decode_rows(H, wte, n_audio, wpe, n_wpe, M, active, n_slots, last_tok, n_gen, X))
 }
 int xtts_debug_sample_slots(xtts_engine* e, int32_t V, int32_t M, const int32_t* active, int32_t n_slots, const float* logits,
                             int32_t ld, const xtts_sampling* sp, int32_t cap, int32_t advance_ctx, const int32_t* forced,

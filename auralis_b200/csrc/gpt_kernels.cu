@@ -40,11 +40,8 @@ __global__ void build_rows_kernel(const RowDesc* __restrict__ rows, GptTables t,
 }
 
 __global__ void build_decode_rows_kernel(const int* __restrict__ active, const int* __restrict__ last_tok,
-                                         const int* __restrict__ n_gen, GptTables t, float* __restrict__ X,
-                                         unsigned* __restrict__ dep_flags, int n_flags) {
+                                         const int* __restrict__ n_gen, GptTables t, float* __restrict__ X) {
     trace_pt(TR_ROWS, 0); pdl_trigger(); pdl_wait(); trace_pt(TR_ROWS, 1);
-    // first kernel of the step, behind a full dependency wait: the step's dependency counters start from zero
-    if (blockIdx.x == 0) for (int i = threadIdx.x; i < n_flags; i += blockDim.x) dep_flags[i] = 0u;
     const int slot = active[blockIdx.x];
     const int H = t.H;
     const float4* a = reinterpret_cast<const float4*>(t.wte + (size_t)last_tok[slot] * H);
@@ -82,20 +79,6 @@ init_slots_kernel(const SlotInit* __restrict__ init, const int* __restrict__ pag
         a.block_tables[(size_t)slot * a.max_pages + i] = i < d.n_pages ? pg[i] : 0;
 }
 
-// Holds its stream for `ns` nanoseconds (one thread).  Used once per decode step to start the second row branch half a layer
-// late: two identical branches otherwise run in lock-step — both in the HBM-bound attention at the same time (each at half
-// the bandwidth), then both in the latency-bound GEMM chain (contending for SMs) — instead of one's attention under the
-// other's GEMMs.
-__global__ void stream_delay_kernel(unsigned ns) {
-    pdl_trigger(); pdl_wait();
-    unsigned long long t0, t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-    do {
-        __nanosleep(200);
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    } while (t - t0 < (unsigned long long)ns && t - t0 < 2000000ull);
-}
-
 struct GatherIdx { int idx[kVocMaxItems]; };
 __global__ void gather_rows_kernel(const float* __restrict__ src, const GatherIdx G, int width, float* __restrict__ dst) {
     const float* s = src + (size_t)G.idx[blockIdx.x] * width;
@@ -109,12 +92,9 @@ __global__ void gather_rows_kernel(const float* __restrict__ src, const GatherId
 template <typename TOut>
 __global__ void __launch_bounds__(256)
 layernorm_kernel(const float* __restrict__ X, const float* __restrict__ w, const float* __restrict__ b,
-                 TOut* __restrict__ Y, int H, float eps, const DepFlag dep) {
+                 TOut* __restrict__ Y, int H, float eps) {
     __shared__ float red[32];
-    trace_pt(TR_LN, 0); pdl_trigger();
-    if (threadIdx.x == 0) dep_wait(dep);
-    __syncthreads();
-    trace_pt(TR_LN, 1);
+    trace_pt(TR_LN, 0); pdl_trigger(); pdl_wait(); trace_pt(TR_LN, 1);
     const float* x = X + (size_t)blockIdx.x * H;
     float s = 0.f;
     for (int i = threadIdx.x; i < H; i += blockDim.x) s += x[i];
@@ -125,7 +105,6 @@ layernorm_kernel(const float* __restrict__ X, const float* __restrict__ w, const
     const float rstd = 1.0f / sqrtf(var + eps);
     TOut* y = Y + (size_t)blockIdx.x * H;
     for (int i = threadIdx.x; i < H; i += blockDim.x) y[i] = from_f32<TOut>((x[i] - mean) * rstd * w[i] + b[i]);
-    dep_arrive(dep, threadIdx.x == 0);
 }
 
 __device__ __forceinline__ void smem_layernorm(float* buf, const float* __restrict__ w, const float* __restrict__ b,
@@ -145,13 +124,10 @@ template <typename TOut>
 __global__ void __launch_bounds__(256)
 residual_reduce_ln_kernel(float* __restrict__ X, const float* __restrict__ P, int splits, size_t split_stride,
                           const float* __restrict__ bias, const float* __restrict__ w, const float* __restrict__ b,
-                          TOut* __restrict__ Y, int H, float eps, const DepFlag dep) {
+                          TOut* __restrict__ Y, int H, float eps) {
     extern __shared__ float buf[];
     __shared__ float red[32];
-    trace_pt(TR_REDUCE_LN, 0); pdl_trigger();
-    if (threadIdx.x == 0) dep_wait(dep);
-    __syncthreads();
-    trace_pt(TR_REDUCE_LN, 1);
+    trace_pt(TR_REDUCE_LN, 0); pdl_trigger(); pdl_wait(); trace_pt(TR_REDUCE_LN, 1);
     float* x = X + (size_t)blockIdx.x * H;
     const float* p = P + (size_t)blockIdx.x * H;
     // 16-byte lanes: with H = 1024 every thread owns one float4, so the residual, the bias and all split partials of the
@@ -170,11 +146,10 @@ residual_reduce_ln_kernel(float* __restrict__ X, const float* __restrict__ P, in
         *reinterpret_cast<float4*>(buf + c) = v;
     }
     __syncthreads();
-    if (Y == nullptr) { dep_arrive(dep, threadIdx.x == 0); return; }
+    if (Y == nullptr) return;
     smem_layernorm(buf, w, b, H, eps, red);
     TOut* y = Y + (size_t)blockIdx.x * H;
     for (int c = threadIdx.x; c < H; c += blockDim.x) y[c] = from_f32<TOut>(buf[c]);
-    dep_arrive(dep, threadIdx.x == 0);
     trace_pt(TR_REDUCE_LN, 2);
 }
 
@@ -281,7 +256,7 @@ template <typename TKV, typename TOut, int NW>
 __global__ void __launch_bounds__(32 * NW)
 attn_decode_kernel(const float* __restrict__ QKV, const int* __restrict__ active, const int* __restrict__ ctx_len,
                    const int* __restrict__ block_tables, int max_pages, TKV* __restrict__ kpool, TKV* __restrict__ vpool,
-                   TOut* __restrict__ out, int heads, int n_items, const DepFlag dep, int l2_pages) {
+                   TOut* __restrict__ out, int heads, int n_items) {
     constexpr int X = KVec<TKV>::X;
     constexpr int NCH = kHeadDim / X;                 // 16-byte atoms per token row (8 bf16 / 16 fp32)
     constexpr int TPI = 32 / NCH;                     // tokens covered by one warp-wide V load (4 / 2)
@@ -291,9 +266,8 @@ attn_decode_kernel(const float* __restrict__ QKV, const int* __restrict__ active
     __shared__ float pacc[NW][kHeadDim];
     trace_pt(TR_ATTN, 0); pdl_trigger();
     // ncu: 24 resident warps per SM, long-scoreboard stalls dominate: the kernel is bound by the bytes its warps keep in
-    // flight against ~1.6 us of HBM latency under load.  Option "attn_l2_pages": cp.async.bulk.prefetch.L2 holds no registers.
-    if (threadIdx.x == 0) dep_wait(dep);
-    __syncthreads();
+    // flight against ~1.6 us of HBM latency under load.
+    pdl_wait();
     trace_pt(TR_ATTN, 1);
     const int H = heads * kHeadDim;
     // work items = (active row, head); the grid may be capped below M*heads (engine option "attn_ctas_per_sm") so that the
@@ -304,23 +278,11 @@ attn_decode_kernel(const float* __restrict__ QKV, const int* __restrict__ active
     const int past = ctx_len[slot];                   // tokens already cached; the new one goes to position `past`
     const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
     const int* bt = block_tables + (size_t)slot * max_pages;
-    if (l2_pages > 0 && lane == 0) {
-        // ask L2 for this warp's pages 2 .. 1 + l2_pages now (its first page is loaded right away): kept out of the page
-        // loop, where the address arithmetic of a prefetch costs the 16 in-flight loads per lane their registers (69 -> 96)
-        const int np = (past + kPageTokens - 1) / kPageTokens;
-        for (int j = 1; j <= l2_pages; ++j) {
-            const int pf = w + j * NW;
-            if (pf >= np) break;
-            const size_t pb = ((size_t)bt[pf] * heads + h) * (kPageTokens * kHeadDim);
-            asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(kpool + pb), "r"((int)(kPageTokens * kHeadDim * sizeof(TKV))));
-            asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(vpool + pb), "r"((int)(min(kPageTokens, past - pf * kPageTokens) * kHeadDim * sizeof(TKV))));
-        }
-    }
     {
         const float* row = QKV + (size_t)i * 3 * H + h * kHeadDim;
         const int page = bt[past / kPageTokens], tk = past % kPageTokens;
         const size_t pbase = ((size_t)page * heads + h) * (kPageTokens * kHeadDim);
-        for (int t = tid; t < 2 * kHeadDim; t += 32 * NW) {              // (NW < 4: fewer than 128 threads stage the row)
+        for (int t = tid; t < 2 * kHeadDim; t += 32 * NW) {
             const int dd = t & 63;
             if (t < 64) {
                 qs[dd] = row[dd] * 0.125f;                                           // 64^-0.5
@@ -421,271 +383,6 @@ attn_decode_kernel(const float* __restrict__ QKV, const int* __restrict__ active
         out[(size_t)i * H + h * kHeadDim + t] = from_f32<TOut>(o / L);
     }
     __syncthreads();                                  // qs/ks/vs/pacc are reused by the next item
-    }
-    dep_arrive(dep, threadIdx.x == 0);
-    trace_pt(TR_ATTN, 2);
-}
-
-// ------------------------------------------------------------------------------------------------
-// Decode attention, bulk-copy form (16-bit caches): the cache pages of a (row, head) item are contiguous 4 KB blocks (K atoms,
-// V rows), so one producer thread streams them into a shared-memory ring with cp.async.bulk + mbarriers and four consumer warps
-// do the arithmetic of attn_decode_kernel<.., 4> out of shared memory (same page -> warp assignment, same operation order:
-// results are bit-identical).  Why:
-//   * bytes in flight no longer depend on resident warps: ONE 160-thread CTA per SM with an 8-stage ring keeps 64 KB per SM
-//     outstanding, so the kernel leaves registers, thread slots and ~160 KB of shared memory to the GEMM CTAs of the other
-//     decode branch (the load-into-registers kernel needs ~9 CTAs per SM to reach the same bandwidth and starves them);
-//   * the cached pages, block tables and context lengths of this step were written by EARLIER graph launches, so the producer
-//     starts streaming BEFORE griddepcontrol.wait — the ring is full when the QKV GEMM retires; only q and the step's own
-//     k/v (read from the QKV row) wait for the predecessor;
-//   * the producer walks straight from one item's pages into the next item's: no per-item ramp.
-// CTA c handles items c, c + grid, ... (at most kBulkMaxItems of them; the host sizes the grid accordingly).
-// ------------------------------------------------------------------------------------------------
-constexpr int kBulkMaxItems = 32;
-constexpr int kBulkStageBytes = 2 * kPageTokens * kHeadDim * 2;       // K page + V page, 16-bit: 8 KB
-
-__device__ __forceinline__ uint32_t ab_s32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void ab_bar_init(uint64_t* b, uint32_t c) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(ab_s32(b)), "r"(c) : "memory");
-}
-__device__ __forceinline__ void ab_bar_arrive(uint64_t* b) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(ab_s32(b)) : "memory");
-}
-__device__ __forceinline__ void ab_bar_expect_tx(uint64_t* b, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(ab_s32(b)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void ab_bar_wait(uint64_t* b, uint32_t parity, int tag) {
-    const long long t0 = clock64();
-    int polls = 0;
-    for (;;) {
-        uint32_t ok;
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(ok) : "r"(ab_s32(b)), "r"(parity) : "memory");
-        if (ok) return;
-        if ((++polls & 1023) == 0 && clock64() - t0 > 4000000000LL) {
-            printf("attn_decode_bulk: mbarrier watchdog (tag %d, block %d, thread %d)\n", tag, blockIdx.x, threadIdx.x);
-            __trap();
-        }
-    }
-}
-__device__ __forceinline__ void ab_bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(ab_s32(dst)), "l"(src), "r"(bytes), "r"(ab_s32(bar)) : "memory");
-}
-template <int NW> __device__ __forceinline__ void ab_consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(32 * NW) : "memory"); }
-
-template <typename TKV, typename TOut, int NW>
-__global__ void __launch_bounds__(32 * NW + 32)
-attn_decode_bulk_kernel(const float* __restrict__ QKV, const int* __restrict__ active, const int* __restrict__ ctx_len,
-                        const int* __restrict__ block_tables, int max_pages, TKV* __restrict__ kpool, TKV* __restrict__ vpool,
-                        TOut* __restrict__ out, int heads, int n_items, int stages, int l2_ahead) {
-    static_assert(sizeof(TKV) == 2, "bulk attention: 16-bit caches only");
-    constexpr int X = 8, NCH = 8, TPI = 4, VIT = 8;
-    extern __shared__ __align__(128) uint8_t ring[];                  // stages x (K page | V page)
-    __shared__ __align__(8) uint64_t full_bar[24], empty_bar[24];
-    __shared__ int s_slot[kBulkMaxItems], s_past[kBulkMaxItems];
-    __shared__ __align__(16) float qs[2][kHeadDim], ks[2][kHeadDim], vs[2][kHeadDim];
-    static_assert(NW == 4 || NW == 8 || NW == 16, "consumer warps: 4, 8 or 16");
-    __shared__ float pm[NW], pl[NW];
-    __shared__ float pacc[NW][kHeadDim];
-    const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-    trace_pt(TR_ATTN, 0); pdl_trigger();
-    const int my_items = (blockIdx.x < n_items) ? (n_items - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-    if (tid < kBulkMaxItems && tid < my_items) {                      // written by earlier graph launches: safe before the wait
-        const int item = blockIdx.x + tid * gridDim.x;
-        const int slot = active[item / heads];
-        s_slot[tid] = slot; s_past[tid] = ctx_len[slot];
-    }
-    if (tid == 0)
-        for (int s = 0; s < stages; ++s) { ab_bar_init(&full_bar[s], 1); ab_bar_init(&empty_bar[s], 1); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    __syncthreads();
-    const int H = heads * kHeadDim;
-
-    const int D = stages / NW;                                        // ring depth per consumer warp
-    if (w == NW) {
-        // ------------------------------------------------------------ producer warp: one bulk copy per K page, one per V page.
-        // Page pg of an item belongs to consumer warp pg % 4 and goes to that warp's own D-deep sub-ring, so every stage is
-        // always drained by the same warp, in order (an mbarrier parity wait can only tell the current phase from the previous
-        // one).  A single thread issues ~one 4 KB copy per 270 cycles (29 GB/s per SM, tools/probes/bulk_probe.cu), so up to
-        // `stages` lanes issue at once, each for the page whose id it read from the block table; rounds of `stages` pages keep
-        // every empty-barrier wait at most one phase ahead.
-        uint32_t handed = 0;                                          // lane w < NW: pages handed to consumer warp w so far
-        // HBM latency under load is ~1.6 us: 64 KB per SM in flight reach only ~39 GB/s per SM.  The ring therefore only covers
-        // the L2 -> shared latency; HBM -> L2 runs one item ahead on cp.async.bulk.prefetch.L2 (no SM resources held).
-        auto prefetch_item = [&](int k) {
-            const int item = blockIdx.x + k * gridDim.x;
-            const int h = item % heads;
-            const int past = s_past[k];
-            const int npages = (past + kPageTokens - 1) / kPageTokens;
-            const int* bt = block_tables + (size_t)s_slot[k] * max_pages;
-            for (int pg = lane; pg < npages; pg += 32) {
-                const size_t pbase = ((size_t)bt[pg] * heads + h) * (kPageTokens * kHeadDim);
-                const int nvalid = min(kPageTokens, past - pg * kPageTokens);
-                asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(kpool + pbase), "r"(kPageTokens * kHeadDim * 2) : "memory");
-                asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(vpool + pbase), "r"(nvalid * kHeadDim * 2) : "memory");
-            }
-        };
-        if (l2_ahead && my_items > 0) prefetch_item(0);
-        for (int k = 0; k < my_items; ++k) {
-            const int item = blockIdx.x + k * gridDim.x;
-            const int h = item % heads;
-            const int slot = s_slot[k], past = s_past[k];
-            const int npages = (past + kPageTokens - 1) / kPageTokens;
-            const int* bt = block_tables + (size_t)slot * max_pages;
-            if (l2_ahead && k + 1 < my_items) prefetch_item(k + 1);
-            for (int pg0 = 0; pg0 < npages; pg0 += 32) {
-                const int n = min(32, npages - pg0);
-                const int page = (lane < n) ? bt[pg0 + lane] : 0;     // one coalesced read per 32 pages
-                const int wt = lane % NW;                             // (pg0 is a multiple of 32, 32 % NW == 0)
-                const uint32_t pos = __shfl_sync(0xffffffffu, handed, wt) + (uint32_t)(lane / NW);
-                for (int r = 0; r * stages < n; ++r) {
-                    if (lane < n && lane / stages == r) {
-                        const int s = wt * D + (int)(pos % D);
-                        ab_bar_wait(&empty_bar[s], ((pos / D) & 1) ^ 1, 1);
-                        const int nvalid = min(kPageTokens, past - (pg0 + lane) * kPageTokens);
-                        const size_t pbase = ((size_t)page * heads + h) * (kPageTokens * kHeadDim);
-                        uint8_t* dst = ring + (size_t)s * kBulkStageBytes;
-                        ab_bar_expect_tx(&full_bar[s], (uint32_t)(kPageTokens * kHeadDim * 2 + nvalid * kHeadDim * 2));
-                        ab_bulk_g2s(dst, kpool + pbase, kPageTokens * kHeadDim * 2, &full_bar[s]);
-                        ab_bulk_g2s(dst + kPageTokens * kHeadDim * 2, vpool + pbase, (uint32_t)(nvalid * kHeadDim * 2), &full_bar[s]);
-                    }
-                    __syncwarp();
-                }
-                if (lane < NW) handed += (uint32_t)((n + NW - 1 - lane) / NW);
-            }
-        }
-        return;
-    }
-
-    // ---------------------------------------------------------------- consumers: 4 warps, pages round-robin inside an item
-    pdl_wait();                                                       // QKV of this step; `out` may still be read upstream
-    trace_pt(TR_ATTN, 1);
-    // stage item k's row (q scaled, k / v rounded to the cache type) and append k / v to the cache: thread t < 64 owns q[t]
-    // and v[t], thread t >= 64 owns k[t - 64]
-    auto load_row = [&](int k, float& a, float& b) {
-        const int item = blockIdx.x + k * gridDim.x;
-        const int i = item / heads, h = item - i * heads;
-        const float* row = QKV + (size_t)i * 3 * H + h * kHeadDim;
-        if (tid < 64) { a = row[tid]; b = row[2 * H + tid]; } else if (tid < 128) { a = row[H + tid - 64]; b = 0.f; }
-    };
-    auto stage_row = [&](int k, int buf, float a, float b, int page_new) {
-        const int item = blockIdx.x + k * gridDim.x;
-        const int h = item % heads;
-        const int tk = s_past[k] % kPageTokens;
-        const size_t pbase = ((size_t)page_new * heads + h) * (kPageTokens * kHeadDim);
-        if (tid < 64) {
-            qs[buf][tid] = a * 0.125f;                                               // 64^-0.5
-            const TKV v = from_f32<TKV>(b);
-            vs[buf][tid] = to_f32<TKV>(v);
-            vpool[pbase + (size_t)tk * kHeadDim + tid] = v;
-        } else if (tid < 128) {
-            const int dd = tid - 64;
-            const TKV kk = from_f32<TKV>(a);
-            ks[buf][dd] = to_f32<TKV>(kk);
-            kpool[pbase + ((size_t)(dd / X) * kPageTokens + tk) * X + (dd % X)] = kk;
-        }
-    };
-    float ra = 0.f, rb = 0.f; int rpage = 0;
-    if (my_items > 0) {
-        load_row(0, ra, rb);
-        rpage = block_tables[(size_t)s_slot[0] * max_pages + s_past[0] / kPageTokens];
-        stage_row(0, 0, ra, rb, rpage);
-    }
-    ab_consumer_sync<NW>();
-    uint32_t mypos = 0;                                               // pages this warp has drained (its sub-ring position)
-    const int tg = lane / NCH, dc = lane % NCH;                       // PV role of this lane: token group, dim chunk
-    for (int k = 0; k < my_items; ++k) {
-        const int buf = k & 1;
-        const int item = blockIdx.x + k * gridDim.x;
-        const int i = item / heads, h = item - i * heads;
-        const int past = s_past[k];
-        const int npages = (past + kPageTokens - 1) / kPageTokens;
-        if (k + 1 < my_items) {                                       // next item's row + page id: in flight during this item
-            load_row(k + 1, ra, rb);
-            rpage = block_tables[(size_t)s_slot[k + 1] * max_pages + s_past[k + 1] / kPageTokens];
-        }
-        float m = -INFINITY, l = 0.f;
-        float acc[X];
-#pragma unroll
-        for (int e = 0; e < X; ++e) acc[e] = 0.f;
-        for (int pg = w; pg < npages; pg += NW, ++mypos) {
-            const int s = w * D + (int)(mypos % D);
-            ab_bar_wait(&full_bar[s], (mypos / D) & 1, 2);
-            const uint8_t* st = ring + (size_t)s * kBulkStageBytes;
-            const int nvalid = min(kPageTokens, past - pg * kPageTokens);
-            uint4 kraw[NCH], vraw[VIT];
-#pragma unroll
-            for (int cc = 0; cc < NCH; ++cc) kraw[cc] = *reinterpret_cast<const uint4*>(st + ((size_t)cc * kPageTokens + lane) * 16);
-#pragma unroll
-            for (int it = 0; it < VIT; ++it)                          // rows >= nvalid were not copied: never multiplied in
-                vraw[it] = *reinterpret_cast<const uint4*>(st + kPageTokens * kHeadDim * 2 + ((size_t)(it * TPI + tg) * kHeadDim + dc * X) * 2);
-            __syncwarp();
-            if (lane == 0) ab_bar_arrive(&empty_bar[s]);              // the page is in registers: hand the slot back
-            float sc = 0.f;
-#pragma unroll
-            for (int cc = 0; cc < NCH; ++cc) {
-                float kf[X];
-                KVec<TKV>::unpack(kraw[cc], kf);
-#pragma unroll
-                for (int e = 0; e < X; ++e) sc = fmaf(kf[e], qs[buf][cc * X + e], sc);
-            }
-            const bool valid = lane < nvalid;
-            sc = valid ? sc : -INFINITY;
-            const float mnew = fmaxf(m, warp_max(sc));
-            const float p = valid ? expf(sc - mnew) : 0.f;
-            const float corr = (m == -INFINITY) ? 0.f : expf(m - mnew);
-            l = l * corr + warp_sum(p);
-#pragma unroll
-            for (int e = 0; e < X; ++e) acc[e] *= corr;
-#pragma unroll
-            for (int it = 0; it < VIT; ++it) {
-                const int j = it * TPI + tg;
-                const float pj = __shfl_sync(0xffffffffu, p, j);
-                if (j < nvalid) {
-                    float vf[X];
-                    KVec<TKV>::unpack(vraw[it], vf);
-#pragma unroll
-                    for (int e = 0; e < X; ++e) acc[e] = fmaf(pj, vf[e], acc[e]);
-                }
-            }
-            m = mnew;
-        }
-        if (w == 0) {                                                 // the step's own token, from shared memory
-            float sc = qs[buf][lane] * ks[buf][lane] + qs[buf][lane + 32] * ks[buf][lane + 32];
-            sc = warp_sum(sc);
-            const float mnew = fmaxf(m, sc);
-            const float p = expf(sc - mnew);
-            const float corr = (m == -INFINITY) ? 0.f : expf(m - mnew);
-            l = l * corr + p;
-#pragma unroll
-            for (int e = 0; e < X; ++e) acc[e] = acc[e] * corr + ((tg == 0) ? p * vs[buf][dc * X + e] : 0.f);
-            m = mnew;
-        }
-#pragma unroll
-        for (int o = NCH; o < 32; o <<= 1)
-#pragma unroll
-            for (int e = 0; e < X; ++e) acc[e] += __shfl_xor_sync(0xffffffffu, acc[e], o);
-        if (lane == 0) { pm[w] = m; pl[w] = l; }
-        if (lane < NCH) {
-#pragma unroll
-            for (int e = 0; e < X; ++e) pacc[w][dc * X + e] = acc[e];
-        }
-        ab_consumer_sync<NW>();
-        if (tid < kHeadDim) {
-            float M = pm[0];
-#pragma unroll
-            for (int q = 1; q < NW; ++q) M = fmaxf(M, pm[q]);
-            float L = 0.f, o = 0.f;
-#pragma unroll
-            for (int q = 0; q < NW; ++q) {
-                const float e = (pm[q] == -INFINITY) ? 0.f : expf(pm[q] - M);
-                L = fmaf(pl[q], e, L);
-                o = fmaf(pacc[q][tid], e, o);
-            }
-            out[(size_t)i * H + h * kHeadDim + tid] = from_f32<TOut>(o / L);
-        }
-        if (k + 1 < my_items) stage_row(k + 1, buf ^ 1, ra, rb, rpage);
-        ab_consumer_sync<NW>();                                           // next row staged; pm / pl / pacc free again
     }
     trace_pt(TR_ATTN, 2);
 }
@@ -1097,12 +794,6 @@ void launch_init_slots(const SlotInit* init, const int* pages, int n, SlotArrays
     COUNT_LAUNCH(); KERNEL_CHECK();
 }
 
-void launch_stream_delay(unsigned ns, cudaStream_t st, bool pdl) {
-    if (ns == 0) return;
-    launch_k(stream_delay_kernel, dim3(1), dim3(32), 0, st, pdl, ns);
-    COUNT_LAUNCH(); KERNEL_CHECK();
-}
-
 void launch_gather_rows(const float* src, const int* idx_host, int n, int width, float* dst, cudaStream_t st) {
     if (n <= 0) return;
     if (n > kVocMaxItems) throw CudaError("gather_rows: too many rows");
@@ -1121,36 +812,36 @@ void launch_build_rows(const RowDesc* rows, int n_rows, GptTables t, float* X, c
 }
 
 void launch_build_decode_rows(const int* active, int M, const int* last_tok, const int* n_gen, GptTables t,
-                              float* X, cudaStream_t st, bool pdl, unsigned* flags, int n_flags) {
+                              float* X, cudaStream_t st, bool pdl) {
     if (M <= 0) return;
     ProfScope ps(KF_EMBED, st, 0, 12.0 * M * t.H);
-    launch_k(build_decode_rows_kernel, dim3(M), dim3(256), 0, st, pdl, active, last_tok, n_gen, t, X, flags, flags ? n_flags : 0);
+    launch_k(build_decode_rows_kernel, dim3(M), dim3(256), 0, st, pdl, active, last_tok, n_gen, t, X);
     COUNT_LAUNCH(); KERNEL_CHECK();
 }
 
 template <typename TOut>
 void launch_layernorm(const float* X, const float* w, const float* b, TOut* Y, int M, int H, float eps,
-                      cudaStream_t st, bool pdl, DepFlag dep) {
+                      cudaStream_t st, bool pdl) {
     if (M <= 0) return;
     ProfScope ps(KF_NORM, st, 0, (4.0 + sizeof(TOut)) * M * H);
-    launch_k(layernorm_kernel<TOut>, dim3(M), dim3(256), 0, st, pdl, X, w, b, Y, H, eps, dep);
+    launch_k(layernorm_kernel<TOut>, dim3(M), dim3(256), 0, st, pdl, X, w, b, Y, H, eps);
     COUNT_LAUNCH(); KERNEL_CHECK();
 }
-template void launch_layernorm<float>(const float*, const float*, const float*, float*, int, int, float, cudaStream_t, bool, DepFlag);
-template void launch_layernorm<__nv_bfloat16>(const float*, const float*, const float*, __nv_bfloat16*, int, int, float, cudaStream_t, bool, DepFlag);
-template void launch_layernorm<__half>(const float*, const float*, const float*, __half*, int, int, float, cudaStream_t, bool, DepFlag);
+template void launch_layernorm<float>(const float*, const float*, const float*, float*, int, int, float, cudaStream_t, bool);
+template void launch_layernorm<__nv_bfloat16>(const float*, const float*, const float*, __nv_bfloat16*, int, int, float, cudaStream_t, bool);
+template void launch_layernorm<__half>(const float*, const float*, const float*, __half*, int, int, float, cudaStream_t, bool);
 
 template <typename TOut>
 void launch_residual_reduce_layernorm(float* X, const float* partials, int splits, const float* bias, const float* w,
-                                      const float* b, TOut* Y, int M, int H, float eps, cudaStream_t st, bool pdl, DepFlag dep) {
+                                      const float* b, TOut* Y, int M, int H, float eps, cudaStream_t st, bool pdl) {
     if (M <= 0) return;
     ProfScope ps(KF_NORM, st, 0, (8.0 + 4.0 * splits + sizeof(TOut)) * M * H);
-    launch_k(residual_reduce_ln_kernel<TOut>, dim3(M), dim3(256), H * sizeof(float), st, pdl, X, partials, splits, (size_t)M * H, bias, w, b, Y, H, eps, dep);
+    launch_k(residual_reduce_ln_kernel<TOut>, dim3(M), dim3(256), H * sizeof(float), st, pdl, X, partials, splits, (size_t)M * H, bias, w, b, Y, H, eps);
     COUNT_LAUNCH(); KERNEL_CHECK();
 }
-template void launch_residual_reduce_layernorm<float>(float*, const float*, int, const float*, const float*, const float*, float*, int, int, float, cudaStream_t, bool, DepFlag);
-template void launch_residual_reduce_layernorm<__nv_bfloat16>(float*, const float*, int, const float*, const float*, const float*, __nv_bfloat16*, int, int, float, cudaStream_t, bool, DepFlag);
-template void launch_residual_reduce_layernorm<__half>(float*, const float*, int, const float*, const float*, const float*, __half*, int, int, float, cudaStream_t, bool, DepFlag);
+template void launch_residual_reduce_layernorm<float>(float*, const float*, int, const float*, const float*, const float*, float*, int, int, float, cudaStream_t, bool);
+template void launch_residual_reduce_layernorm<__nv_bfloat16>(float*, const float*, int, const float*, const float*, const float*, __nv_bfloat16*, int, int, float, cudaStream_t, bool);
+template void launch_residual_reduce_layernorm<__half>(float*, const float*, int, const float*, const float*, const float*, __half*, int, int, float, cudaStream_t, bool);
 
 template <typename TOut>
 void launch_head_norms(const float* X, const int* row_index, const float* lnf_w, const float* lnf_b,
@@ -1181,10 +872,10 @@ template void launch_kv_write<__nv_bfloat16>(const float*, int, const int*, cons
 template void launch_kv_write<__half>(const float*, int, const int*, const int*, const int*, const int*, int, __half*, __half*, int, cudaStream_t);
 
 template <typename TKV, typename TOut>
-int launch_attn_decode(const float* QKV, const int* active, int M, const int* ctx_len, const int* block_tables,
+void launch_attn_decode(const float* QKV, const int* active, int M, const int* ctx_len, const int* block_tables,
                         int max_pages, TKV* kpool, TKV* vpool, TOut* out, int heads, cudaStream_t st,
-                        double ctx_sum_hint, bool pdl, DepFlag dep) {
-    if (M <= 0) return 0;
+                        double ctx_sum_hint, bool pdl) {
+    if (M <= 0) return;
     // algorithmic bytes: K and V of every cached token of every sequence, once
     ProfScope ps(KF_ATTN_DECODE, st, 4.0 * ctx_sum_hint * heads * kHeadDim,
                  2.0 * ctx_sum_hint * heads * kHeadDim * sizeof(TKV));
@@ -1195,60 +886,13 @@ int launch_attn_decode(const float* QKV, const int* active, int M, const int* ct
     } else if (g_attn_ctas_per_sm < 0) {
         grid = std::min(n_items, -g_attn_ctas_per_sm);          // test hook: an absolute grid size
     }
-    if constexpr (sizeof(TKV) == 2) {
-        if (g_attn_bulk > 0 && dep.wait == nullptr && dep.arrive == nullptr) {
-            // bulk-copy form: `attn_bulk` persistent CTAs per SM, each with an `attn_stages`-deep ring of 8 KB pages
-            int g = std::min(n_items, sm_count() * g_attn_bulk);
-            if (g_attn_ctas_per_sm < 0) g = std::min(n_items, -g_attn_ctas_per_sm);          // test hook: an absolute grid size
-            g = std::max(g, ceil_div(n_items, kBulkMaxItems));
-            // consumer warps per CTA = option "attn_warps" (4 / 8 / 16; same page -> warp assignment and combination order as
-            // attn_decode_kernel<.., NW>); ring = one sub-ring of attn_stages / NW pages per consumer warp
-            const int nw = (g_attn_warps == 8 || g_attn_warps == 16) ? g_attn_warps : 4;
-            const int depth = std::max(1, std::min(g_attn_stages / nw, 24 / nw));
-            const int stages = nw * depth;
-            const size_t smem = (size_t)stages * kBulkStageBytes;
-            static bool attr[64] = {};
-            if (first_on_device(attr)) {
-                CUDA_CHECK(cudaFuncSetAttribute(attn_decode_bulk_kernel<TKV, TOut, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 24 * kBulkStageBytes));
-                CUDA_CHECK(cudaFuncSetAttribute(attn_decode_bulk_kernel<TKV, TOut, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 24 * kBulkStageBytes));
-                CUDA_CHECK(cudaFuncSetAttribute(attn_decode_bulk_kernel<TKV, TOut, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 24 * kBulkStageBytes));
-            }
-            auto go = [&](auto kern) {
-                launch_k(kern, dim3(g), dim3(32 * nw + 32), smem, st, pdl, QKV, active, ctx_len, block_tables, max_pages,
-                         kpool, vpool, out, heads, n_items, stages, g_attn_l2_ahead);
-            };
-            if (nw == 16) go(attn_decode_bulk_kernel<TKV, TOut, 16>);
-            else if (nw == 8) go(attn_decode_bulk_kernel<TKV, TOut, 8>);
-            else go(attn_decode_bulk_kernel<TKV, TOut, 4>);
-            COUNT_LAUNCH(); KERNEL_CHECK();
-            return g;
-        }
-    }
-    // warps per (row, head) item: the cache pages of an item are dealt round-robin to its warps.  4 is the default; 8 (engine
-    // option "attn_warps", bf16 only) halves an item's latency and was meant to shorten the under-filled tail of the kernel —
-    // measured 18 % SLOWER per decode step (run 7: 256-thread CTAs, three per SM), kept as an option.
-    const int l2_pages = (sizeof(TKV) == 2) ? g_attn_l2_pages : 0;
-    if (sizeof(TKV) == 2 && g_attn_warps == 16)
-        launch_k(attn_decode_kernel<TKV, TOut, 16>, dim3(grid), dim3(512), 0, st, pdl, QKV, active, ctx_len, block_tables, max_pages,
-                 kpool, vpool, out, heads, n_items, dep, l2_pages);
-    else if (sizeof(TKV) == 2 && g_attn_warps == 8)
-        launch_k(attn_decode_kernel<TKV, TOut, 8>, dim3(grid), dim3(256), 0, st, pdl, QKV, active, ctx_len, block_tables, max_pages,
-                 kpool, vpool, out, heads, n_items, dep, l2_pages);
-    else if (sizeof(TKV) == 2 && g_attn_warps == 2)
-        launch_k(attn_decode_kernel<TKV, TOut, 2>, dim3(grid), dim3(64), 0, st, pdl, QKV, active, ctx_len, block_tables, max_pages,
-                 kpool, vpool, out, heads, n_items, dep, l2_pages);
-    else if (sizeof(TKV) == 2 && g_attn_warps == 1)
-        launch_k(attn_decode_kernel<TKV, TOut, 1>, dim3(grid), dim3(32), 0, st, pdl, QKV, active, ctx_len, block_tables, max_pages,
-                 kpool, vpool, out, heads, n_items, dep, l2_pages);
-    else
-        launch_k(attn_decode_kernel<TKV, TOut, 4>, dim3(grid), dim3(128), 0, st, pdl, QKV, active, ctx_len, block_tables, max_pages,
-                 kpool, vpool, out, heads, n_items, dep, l2_pages);
+    launch_k(attn_decode_kernel<TKV, TOut, 4>, dim3(grid), dim3(128), 0, st, pdl, QKV, active, ctx_len, block_tables, max_pages,
+             kpool, vpool, out, heads, n_items);
     COUNT_LAUNCH(); KERNEL_CHECK();
-    return grid;
 }
-template int launch_attn_decode<float, float>(const float*, const int*, int, const int*, const int*, int, float*, float*, float*, int, cudaStream_t, double, bool, DepFlag);
-template int launch_attn_decode<__nv_bfloat16, __nv_bfloat16>(const float*, const int*, int, const int*, const int*, int, __nv_bfloat16*, __nv_bfloat16*, __nv_bfloat16*, int, cudaStream_t, double, bool, DepFlag);
-template int launch_attn_decode<__half, __half>(const float*, const int*, int, const int*, const int*, int, __half*, __half*, __half*, int, cudaStream_t, double, bool, DepFlag);
+template void launch_attn_decode<float, float>(const float*, const int*, int, const int*, const int*, int, float*, float*, float*, int, cudaStream_t, double, bool);
+template void launch_attn_decode<__nv_bfloat16, __nv_bfloat16>(const float*, const int*, int, const int*, const int*, int, __nv_bfloat16*, __nv_bfloat16*, __nv_bfloat16*, int, cudaStream_t, double, bool);
+template void launch_attn_decode<__half, __half>(const float*, const int*, int, const int*, const int*, int, __half*, __half*, __half*, int, cudaStream_t, double, bool);
 
 template <typename TOut>
 void launch_attn_generic(AttnLayout L, const AttnSeq* seqs, int nseq, int max_nq, TOut* out, int out_row_stride,

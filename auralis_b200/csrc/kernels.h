@@ -12,7 +12,7 @@ namespace xtts {
 //          GEMM_RESID -> out = resid + (...)   (resid may alias out)
 // ------------------------------------------------------------------------------------------
 // GEMM_OUT_BF16: 16-bit output in the operand format;  GEMM_F16: the 16-bit operands (and that output) are IEEE fp16, not bf16
-enum : int { GEMM_GELU = 1, GEMM_RESID = 2, GEMM_OUT_BF16 = 4, GEMM_F16 = 8, GEMM_NO_L2PF = 16 /* internal: engine option gemm_l2_prefetch = 0 */ };
+enum : int { GEMM_GELU = 1, GEMM_RESID = 2, GEMM_OUT_BF16 = 4, GEMM_F16 = 8 };
 
 // fp32 CUDA-core path (parity mode; also the GPU-side reference for the tensor-core path)
 void launch_gemm_f32(const float* A, const float* W, const float* bias, const float* resid, float* out,
@@ -22,32 +22,15 @@ void launch_gemm_f32(const float* A, const float* W, const float* bias, const fl
 // out is fp32 unless GEMM_OUT_BF16.  K % 64 == 0, N % 32 == 0 required.
 // `pdl`: launch with the programmatic-dependent-launch attribute (decode chain); every kernel that can be launched
 // that way executes griddepcontrol.wait before touching its predecessor's outputs
-// `dep` (decode chain): wait / arrive counters instead of griddepcontrol.wait (common.cuh).  Returns the number of CTAs
-// launched = the value the kernel's arrive counter reaches (0 when the launch went to the wide-tile kernel).
-int launch_gemm_bf16_tc(const __nv_bfloat16* A, const __nv_bfloat16* W, const float* bias, const float* resid,
-                        void* out, int M, int N, int K, int flags, cudaStream_t st, bool pdl = false, DepFlag dep = DepFlag());
+void launch_gemm_bf16_tc(const __nv_bfloat16* A, const __nv_bfloat16* W, const float* bias, const float* resid,
+                         void* out, int M, int N, int K, int flags, cudaStream_t st, bool pdl = false);
 // large-shape path (gemm_wgmma_wide.cu): persistent CTAs, 128 x 256 tiles
 bool gemm_wide_supported(int M, int N, int K);
 void launch_gemm_bf16_wide(const __nv_bfloat16* A, const __nv_bfloat16* W, const float* bias, const float* resid,
                            void* out, int M, int N, int K, int flags, cudaStream_t st);
-int launch_gemm_bf16_tc_splitk(const __nv_bfloat16* A, const __nv_bfloat16* W, float* partials, int M, int N, int K,
-                               int splits, cudaStream_t st, bool pdl = false, DepFlag dep = DepFlag(), int flags = 0);
+void launch_gemm_bf16_tc_splitk(const __nv_bfloat16* A, const __nv_bfloat16* W, float* partials, int M, int N, int K,
+                                int splits, cudaStream_t st, bool pdl = false, int flags = 0);
 
-// Fused decode chain (gemm_wgmma.cu): one persistent launch runs, for one layer boundary of the decode step,
-//   proj (split-K) -> residual+LN2 -> fc+gelu -> fc2 (split-K) -> residual+LN1(next layer) -> qkv(next layer)
-// with device-wide barriers between the phases.  `phases` selects a contiguous subset (DC_* bits).
-enum { DC_PROJ = 1, DC_LN2 = 2, DC_FC = 4, DC_FC2 = 8, DC_LN1 = 16, DC_QKV = 32 };
-struct DecodeChainArgs {
-    int phases, M, H, FF;
-    float eps;
-    const __nv_bfloat16* ATT; const __nv_bfloat16* Wo; const __nv_bfloat16* Wfc; const __nv_bfloat16* Wproj; const __nv_bfloat16* Wqkv;
-    const float* proj_bias; const float* ln2_w; const float* ln2_b; const float* fc_bias; const float* fc2_bias;
-    const float* ln1_w; const float* ln1_b; const float* qkv_bias;
-    float* X; __nv_bfloat16* Xn; __nv_bfloat16* FFb; float* QKV; float* PART;
-    unsigned* sync;          // 64 words, zero-initialised once, owned by the chain kernel (self-resetting barrier)
-};
-bool decode_chain_supported(int M, int H, int FF);
-void launch_decode_chain(const DecodeChainArgs& a, cudaStream_t st, bool pdl);
 bool gemm_tc_init(std::string* err);   // resolves cuTensorMapEncodeTiled; false -> err filled
 // TMA descriptor of a row-major 16-bit matrix [rows, cols]: boxes of 64 columns (128 B, SWIZZLE_128B) x box_rows rows, the
 // operand image the wgmma kernels read (gemm_wgmma.cu, gemm_wgmma_wide.cu); rows past the end are zero-filled
@@ -80,20 +63,18 @@ struct GptTables {        // embedding tables (device, fp32)
 
 void launch_build_rows(const RowDesc* rows, int n_rows, GptTables t, float* X, cudaStream_t st);
 // decode input rows: X[i] = wte[last_tok[slot]] + wpe[n_gen[slot]],  slot = active[i]
-// (also zeroes `n_flags` dependency counters at `flags`: the step's first kernel, behind a full dependency wait)
 void launch_build_decode_rows(const int* active, int M, const int* last_tok, const int* n_gen, GptTables t,
-                              float* X, cudaStream_t st, bool pdl = false, unsigned* flags = nullptr, int n_flags = 0);
+                              float* X, cudaStream_t st, bool pdl = false);
 
 template <typename TOut>
 void launch_layernorm(const float* X, const float* w, const float* b, TOut* Y, int M, int H, float eps,
-                      cudaStream_t st, bool pdl = false, DepFlag dep = DepFlag());
+                      cudaStream_t st, bool pdl = false);
 
 // X[m] += bias + sum_z partials[z][m]  (deterministic split-K reduction fused with the residual add), then
 // Y[m] = LN(X[m]) when Y != nullptr  (the following block's LayerNorm)
 template <typename TOut>
 void launch_residual_reduce_layernorm(float* X, const float* partials, int splits, const float* bias, const float* w,
-                                      const float* b, TOut* Y, int M, int H, float eps, cudaStream_t st, bool pdl = false,
-                                      DepFlag dep = DepFlag());
+                                      const float* b, TOut* Y, int M, int H, float eps, cudaStream_t st, bool pdl = false);
 
 // y = LN_fn(LN_lnf(X[row_index[i]]));  Y[i] = y (GEMM operand);
 // latents[slots[i]][lat_pos ? lat_pos[i] : n_gen[slots[i]]] = LN_fn(y)
@@ -112,11 +93,10 @@ void launch_kv_write(const float* QKV, int M, const int* row_slot, const int* ro
 
 // decode attention over the paged cache, ctx = ctx_len[slot] + 1.  The kernel also appends the new token's K/V
 // (read from the QKV row) to the cache — the reshape_and_cache step — so no separate kv_write launch is needed.
-// returns the number of CTAs launched
 template <typename TKV, typename TOut>
-int launch_attn_decode(const float* QKV, const int* active, int M, const int* ctx_len,
-                       const int* block_tables, int max_pages, TKV* kpool, TKV* vpool,
-                       TOut* out, int heads, cudaStream_t st, double ctx_sum_hint = 0, bool pdl = false, DepFlag dep = DepFlag());
+void launch_attn_decode(const float* QKV, const int* active, int M, const int* ctx_len,
+                        const int* block_tables, int max_pages, TKV* kpool, TKV* vpool,
+                        TOut* out, int heads, cudaStream_t st, double ctx_sum_hint = 0, bool pdl = false);
 
 struct AttnSeq { int q_start, nq, kv_start, nk; };
 struct AttnLayout {
@@ -273,8 +253,6 @@ struct SlotArrays {       // per-slot device arrays (mutable view of SampleState
 };
 // pages: [n][max_pages] page ids of each sequence (first n_pages valid)
 void launch_init_slots(const SlotInit* init, const int* pages, int n, SlotArrays a, cudaStream_t st);
-// occupies `st` for ns nanoseconds (branch stagger of the decode step, see gpt_kernels.cu)
-void launch_stream_delay(unsigned ns, cudaStream_t st, bool pdl = false);
 // dst[i][0..width) = src[idx[i]][0..width)   (i < n <= kVocMaxItems): speaker-bias rows of a vocoder batch
 void launch_gather_rows(const float* src, const int* idx_host, int n, int width, float* dst, cudaStream_t st);
 // y[c] = W[c,:] . g + b[c]   (speaker conditioning 1x1 convs)

@@ -194,12 +194,12 @@ def load_library(path: Optional[str] = None):
     lib.xtts_debug_conv_tc.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, i32p, f32p, f32p, f32p, i32, f32p, f32p, i32,
                                        C.c_float, C.c_float, i32, f32p, f32p]
     u32p = C.POINTER(C.c_uint32)
-    lib.xtts_debug_ln_gemm.argtypes = [vp, i32, i32, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, f32p, i32, f32p, f32p, i32p, u32p]
+    lib.xtts_debug_ln_gemm.argtypes = [vp, i32, i32, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, f32p, i32, f32p, f32p]
     lib.xtts_debug_norms.argtypes = [vp, i32, i32, i32, f32p, i32, i32p, f32p, f32p, f32p, f32p, f32p, f32p, i32, i32, i32p, i32p,
                                      i32p]
     lib.xtts_debug_kv_write.argtypes = [vp, i32, i32, i32, f32p, i32p, i32p, i32, i32p, i32p, i32, i32, vp, vp]
     lib.xtts_debug_build_rows.argtypes = [vp, i32, i32, f32p, i32, f32p, i32, f32p, i32, f32p, i32, f32p, i32, i32p, i32, f32p]
-    lib.xtts_debug_build_decode_rows.argtypes = [vp, i32, f32p, i32, f32p, i32, i32, i32p, i32, i32p, i32p, f32p, u32p, i32, i32]
+    lib.xtts_debug_build_decode_rows.argtypes = [vp, i32, f32p, i32, f32p, i32, i32, i32p, i32, i32p, i32p, f32p]
     lib.xtts_debug_beam_step.argtypes = [vp, i32, i32, i32, i32, C.POINTER(XttsSampling), C.POINTER(XttsBeam), i32, i32, f32p,
                                          i32p, i32p, i32p, u32p, i32, i32p, i32, i32p, i32, i32p, C.POINTER(XttsBeamState),
                                          vp, vp, f32p]
@@ -642,12 +642,11 @@ class NativeEngine:
                                            flags, iters, C.byref(ms)), "debug_gemm")
         return out, ms.value
 
-    LN_GEMM_PLAIN, LN_GEMM_PDL, LN_GEMM_COUNTERS = 0, 1, 2
+    LN_GEMM_PLAIN, LN_GEMM_PDL = 0, 1
 
     def debug_ln_gemm(self, mode: int, launch: int, X, ln_w, ln_b, W, bias=None, resid=None, gelu: bool = False,
                       out16: bool = False):
-        """The decode LayerNorm -> GEMM pair (xtts_debug_ln_gemm).  -> (Y [M, K] the 16-bit LN output, out [M, N], the GEMM's
-        CTA count, counters [2] after the launch)."""
+        """The decode LayerNorm -> GEMM pair (xtts_debug_ln_gemm).  -> (Y [M, K] the 16-bit LN output, out [M, N])."""
         X, W, lw, lb = _f32(X), _f32(W), _f32(ln_w), _f32(ln_b)
         M, K = X.shape
         N = W.shape[0]
@@ -655,13 +654,10 @@ class NativeEngine:
         r = _f32(resid) if resid is not None else None
         Y = np.empty((M, K), np.float32)
         out = np.empty((M, N), np.float32)
-        n = C.c_int32(0)
-        cnt = np.zeros(2, np.uint32)
         flags = (GEMM_GELU if gelu else 0) | (GEMM_OUT16 if out16 else 0)
         self._chk(self.lib.xtts_debug_ln_gemm(self.h, mode, launch, M, N, K, _fp(X), _fp(lw), _fp(lb), _fp(W), _fp(b), _fp(r),
-                                              flags, _fp(Y), _fp(out), C.byref(n),
-                                              cnt.ctypes.data_as(C.POINTER(C.c_uint32))), "debug_ln_gemm")
-        return Y, out, int(n.value), cnt
+                                              flags, _fp(Y), _fp(out)), "debug_ln_gemm")
+        return Y, out
 
     def debug_norms(self, out_type: int, X, w1, b1, w2=None, b2=None, M: Optional[int] = None, row_index=None, latents=None,
                     slots=None, lat_pos=None, n_gen=None):
@@ -706,19 +702,15 @@ class NativeEngine:
                   "debug_build_rows")
         return X
 
-    def debug_build_decode_rows(self, active, last_tok, n_gen, wte, wpe, counters=None, n_flags: int = 0):
-        """Decode row build (xtts_debug_build_decode_rows): last_tok / n_gen [n_slots]; counters (uint32, incoming contents)
-        whose first n_flags words the kernel zeroes.  -> (X [M, H], counters after or None)."""
+    def debug_build_decode_rows(self, active, last_tok, n_gen, wte, wpe):
+        """Decode row build (xtts_debug_build_decode_rows): last_tok / n_gen [n_slots].  -> X [M, H]."""
         act, lt, ng = _i32(active), _i32(last_tok), _i32(n_gen)
         a, p = _f32(wte), _f32(wpe)
         H = a.shape[1]
         X = np.empty((act.size, H), np.float32)
-        cnt = np.ascontiguousarray(counters, dtype=np.uint32).copy() if counters is not None else None
         self._chk(self.lib.xtts_debug_build_decode_rows(self.h, H, _fp(a), a.shape[0], _fp(p), p.shape[0], act.size, _ip(act), lt.size,
-                                                        _ip(lt), _ip(ng), _fp(X),
-                                                        cnt.ctypes.data_as(C.POINTER(C.c_uint32)) if cnt is not None else None,
-                                                        n_flags, cnt.size if cnt is not None else 0), "debug_build_decode_rows")
-        return X, cnt
+                                                        _ip(lt), _ip(ng), _fp(X)), "debug_build_decode_rows")
+        return X
 
     def debug_sample(self, logits, seen, sp: Sampling, step: int = 0):
         """Row b of logits [B, V] sampled as slot b with sp and seq_seed sp.seq_seed + b at step `step`; seen [B, V] (0/1)

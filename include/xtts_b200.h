@@ -283,8 +283,8 @@ int xtts_fetch(xtts_engine* e, uint64_t seq_id, int32_t* tokens, float* wav, flo
  *   "d2h_wav"             0 = leave waveforms in HBM (kernel-only timing), 1 = D2H into pinned memory (default)
  *   "cuda_graphs" / "pdl" / "splitk" / "tc_vocoder"   0/1, fast-mode execution features (all default 1)
  *   "hold_admission"      1 = queue submissions without admitting them, 0 = release (atomic batch submit)
- *   "decode_chain"        1 = fused persistent per-layer GEMM/LayerNorm chain kernel in the decode step, 0 = one launch per
- *                         GEMM / LayerNorm with "microbatches" concurrent row branches (default: measured faster)
+ *   "decode_chain"        0 only (a no-op, kept so that callers passing it keep working); any other value is an error:
+ *                         the fused persistent per-layer GEMM/LayerNorm chain kernel was removed
  *   "microbatches"        1..4 concurrent branches the decode step's rows are split into (default 2)
  *   "microbatch_min_rows" steps with fewer active rows stay single-branch (default 48)
  *   "gemm_wide"           4 (default), 3 or 2 = GEMMs with M >= 256 rows (prefill, conditioning) run on the persistent
@@ -308,17 +308,7 @@ int xtts_fetch(xtts_engine* e, uint64_t seq_id, int32_t* tokens, float* wav, flo
  *   "tc_epilogue"         epilogue of the fast-mode vocoder's tensor-core Conv1d: 1 (default) = staged through shared
  *                         memory (residual prefetched by a loader warp, outputs drained by bulk copies while the next
  *                         tile's MMAs run), 0 = straight from the accumulators.  Bit-identical results either way.
- *   "attn_warps"          warps per (row, head) item of the 16-bit decode attention: 4 (default), 1 / 2 / 8 / 16 measured slower
  *   "attn_ctas_per_sm"    > 0 caps the decode-attention grid (each CTA walks several items); < 0: absolute grid size (tests)
- *   "attn_l2_pages"       n > 0: each warp of the decode attention asks L2 for n of its later pages per item
- *                         (cp.async.bulk.prefetch.L2); default 0 (measured slower: the kernel is throughput-, not latency-bound)
- *   "attn_bulk"           c > 0: decode attention in bulk-copy form (c persistent CTAs per SM stream cache pages with
- *                         cp.async.bulk into "attn_stages" x 8 KB of shared-memory sub-rings, "attn_l2_ahead" = L2 prefetch
- *                         one item ahead); bit-identical to the default register-load kernel, measured slower; default 0
- *   "gemm_deep_ring"      1 = unsplit decode GEMMs use a ring that fills the SM (one CTA per SM); default 0 (measured slower)
- *   "gemm_l2_prefetch"    1 = decode GEMMs prefetch the weight tiles of their later ring passes into L2 before the
- *                         dependency wait; default 0 (no measurable effect)
- *   "dep_flags" / "branch_stagger_us"   counter dependencies / delayed second branch in the decode step (default off)
  *   "profile"             1 = CUDA events around every launch (xtts_get_kernel_profile), "reset_stats" = zero the counters */
 int xtts_set_option(xtts_engine* e, const char* key, int64_t value);
 int xtts_get_stats(xtts_engine* e, xtts_stats* out);
@@ -355,8 +345,7 @@ int xtts_gpt_teacher_forced(xtts_engine* e, const int32_t* text_ids, int32_t n_t
                             const int32_t* forced_tokens, int32_t n, const xtts_sampling* sp, float* logits_out,
                             float* latents_out, int32_t* sampled_out);
 /* GEMM under test: mode 0 = fp32 CUDA-core, 1 = bf16 wgmma, 2 = fp16 wgmma.  A [M,K], W [N,K], bias [N] or NULL, resid [M,N] or NULL;
- * out [M,N] = epi(A . W^T + bias) under the engine's current GEMM options ("gemm_wide", "gemm_bn", "gemm_deep_ring",
- * "gemm_l2_prefetch").  flags (XTTS_DEBUG_GEMM_*; 0 / 1 = without / with GELU, as before the flag word):
+ * out [M,N] = epi(A . W^T + bias) under the engine's current GEMM options ("gemm_wide", "gemm_bn").  flags (XTTS_DEBUG_GEMM_*; 0 / 1 = without / with GELU, as before the flag word):
  *   GELU    gelu_new after the bias, before the residual
  *   OUT16   16-bit output in the operand type (modes 1 / 2, no resid), returned widened to fp32
  *   INPLACE out is preloaded with resid and passed as the residual too (the engine's o-proj / down-proj without split-K)
@@ -411,13 +400,11 @@ int xtts_debug_splitk_ln(xtts_engine* e, int32_t mode, int32_t M, int32_t N, int
 /* the decode step's LayerNorm -> GEMM pair as the fast-mode decode launches it (mode 1 bf16 / 2 fp16): Y [M,K] =
  * LayerNorm(X [M,K]; ln_w, ln_b, the engine's eps) in the 16-bit type (returned as fp32), then out [M,N] = epi(Y . W^T + bias)
  * + resid on the one-tile GEMM, flags XTTS_DEBUG_GEMM_GELU / OUT16 only (OUT16: 16-bit out, returned as fp32, no resid).
- * launch 0: plain launches; 1: both with PDL; 2: PDL plus dependency counters (LN counts its M CTAs into counters[0], the
- * GEMM waits for counters[0] == M instead of griddepcontrol.wait and counts its CTAs into counters[1]).  *n_ctas = the CTA
- * count the GEMM launcher returned; counters [2] = their final values (0 unless launch 2).  Rejected before any launch: a
- * resid with launch 2 (a counter cannot order the residual read), N % 32, K % 64, K > 8192, NULL except bias / resid. */
+ * launch 0: plain launches; 1: both with PDL.  Rejected before any launch: another launch mode, N % 32, K % 64, K > 8192,
+ * NULL except bias / resid. */
 int xtts_debug_ln_gemm(xtts_engine* e, int32_t mode, int32_t launch, int32_t M, int32_t N, int32_t K, const float* X,
                        const float* ln_w, const float* ln_b, const float* W, const float* bias, const float* resid, int32_t flags,
-                       float* Y, float* out, int32_t* n_ctas, uint32_t* counters);
+                       float* Y, float* out);
 /* LayerNorms in the output type out_type (0 fp32, 1 bf16, 2 fp16; returned as fp32), eps = the engine's, H <= 8192.
  * w2 == b2 == NULL: Y[i] = LN(X[i]; w1, b1) for i < M (row_index, latents NULL; x_rows >= M).
  * w2 != NULL, the GPT head: r = row_index ? row_index[i] : i (< x_rows), y = LN(LN(X[r]; w1, b1); w2, b2), Y[i] = y, and with
@@ -441,12 +428,11 @@ int xtts_debug_kv_write(xtts_engine* e, int32_t kv_type, int32_t heads, int32_t 
 int xtts_debug_build_rows(xtts_engine* e, int32_t H, int32_t n_cond, const float* text_emb, int32_t n_text, const float* text_pos,
                           int32_t n_text_pos, const float* wte, int32_t n_audio, const float* wpe, int32_t n_wpe,
                           const float* spk_cond, int32_t n_spk, const int32_t* rows, int32_t n_rows, float* X);
-/* decode row build: X[i] = wte[last_tok[s]] + wpe[n_gen[s]], s = active[i] < n_slots; counters [n_words] in/out: the kernel
- * zeroes the first n_flags words (the step's dependency counters) and must leave the rest alone.  Launched with PDL when
- * option "pdl" is on.  Rejected before any launch: a slot, token or position outside its table, n_flags > n_words. */
+/* decode row build: X[i] = wte[last_tok[s]] + wpe[n_gen[s]], s = active[i] < n_slots.  Launched with PDL when option "pdl"
+ * is on.  Rejected before any launch: a slot, token or position outside its table. */
 int xtts_debug_build_decode_rows(xtts_engine* e, int32_t H, const float* wte, int32_t n_audio, const float* wpe, int32_t n_wpe,
                                  int32_t M, const int32_t* active, int32_t n_slots, const int32_t* last_tok, const int32_t* n_gen,
-                                 float* X, uint32_t* counters, int32_t n_flags, int32_t n_words);
+                                 float* X);
 /* fast-mode vocoder convolution on the tensor cores (fp16 operands, fp32 accumulate), weights packed as the engine packs
  * them.  up 0: Conv1d(Cin -> Cout, odd K, dilation dil, "same" padding), w [Cout][Cin][K]; up u in {2, 4, 8}:
  * ConvTranspose1d(Cin -> Cout, kernel K = 2u, stride u, padding u/2), w [Cin][Cout][2u], dil 1, no resid, mode 0,

@@ -1,8 +1,7 @@
 """The GPT forward's remaining kernels launched on their own and compared with a float64 reference of the same operation:
 the one-tile tensor-core GEMM in the configurations the decode step and fast-mode prefill use (16-bit output with GELU, a
-residual that aliases the output, PDL launches, every decode tile width, the deep ring and the L2 prefetch), the decode
-LayerNorm -> GEMM pair with and without dependency counters, the LayerNorm and GPT head norm kernels in all three output
-types, the prefill's paged-cache write and both row builds.  The reference sees the operands rounded exactly as the kernel
+residual that aliases the output, PDL launches, every decode tile width), the decode LayerNorm -> GEMM pair with and
+without PDL, the LayerNorm and GPT head norm kernels in all three output types, the prefill's paged-cache write and both row builds.  The reference sees the operands rounded exactly as the kernel
 rounds them, so each bound is the output rounding plus an fp32 arithmetic term derived next to it.  Scheduling options must
 not change a single bit; the end-to-end test checks that for the decode step's non-default execution paths."""
 import numpy as np
@@ -289,40 +288,37 @@ def test_gemm_wide_vs_narrow(engine_small, mode):
           f"bit-identical in {sum(same)} / {len(same)} cases")
 
 
-# Deep-ring shapes: K / 64 k-blocks exceed the default ring (BN 32: 5 stages, BN 64: 4), M <= 256, no split-K
-DEEP_RING_SHAPES = [(1, 1024, 4096), (7, 4096, 1024), (168, 3072, 1024), (255, 1056, 1024), (256, 1024, 1024), (33, 384, 512)]
+# Multi-pass shapes: K / 64 k-blocks exceed the ring (BN 32: 5 stages, BN 64: 4), M <= 256, no split-K
+MULTI_PASS_SHAPES = [(1, 1024, 4096), (7, 4096, 1024), (168, 3072, 1024), (255, 1056, 1024), (256, 1024, 1024), (33, 384, 512)]
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("mode", [1, 2], ids=["bf16", "fp16"])
 def test_gemm_scheduling_options_are_bit_identical(engine_small, mode):
-    """Within the one-tile kernel, the tile width ("gemm_bn" 0 / 32 / 64 / 128), the deep ring ("gemm_deep_ring"), the L2
-    prefetch of later weight tiles ("gemm_l2_prefetch") and a PDL launch change scheduling only: every output element sees
-    the same MMAs in the same k order, so all 32 combinations give the same bits, in the fp32 and the 16-bit epilogue."""
+    """Within the one-tile kernel, the tile width ("gemm_bn" 0 / 32 / 64 / 128) and a PDL launch change scheduling only:
+    every output element sees the same MMAs in the same k order, so all 8 combinations give the same bits, in the fp32 and
+    the 16-bit epilogue."""
     eng = engine_small
     try:
         eng.set_option("gemm_wide", 0)                  # M = 256 stays on the one-tile kernel for the plain launch too
-        for (M, N, K) in DEEP_RING_SHAPES:
+        for (M, N, K) in MULTI_PASS_SHAPES:
             A, W, b, r, A16, W16 = _gemm_data(M, N, K, mode, seed=M * 7 + N + K)
             prod = gemm_products(A16, W16)
             for gelu, out16, inplace in ((True, True, False), (False, False, True)):
                 ref, tol = ref_gemm16(A16, W16, b, r if inplace else None, gelu, mode if out16 else 0, prod)
                 base = None
                 for bn in (0, 32, 64, 128):
-                    for deep in (0, 1):
-                        for l2 in (0, 1):
-                            for pdl in (False, True):
-                                eng.set_option("gemm_bn", bn); eng.set_option("gemm_deep_ring", deep)
-                                eng.set_option("gemm_l2_prefetch", l2)
-                                out, _ = eng.debug_gemm(mode, A, W, b, r if inplace else None, gelu, out16=out16,
-                                                        inplace=inplace, pdl=pdl)
-                                label = (KIND_NAMES[mode], M, N, K, gelu, out16, bn, deep, l2, pdl)
-                                if base is None:
-                                    _check(out, ref, tol, label)
-                                    base = out
-                                np.testing.assert_array_equal(bits(out), bits(base), err_msg=str(label))
+                    for pdl in (False, True):
+                        eng.set_option("gemm_bn", bn)
+                        out, _ = eng.debug_gemm(mode, A, W, b, r if inplace else None, gelu, out16=out16, inplace=inplace,
+                                                pdl=pdl)
+                        label = (KIND_NAMES[mode], M, N, K, gelu, out16, bn, pdl)
+                        if base is None:
+                            _check(out, ref, tol, label)
+                            base = out
+                        np.testing.assert_array_equal(bits(out), bits(base), err_msg=str(label))
     finally:
-        for k, v in (("gemm_wide", 4), ("gemm_bn", 0), ("gemm_deep_ring", 0), ("gemm_l2_prefetch", 0)):
+        for k, v in (("gemm_wide", 4), ("gemm_bn", 0)):
             eng.set_option(k, v)
 
 
@@ -347,7 +343,7 @@ def test_gemm_rejects_bad_flag_combinations(engine_small):
     with pytest.raises(NativeError):
         engine_small.debug_gemm(1, A[:, :40], W[:, :40])            # K % 64
     with pytest.raises(NativeError):
-        engine_small.debug_ln_gemm(1, 2, A, A[0], A[0], W, resid=r)   # a counter cannot order a residual read
+        engine_small.debug_ln_gemm(1, 2, A, A[0], A[0], W)            # launch modes are 0 (plain) and 1 (PDL)
 
 
 # ------------------------------------------------------------------------------------------------ LayerNorm -> GEMM pair
@@ -355,9 +351,9 @@ def test_gemm_rejects_bad_flag_combinations(engine_small):
 @pytest.mark.parametrize("mode", [1, 2], ids=["bf16", "fp16"])
 def test_decode_ln_gemm_launch_modes(engine_small, dims_small, dims_full, mode):
     """The decode step's LayerNorm -> GEMM pair (the first LN and the qkv GEMM of decode_layers_rows; GELU + 16-bit output as
-    the fc GEMM) in its three launch modes — plain, PDL, PDL plus dependency counters — gives the same bits in all three;
-    the LN output is within one 16-bit rounding of the fp64 LayerNorm, the GEMM output within ref_gemm16's bound of the
-    product of the kernel's own LN output; each counter ends at exactly the CTA count of its kernel (M for the LN)."""
+    the fc GEMM) in both launch modes — plain and PDL — gives the same bits in both; the LN output is within one 16-bit
+    rounding of the fp64 LayerNorm, the GEMM output within ref_gemm16's bound of the product of the kernel's own LN
+    output."""
     eng = engine_small
     eps = dims_small.gpt.ln_eps
     worst_y = worst_o = 0.0
@@ -372,20 +368,11 @@ def test_decode_ln_gemm_launch_modes(engine_small, dims_small, dims_full, mode):
             bias = rng.randn(N).astype(np.float32)
             W16 = rnd(W, mode)[1]
             for gelu, out16 in ((False, False), (True, True)):
-                res = {}
-                for launch in (0, 1, 2):
-                    Y, out, n_ctas, cnt = eng.debug_ln_gemm(mode, launch, X, ln_w, ln_b, W, bias, gelu=gelu, out16=out16)
-                    label = (KIND_NAMES[mode], M, N, K, gelu, launch)
-                    res[launch] = (Y, out)
-                    assert n_ctas > 0, label
-                    if launch == 2:
-                        assert cnt.tolist() == [M, n_ctas], (label, cnt.tolist(), n_ctas)
-                    else:
-                        assert cnt.tolist() == [0, 0], label
-                Y, out = res[0]
-                for launch in (1, 2):
-                    np.testing.assert_array_equal(bits(res[launch][0]), bits(Y), err_msg=str((label, "Y")))
-                    np.testing.assert_array_equal(bits(res[launch][1]), bits(out), err_msg=str((label, "out")))
+                label = (KIND_NAMES[mode], M, N, K, gelu)
+                Y, out = eng.debug_ln_gemm(mode, eng.LN_GEMM_PLAIN, X, ln_w, ln_b, W, bias, gelu=gelu, out16=out16)
+                Y_pdl, out_pdl = eng.debug_ln_gemm(mode, eng.LN_GEMM_PDL, X, ln_w, ln_b, W, bias, gelu=gelu, out16=out16)
+                np.testing.assert_array_equal(bits(Y_pdl), bits(Y), err_msg=str((label, "Y")))
+                np.testing.assert_array_equal(bits(out_pdl), bits(out), err_msg=str((label, "out")))
                 (y_ref, s), = ref_ln_chain(X, [(ln_w, ln_b)], eps)
                 worst_y = max(worst_y, _check(Y, y_ref, HALF_ULP[mode] * np.abs(y_ref) + (1 + HALF_ULP[mode]) * s + 1e-30,
                                               (label, "Y")))
@@ -521,34 +508,30 @@ def test_build_rows_match_float32_add(engine_small, H):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("H", [128, 1024])
-def test_build_decode_rows_and_counter_reset(engine_small, H):
+def test_build_decode_rows_match_float32_add(engine_small, H):
     """build_decode_rows_kernel: X[i] = wte[last_tok[s]] + wpe[n_gen[s]] (s = active[i], shuffled, sparse slots) exactly as
-    a float32 add; the first n_flags counter words become 0 and the guard words after them are untouched."""
+    a float32 add."""
     rng = np.random.RandomState(H + 1)
     t = _tables(H, rng)
     n_slots = 9
     last_tok = rng.randint(0, t["wte"].shape[0], n_slots).astype(np.int32)
     n_gen = rng.randint(0, t["wpe"].shape[0], n_slots).astype(np.int32)
     last_tok[0], n_gen[0] = t["wte"].shape[0] - 1, t["wpe"].shape[0] - 1
-    for active, n_flags, guard in (([3, 0, 8, 5, 1], 4 * 2 * 7, 16), ([0], 0, 8), (list(rng.permutation(n_slots)), 4 * 30 * 7, 33)):
-        counters = rng.randint(1, 2 ** 32 - 1, n_flags + guard, dtype=np.uint64).astype(np.uint32)
-        X, after = engine_small.debug_build_decode_rows(active, last_tok, n_gen, t["wte"], t["wpe"], counters, n_flags)
+    for active in ([3, 0, 8, 5, 1], [0], list(rng.permutation(n_slots))):
+        X = engine_small.debug_build_decode_rows(active, last_tok, n_gen, t["wte"], t["wpe"])
         s = np.asarray(active)
         np.testing.assert_array_equal(X, t["wte"][last_tok[s]] + t["wpe"][n_gen[s]])
-        np.testing.assert_array_equal(after[:n_flags], 0)
-        np.testing.assert_array_equal(after[n_flags:], counters[n_flags:])
 
 
 # ------------------------------------------------------------------------------------------------ end to end
-OPTION_DEFAULTS = dict(dep_flags=0, pdl=1, branch_stagger_us=0, voc_batch=32)
+OPTION_DEFAULTS = dict(pdl=1, voc_batch=32)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("which", ["fp16", "bf16"])
 def test_decode_execution_options_are_bit_identical(request, dims_full, which):
-    """The decode step's non-default execution paths — dependency counters instead of griddepcontrol.wait ("dep_flags" 1),
-    no programmatic dependent launch ("pdl" 0), a delayed second row branch ("branch_stagger_us" 50) — and one vocoder
-    window per launch ("voc_batch" 1) change scheduling only.  With both row branches running (microbatch_min_rows 2) and
+    """The decode step without programmatic dependent launch ("pdl" 0) and one vocoder window per launch ("voc_batch" 1)
+    change scheduling only.  With both row branches running (microbatch_min_rows 2) and
     the step replayed from CUDA graphs after its eager steps, tokens, latents and waveforms must equal the defaults' bit for
     bit."""
     eng = request.getfixturevalue(f"engine_full_{which}")
@@ -559,7 +542,7 @@ def test_decode_execution_options_are_bit_identical(request, dims_full, which):
     try:
         eng.set_option("microbatch_min_rows", 2)
         ref = eng.run_batch(jobs, timeout_s=180, want_latents=True)
-        for key, val in (("dep_flags", 1), ("pdl", 0), ("branch_stagger_us", 50), ("voc_batch", 1)):
+        for key, val in (("pdl", 0), ("voc_batch", 1)):
             try:
                 eng.set_option(key, val)
                 got = eng.run_batch(jobs, timeout_s=180, want_latents=True)

@@ -1,7 +1,8 @@
-"""Decode-step time at the bench's batch (163 rows, ~430 cached tokens) for the two decode-attention kernels:
-register loads (attn_bulk = 0) vs the cp.async.bulk ring (attn_bulk = CTAs per SM, attn_stages = ring depth), with 1-3 row
-branches.  ms per decode step = (run to 400 tokens - run to 300 tokens) / 100, interleaved repeats, minimum reported.
-python tools/attn_probe.py [rows] [precision]"""
+"""Decode-step time at the bench's batch (163 rows, ~430 cached tokens) for 1 and 2 row branches ("microbatches") with the
+decode-attention grid uncapped or capped ("attn_ctas_per_sm" = CTAs per SM).  ms per decode step = (run to 400 tokens - run
+to 300 tokens) / 100, interleaved repeats, minimum reported.  Options are set and never reset: every config of a list names
+every option the list varies.
+python tools/attn_probe.py [rows] [precision] [key=value ...]"""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -30,9 +31,8 @@ def measure(**opts):
         t0 = time.time(); eng.run_batch(jobs(nt), timeout_s=600, want_wav=False); t.append(time.time() - t0)
     return 1e3 * (t[1] - t[0]) / 100
 import json
-cfgs = [dict(attn_bulk=b, attn_warps=nw, attn_stages=st, attn_l2_pages=lp, microbatches=mb)
-        for mb in (1, 2) for (b, nw, st, lp) in ((0, 4, 8, 0), (0, 4, 8, 1), (0, 4, 8, 2), (0, 4, 8, 3), (0, 4, 8, 5))]
-if os.environ.get("STEP_CFGS"):          # any list of option dicts, e.g. STEP_CFGS='[{"gemm_deep_ring":0},{"gemm_deep_ring":1}]'
+cfgs = [dict(attn_ctas_per_sm=c, microbatches=mb) for mb in (1, 2) for c in (0, 2, 4, 8)]
+if os.environ.get("STEP_CFGS"):          # any list of option dicts, e.g. STEP_CFGS='[{"gemm_bn":0},{"gemm_bn":64}]'
     cfgs = json.loads(os.environ["STEP_CFGS"])
 for extra in sys.argv[3:]:
     eng.set_option(extra.split("=")[0], int(extra.split("=")[1]))

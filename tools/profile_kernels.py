@@ -18,7 +18,7 @@ cond = torch.randn(32, 1024, generator=g); dv = torch.nn.functional.normalize(to
 eng = native.NativeEngine(dims, precision=1, max_batch=max(nb, 8), max_speakers=2)
 eng.load_state(gs, cs); eng.set_speaker(0, cond.numpy(), dv.numpy())
 eng.set_option("cuda_graphs", 0)
-for kv in os.environ.get("XTTS_OPTS", "").split(","):      # e.g. XTTS_OPTS=decode_chain=1,microbatches=1
+for kv in os.environ.get("XTTS_OPTS", "").split(","):      # e.g. XTTS_OPTS=attn_ctas_per_sm=4,microbatches=1
     if "=" in kv: eng.set_option(kv.split("=")[0], int(kv.split("=")[1]))
           # ncu attributes kernels per launch either way; eager keeps names simple
 rng = np.random.RandomState(1)
