@@ -25,6 +25,38 @@ inline void cuda_check(cudaError_t e, const char* what, const char* file, int li
 #define CUDA_CHECK(x) ::xtts::cuda_check((x), #x, __FILE__, __LINE__)
 #define KERNEL_CHECK() ::xtts::cuda_check(cudaGetLastError(), "kernel launch", __FILE__, __LINE__)
 
+// Owning device array of n elements: not copyable, so exactly one owner frees it; a move hands the allocation over.
+template <typename T>
+struct DBuf {
+    T* p = nullptr;
+    size_t n = 0;
+    DBuf() = default;
+    DBuf(const DBuf&) = delete;
+    DBuf& operator=(const DBuf&) = delete;
+    DBuf(DBuf&& o) noexcept : p(o.p), n(o.n) { o.p = nullptr; o.n = 0; }
+    DBuf& operator=(DBuf&& o) noexcept {
+        if (this != &o) { release(); p = o.p; n = o.n; o.p = nullptr; o.n = 0; }
+        return *this;
+    }
+    ~DBuf() { release(); }
+    void alloc(size_t count) {
+        release();
+        n = count;
+        if (count) CUDA_CHECK(cudaMalloc(&p, count * sizeof(T)));
+    }
+    void ensure(size_t count) { if (count > n) alloc(count); }      // grow only; contents are not kept
+    void zero(cudaStream_t st) { if (n) CUDA_CHECK(cudaMemsetAsync(p, 0, n * sizeof(T), st)); }
+    void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
+    void upload(const T* h, size_t count, cudaStream_t st, size_t off = 0) {
+        CUDA_CHECK(cudaMemcpyAsync(p + off, h, count * sizeof(T), cudaMemcpyHostToDevice, st));
+    }
+    void download(T* h, size_t count, cudaStream_t st, size_t off = 0) const {
+        CUDA_CHECK(cudaMemcpyAsync(h, p + off, count * sizeof(T), cudaMemcpyDeviceToHost, st));
+    }
+    // sized to h and filled from it; synchronises the stream, so h may go away on return
+    void up(const std::vector<T>& h, cudaStream_t st) { alloc(h.size()); upload(h.data(), h.size(), st); CUDA_CHECK(cudaStreamSynchronize(st)); }
+};
+
 // Per-engine launcher state.  Several engines (one per GPU) may live in one process, each with its own scheduler thread:
 // what used to be process globals is a KernelCtx owned by the engine and bound to whichever thread issues that engine's
 // work (the scheduler thread, or an API thread inside a synchronous entry point).  Unbound threads see a default context.

@@ -330,9 +330,9 @@ std::vector<float> mel_fb_t(int n_freqs, double f_min, double f_max, int n_mels,
 
 namespace {
 
-struct Lin { Dev<float> w, b; int N = 0, K = 0; bool has_b = false; };
-struct Bn { Dev<float> scale, shift; };
-struct Block { Dev<float> c1, c2, ds; Bn bn1, bn2, bnd; Lin se1, se2; int cin = 0, cout = 0, stride = 1; bool has_ds = false; };
+struct Lin { DBuf<float> w, b; int N = 0, K = 0; bool has_b = false; };
+struct Bn { DBuf<float> scale, shift; };
+struct Block { DBuf<float> c1, c2, ds; Bn bn1, bn2, bnd; Lin se1, se2; int cin = 0, cout = 0, stride = 1; bool has_ds = false; };
 
 }  // namespace
 
@@ -341,18 +341,18 @@ struct Conditioner::Impl {
     cudaStream_t st;
     int H, NH;
     // front-ends
-    Dev<float> hann, basis22, fb22, mel_stats, hamm, basis16, fb16;
+    DBuf<float> hann, basis22, fb22, mel_stats, hamm, basis16, fb16;
     // cond encoder
-    Lin init; struct AB { Dev<float> nw, nb; Lin qkv, proj; }; std::vector<std::unique_ptr<AB>> blocks;
+    Lin init; struct AB { DBuf<float> nw, nb; Lin qkv, proj; }; std::vector<std::unique_ptr<AB>> blocks;
     // perceiver
-    Dev<float> latents, gamma; struct PL { Lin q, kv, o, f1, f2; }; std::vector<std::unique_ptr<PL>> pl;
+    DBuf<float> latents, gamma; struct PL { Lin q, kv, o, f1, f2; }; std::vector<std::unique_ptr<PL>> pl;
     int inner = 0, ffi = 0;
     // speaker encoder
-    Dev<float> conv1_w, conv1_b; Bn bn1; std::vector<std::unique_ptr<Block>> res; Lin att0, att3, fc; Bn att_bn;
+    DBuf<float> conv1_w, conv1_b; Bn bn1; std::vector<std::unique_ptr<Block>> res; Lin att0, att3, fc; Bn att_bn;
     // workspaces
-    Dev<float> wav22, wav16, pre16, F, D, P, mel, h0, h1, xn, qkv, att, kvin, q, kv, o, lat, ff, gg, img, a0, a1, a2, ds,
+    DBuf<float> wav22, wav16, pre16, F, D, P, mel, h0, h1, xn, qkv, att, kvin, q, kv, o, lat, ff, gg, img, a0, a1, a2, ds,
         chm, gate, xT, at1, at2, pooled;
-    Dev<AttnSeq> seq;
+    DBuf<AttnSeq> seq;
 
     void lin(Lin& l, const HostTensorView& w, const HostTensorView* b) {
         l.N = (int)w.shape[0]; l.K = (int)(w.numel() / w.shape[0]);
@@ -703,17 +703,16 @@ void cond_debug(Conditioner* cnd, int op, const int32_t* dims, int n_dims, const
     }
     if (out_len < 1 || out_len != need_out) throw bad("out has " + std::to_string(out_len) + " floats, expected " + std::to_string(need_out));
 
-    std::vector<std::unique_ptr<Dev<float>>> din;
+    std::vector<DBuf<float>> din(n_in);
     std::vector<const float*> ip(n_in);
     for (int i = 0; i < n_in; ++i) {
-        din.emplace_back(new Dev<float>());
-        din.back()->up(std::vector<float>(in[i], in[i] + in_len[i]), st);
-        ip[i] = din.back()->p;
+        din[i].up(std::vector<float>(in[i], in[i] + in_len[i]), st);
+        ip[i] = din[i].p;
     }
     // out with kGuardWords sentinel words on each side; its incoming contents are uploaded (in-place kernels read them)
     std::vector<uint32_t> h((size_t)out_len + 2 * kGuardWords, kGuardBits);
     std::memcpy(h.data() + kGuardWords, out, (size_t)out_len * sizeof(float));
-    Dev<float> dout;
+    DBuf<float> dout;
     dout.alloc(h.size());
     CUDA_CHECK(cudaMemcpyAsync(dout.p, h.data(), h.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
     float* o = dout.p + kGuardWords;

@@ -15,16 +15,6 @@ namespace xtts {
 
 constexpr double kPi = 3.14159265358979323846;
 
-// device buffer (the conditioner's and the enhancer's workspaces)
-template <typename T>
-struct Dev {
-    T* p = nullptr; size_t n = 0;
-    ~Dev() { if (p) cudaFree(p); }
-    void alloc(size_t c) { if (p) cudaFree(p); p = nullptr; n = c; if (c) CUDA_CHECK(cudaMalloc(&p, c * sizeof(T))); }
-    void ensure(size_t c) { if (c > n) alloc(c); }
-    void up(const std::vector<T>& h, cudaStream_t st) { alloc(h.size()); CUDA_CHECK(cudaMemcpyAsync(p, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, st)); CUDA_CHECK(cudaStreamSynchronize(st)); }
-};
-
 inline int nblk(size_t n, int t = 256) { return (int)((n + t - 1) / t); }
 
 // ---- STFT front-end shared by the conditioner (cond.cu) and the reference enhancer (enhance.cu)

@@ -4,6 +4,7 @@
 #include "../../include/xtts_b200.h"
 #include "kernels.h"
 #include "cond.h"
+#include "harness.h"
 
 #include <algorithm>
 #include <atomic>
@@ -12,6 +13,7 @@
 #include <condition_variable>
 #include <cstring>
 #include <deque>
+#include <functional>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -38,29 +40,6 @@ static double now_s() {
 }
 
 // ------------------------------------------------------------------------------------------------
-template <typename T>
-struct DBuf {
-    T* p = nullptr;
-    size_t n = 0;
-    DBuf() = default;
-    DBuf(const DBuf&) = delete;
-    DBuf& operator=(const DBuf&) = delete;
-    ~DBuf() { release(); }
-    void alloc(size_t count) {
-        release();
-        n = count;
-        if (count) CUDA_CHECK(cudaMalloc(&p, count * sizeof(T)));
-    }
-    void zero(cudaStream_t st) { if (n) CUDA_CHECK(cudaMemsetAsync(p, 0, n * sizeof(T), st)); }
-    void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
-    void upload(const T* h, size_t count, cudaStream_t st, size_t off = 0) {
-        CUDA_CHECK(cudaMemcpyAsync(p + off, h, count * sizeof(T), cudaMemcpyHostToDevice, st));
-    }
-    void download(T* h, size_t count, cudaStream_t st, size_t off = 0) const {
-        CUDA_CHECK(cudaMemcpyAsync(h, p + off, count * sizeof(T), cudaMemcpyDeviceToHost, st));
-    }
-};
-
 struct HostTensor {
     std::vector<float> data;
     std::vector<int64_t> shape;
@@ -185,43 +164,8 @@ public:
                           float* hidden_out, float* logits_out, float* latents_out);
     void gpt_teacher_forced_sync(const int32_t* text, int n_text, int speaker, const int32_t* forced, int n,
                                  const xtts_sampling& sp, float* logits_out, float* latents_out, int32_t* sampled_out);
-    void debug_gemm(int mode, const float* A, const float* W, const float* bias, const float* resid, float* out, int M,
-                    int N, int K, int dflags, int iters, float* ms);
-    void debug_ln_gemm(int mode, int launch, int M, int N, int K, const float* X, const float* ln_w, const float* ln_b,
-                       const float* W, const float* bias, const float* resid, int dflags, float* Y, float* out);
-    void debug_norms(int out_type, int M, int H, const float* X, int x_rows, const int32_t* row_index, const float* w1,
-                     const float* b1, const float* w2, const float* b2, float* Y, float* latents, int n_slots, int lat_rows,
-                     const int32_t* slots, const int32_t* lat_pos, const int32_t* n_gen);
-    void debug_kv_write(int kv_type, int heads, int M, const float* qkv, const int32_t* row_slot, const int32_t* row_pos,
-                        int n_slots, const int32_t* ctx_len, const int32_t* block_tables, int max_pages, int n_pages,
-                        void* kpool, void* vpool);
-    void debug_build_rows(int H, int n_cond, const float* text_emb, int n_text, const float* text_pos, int n_tpos,
-                          const float* wte, int n_audio, const float* wpe, int n_wpe, const float* spk, int n_spk,
-                          const int32_t* rows, int n_rows, float* X);
-    void debug_build_decode_rows(int H, const float* wte, int n_audio, const float* wpe, int n_wpe, int M, const int32_t* active,
-                                 int n_slots, const int32_t* last_tok, const int32_t* n_gen, float* X);
-    void debug_sample_slots(int V, int M, const int32_t* active, int n_slots, const float* logits, int ld,
-                            const xtts_sampling* sp, int cap, int advance_ctx, const int32_t* forced, int32_t* n_gen,
-                            int32_t* ctx_len, int32_t* finished, int32_t* last_tok, uint8_t* seen, int32_t* tokens,
-                            int32_t* sampled);
-    void debug_attn_decode(int kv_type, int heads, int M, const int32_t* active, int n_slots, const int32_t* ctx_len,
-                           const int32_t* block_tables, int max_pages, int n_pages, void* kpool, void* vpool,
-                           const float* qkv, float* out);
-    void debug_attn_prefill(int out_type, int heads, const int32_t* seqs, int nseq, int causal, float scale,
-                            const float* q, int64_t q_len, int q_row_stride, int q_head_stride,
-                            const float* kv, int64_t kv_len, int kv_row_stride, int kv_head_stride, int64_t k_off,
-                            int64_t v_off, float* out, int out_rows);
-    void debug_splitk_ln(int mode, int M, int N, int K, int splits, const float* A, const float* W, const float* bias,
-                         float* X, const float* ln_w, const float* ln_b, float* Y);
-    void debug_conv_tc(int up, int Cin, int Cout, int K, int dil, int batch, int L, const int32_t* item_len, const float* w,
-                       const float* bias, const float* cbias, int cbias_stride, const float* x, const float* resid, int mode,
-                       float slope_out, float scale16, int max_ctas, float* out32, float* out16);
-    void debug_beam_step(int kv_type, int heads, int layers, int Vn, const xtts_sampling& sp, const xtts_beam& bm, int first,
-                         int advance, const float* logits, int32_t* n_gen, int32_t* ctx_len, int32_t* last_tok, uint32_t* seen,
-                         int mp, int32_t* block_tables, int n_pages, int32_t* pool, int cap, int32_t* hist,
-                         xtts_beam_state* state, void* kpool, void* vpool, float* scores);
-    void debug_cond(int op, const int32_t* dims, int n_dims, const float* scal, int n_scal, const float* const* in,
-                    const int64_t* in_len, int n_in, float* out, int64_t out_len);
+    // runs f with this engine's stream and options under its API lock; throws unless the engine is idle
+    void run_idle(const std::function<void(const HarnessCtx&)>& f);
 
 private:
     KernelCtx kctx_;
@@ -438,6 +382,10 @@ private:
     std::vector<std::pair<float*, size_t>> dev_pool;
     void loop();
     void require_finalized() const { if (!finalized) throw std::runtime_error("weights not finalized: call xtts_finalize_weights first"); }
+    void require_idle() const {
+        if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty())
+            throw std::runtime_error("debug entry points need an idle engine");
+    }
 };
 
 // ================================================================================================
@@ -2298,7 +2246,7 @@ void Engine::gpt_prefill_sync(const int32_t* text, int n_text, int speaker, cons
                               float* hidden_out, float* logits_out, float* latents_out) {
     ApiLock lk(this);
     require_finalized();
-    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
+    require_idle();
     CUDA_CHECK(cudaSetDevice(cfg.device));
     Sequence s; s.text_ids.assign(text, text + n_text); s.speaker = speaker; s.slot = B;
     s.sp.max_tokens = CAP; s.sp.stop_token = cfg.stop_audio_token; s.sp.repetition_penalty = 1.f; s.sp.temperature = 0.f;
@@ -2334,7 +2282,7 @@ void Engine::gpt_teacher_forced_sync(const int32_t* text, int n_text, int speake
                                      const xtts_sampling& sp, float* logits_out, float* latents_out, int32_t* sampled_out) {
     ApiLock lk(this);
     require_finalized();
-    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
+    require_idle();
     if (n < 1 || n > CAP) throw std::runtime_error("teacher_forced: n out of range");
     CUDA_CHECK(cudaSetDevice(cfg.device));
     Sequence s; s.text_ids.assign(text, text + n_text); s.speaker = speaker; s.slot = B; s.sp = sp;
@@ -2363,669 +2311,12 @@ void Engine::gpt_teacher_forced_sync(const int32_t* text, int n_text, int speake
     release_slot(s);
 }
 
-// fp32 -> the 16-bit operand type of `mode` (1 bf16, 2 IEEE fp16 bits in the same buffer type)
-static void to16(int mode, const float* in, __nv_bfloat16* out, size_t n, cudaStream_t st) {
-    if (mode == 2) launch_f32_to_f16(in, reinterpret_cast<__half*>(out), n, st);
-    else launch_f32_to_bf16(in, out, n, st);
-}
-
-// 16-bit device values -> fp32 on the host (exact)
-static void widen16(const std::vector<uint16_t>& in, bool f16, float* out) {
-    for (size_t i = 0; i < in.size(); ++i) {
-        if (f16) { __half_raw r; r.x = in[i]; out[i] = __half2float(__half(r)); }
-        else { const uint32_t u = (uint32_t)in[i] << 16; std::memcpy(&out[i], &u, 4); }
-    }
-}
-
-// One GEMM launch on private buffers.  The weights are converted and synchronised first; the activation conversion is the
-// kernel right before the GEMM, so a PDL launch overlaps it exactly as the decode chain overlaps a GEMM with its producer
-// (weight tiles requested before griddepcontrol.wait, activation tiles and the residual after it).
-void Engine::debug_gemm(int mode, const float* A, const float* W, const float* bias, const float* resid, float* out, int M,
-                        int N, int K, int dflags, int iters, float* ms) {
+// The kernel isolation harness (harness.cu) behind the xtts_debug_* entry points: one call at a time on an idle engine
+void Engine::run_idle(const std::function<void(const HarnessCtx&)>& f) {
     ApiLock lk(this);
-    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
-    if (mode < 0 || mode > 2) throw std::runtime_error("debug_gemm: mode 0 (fp32), 1 (bf16) or 2 (fp16)");
-    if (M < 1 || N < 1 || K < 1 || !A || !W || !out) throw std::runtime_error("debug_gemm: empty problem");
-    if (dflags & ~(XTTS_DEBUG_GEMM_GELU | XTTS_DEBUG_GEMM_OUT16 | XTTS_DEBUG_GEMM_INPLACE | XTTS_DEBUG_GEMM_PDL))
-        throw std::runtime_error("debug_gemm: unknown flag bits");
-    const bool out16 = dflags & XTTS_DEBUG_GEMM_OUT16, inplace = dflags & XTTS_DEBUG_GEMM_INPLACE, pdl = dflags & XTTS_DEBUG_GEMM_PDL;
-    if (mode == 0 && (out16 || pdl)) throw std::runtime_error("debug_gemm: 16-bit output and PDL need mode 1 or 2");
-    if (inplace && (!resid || out16)) throw std::runtime_error("debug_gemm: an in-place residual needs resid and fp32 output");
-    if (mode >= 1 && (K % 64 != 0 || N % 32 != 0)) throw std::runtime_error("debug_gemm: modes 1 / 2 need K % 64 == 0 and N % 32 == 0");
+    require_idle();
     CUDA_CHECK(cudaSetDevice(cfg.device));
-    DBuf<float> dA, dW, db, dr, dout;
-    DBuf<__nv_bfloat16> dout16;
-    dA.alloc((size_t)M * K); dW.alloc((size_t)N * K);
-    if (out16) dout16.alloc((size_t)M * N); else dout.alloc((size_t)M * N);
-    dA.upload(A, (size_t)M * K, st); dW.upload(W, (size_t)N * K, st);
-    if (bias) { db.alloc(N); db.upload(bias, N, st); }
-    if (resid && !inplace) { dr.alloc((size_t)M * N); dr.upload(resid, (size_t)M * N, st); }
-    const int flags = ((dflags & XTTS_DEBUG_GEMM_GELU) ? GEMM_GELU : 0) | (resid ? GEMM_RESID : 0) | (out16 ? GEMM_OUT_BF16 : 0) |
-                      (mode == 2 ? GEMM_F16 : 0);
-    DBuf<__nv_bfloat16> hA, hW;                     // 16-bit operands (IEEE fp16 bits in mode 2)
-    if (mode >= 1) {
-        std::string err;
-        if (!gemm_tc_init(&err)) throw std::runtime_error(err);
-        hA.alloc((size_t)M * K); hW.alloc((size_t)N * K);
-        to16(mode, dW.p, hW.p, (size_t)N * K, st);
-    }
-    CUDA_CHECK(cudaStreamSynchronize(st));
-    // in place: out holds the residual and is passed as both (the engine's o-proj / down-proj without split-K)
-    const float* rp = inplace ? dout.p : dr.p;
-    void* op = out16 ? (void*)dout16.p : (void*)dout.p;
-    cudaEvent_t e0, e1;
-    CUDA_CHECK(cudaEventCreate(&e0)); CUDA_CHECK(cudaEventCreate(&e1));
-    auto run = [&] {
-        if (mode >= 1) launch_gemm_bf16_tc(hA.p, hW.p, db.p, rp, op, M, N, K, flags, st, pdl);
-        else launch_gemm_f32(dA.p, dW.p, db.p, rp, dout.p, M, N, K, flags, st);
-    };
-    if (inplace) dout.upload(resid, (size_t)M * N, st);
-    if (mode >= 1) to16(mode, dA.p, hA.p, (size_t)M * K, st);
-    run();
-    CUDA_CHECK(cudaStreamSynchronize(st));
-    if (out16) {
-        std::vector<uint16_t> o((size_t)M * N);
-        dout16.download(reinterpret_cast<__nv_bfloat16*>(o.data()), o.size(), st);
-        CUDA_CHECK(cudaStreamSynchronize(st));
-        widen16(o, mode == 2, out);
-    } else {
-        dout.download(out, (size_t)M * N, st);
-        CUDA_CHECK(cudaStreamSynchronize(st));
-    }
-    if (iters > 0) {
-        CUDA_CHECK(cudaEventRecord(e0, st));
-        for (int i = 0; i < iters; ++i) run();
-        CUDA_CHECK(cudaEventRecord(e1, st));
-        CUDA_CHECK(cudaEventSynchronize(e1));
-        float t = 0; CUDA_CHECK(cudaEventElapsedTime(&t, e0, e1));
-        if (ms) *ms = t / iters;
-    }
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-}
-
-// One launch of the fused sampler (launch_sample) on private per-slot arrays: row r of logits samples for slot active[r]
-// with that slot's parameters, and every state array comes back as the kernel left it.  seen crosses as one byte per id
-// and is packed into ceil(V / 32) bitmap words per slot, as the engine keeps it.
-void Engine::debug_sample_slots(int Vn, int M, const int32_t* active, int n_slots, const float* logits, int ld,
-                                const xtts_sampling* sp, int cap, int advance_ctx, const int32_t* forced, int32_t* n_gen,
-                                int32_t* ctx_len, int32_t* finished, int32_t* last_tok, uint8_t* seen, int32_t* tokens,
-                                int32_t* sampled) {
-    ApiLock lk(this);
-    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
-    if (Vn < 1 || Vn > 2048) throw std::runtime_error("debug_sample_slots: V must be 1..2048");
-    if (n_slots < 1 || M < 1 || M > n_slots) throw std::runtime_error("debug_sample_slots: M must be 1..n_slots");
-    if (ld < Vn) throw std::runtime_error("debug_sample_slots: ld < V");
-    if (cap < 1) throw std::runtime_error("debug_sample_slots: cap must be >= 1");
-    if (!active || !logits || !sp || !n_gen || !ctx_len || !finished || !last_tok || !seen || !tokens || !sampled)
-        throw std::runtime_error("debug_sample_slots: only forced may be NULL");
-    std::vector<char> used(n_slots, 0);
-    for (int i = 0; i < M; ++i) {
-        const int s = active[i];
-        if (s < 0 || s >= n_slots || used[s]) throw std::runtime_error("debug_sample_slots: active slots must be distinct and < n_slots");
-        used[s] = 1;
-        // the kernel reads forced[slot][n_gen] without a bound check and sets the forced id's seen bit
-        if (n_gen[s] < 0) throw std::runtime_error("debug_sample_slots: n_gen must be >= 0");
-        if (forced && n_gen[s] >= cap) throw std::runtime_error("debug_sample_slots: with forced, n_gen must be < cap");
-        if (forced && forced[(size_t)s * cap + n_gen[s]] >= Vn) throw std::runtime_error("debug_sample_slots: forced id >= V");
-    }
-    CUDA_CHECK(cudaSetDevice(cfg.device));
-    const int sw = (Vn + 31) / 32;
-    const size_t nt = (size_t)n_slots * cap;
-    std::vector<unsigned> sb((size_t)n_slots * sw, 0u);
-    for (int s = 0; s < n_slots; ++s)
-        for (int v = 0; v < Vn; ++v)
-            if (seen[(size_t)s * Vn + v]) sb[(size_t)s * sw + (v >> 5)] |= 1u << (v & 31);
-    std::vector<float> T(n_slots), tp(n_slots), pen(n_slots);
-    std::vector<int> tk(n_slots), mt(n_slots), stp(n_slots), ss(n_slots);
-    std::vector<unsigned long long> seed(n_slots);
-    for (int s = 0; s < n_slots; ++s) {
-        T[s] = sp[s].temperature; tp[s] = sp[s].top_p; pen[s] = sp[s].repetition_penalty; tk[s] = sp[s].top_k;
-        mt[s] = sp[s].max_tokens; stp[s] = sp[s].stop_token; ss[s] = sp[s].seq_seed; seed[s] = sp[s].seed;
-    }
-    DBuf<float> dlg, dT, dtp, dpen;
-    DBuf<int> dact, dng, dctx, dfin, dlast, dtok, dsmp, dfor, dtk, dmt, dstp, dss;
-    DBuf<unsigned> dseen;
-    DBuf<unsigned long long> dseed;
-    dlg.alloc((size_t)M * ld); dact.alloc(M);
-    for (auto* b : {&dng, &dctx, &dfin, &dlast, &dtk, &dmt, &dstp, &dss}) b->alloc(n_slots);
-    for (auto* b : {&dT, &dtp, &dpen}) b->alloc(n_slots);
-    dtok.alloc(nt); dsmp.alloc(nt); dseen.alloc(sb.size()); dseed.alloc(n_slots);
-    dlg.upload(logits, (size_t)M * ld, st); dact.upload(active, M, st);
-    dng.upload(n_gen, n_slots, st); dctx.upload(ctx_len, n_slots, st); dfin.upload(finished, n_slots, st);
-    dlast.upload(last_tok, n_slots, st); dtok.upload(tokens, nt, st); dsmp.upload(sampled, nt, st);
-    dseen.upload(sb.data(), sb.size(), st);
-    dT.upload(T.data(), n_slots, st); dtp.upload(tp.data(), n_slots, st); dpen.upload(pen.data(), n_slots, st);
-    dtk.upload(tk.data(), n_slots, st); dmt.upload(mt.data(), n_slots, st); dstp.upload(stp.data(), n_slots, st);
-    dss.upload(ss.data(), n_slots, st); dseed.upload(seed.data(), n_slots, st);
-    if (forced) { dfor.alloc(nt); dfor.upload(forced, nt, st); }
-    SampleState S;
-    S.last_tok = dlast.p; S.n_gen = dng.p; S.ctx_len = dctx.p; S.finished = dfin.p;
-    S.tokens = dtok.p; S.sampled = dsmp.p; S.forced = forced ? dfor.p : nullptr;
-    S.seen = dseen.p; S.temperature = dT.p; S.top_p = dtp.p; S.top_k = dtk.p; S.penalty = dpen.p;
-    S.max_tokens = dmt.p; S.stop_token = dstp.p; S.seed = dseed.p; S.seq_seed = dss.p; S.beam = nullptr;
-    S.tokens_cap = cap; S.seen_words = sw;
-    launch_sample(dlg.p, ld, dact.p, M, Vn, S, advance_ctx, st);
-    dng.download(n_gen, n_slots, st); dctx.download(ctx_len, n_slots, st); dfin.download(finished, n_slots, st);
-    dlast.download(last_tok, n_slots, st); dtok.download(tokens, nt, st); dsmp.download(sampled, nt, st);
-    dseen.download(sb.data(), sb.size(), st);
-    CUDA_CHECK(cudaStreamSynchronize(st));
-    for (int s = 0; s < n_slots; ++s) {
-        for (int v = 0; v < Vn; ++v) seen[(size_t)s * Vn + v] = (uint8_t)((sb[(size_t)s * sw + (v >> 5)] >> (v & 31)) & 1u);
-        if (Vn % 32 && (sb[(size_t)s * sw + sw - 1] >> (Vn % 32)))
-            throw std::runtime_error("debug_sample_slots: the kernel set a seen bit at an id >= V");
-    }
-}
-
-// One launch of the paged decode attention (launch_attn_decode) on private buffers, under the engine's current attention
-// options.  The pools are raw cache-typed arrays in the device layout (kernels.h); they come back with the appended tokens.
-void Engine::debug_attn_decode(int kv_type, int heads, int M, const int32_t* active, int n_slots, const int32_t* ctx_len,
-                               const int32_t* block_tables, int mp, int n_pages, void* kpool, void* vpool,
-                               const float* qkv, float* out) {
-    ApiLock lk(this);
-    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
-    if (kv_type < 0 || kv_type > 2) throw std::runtime_error("debug_attn_decode: kv_type 0 (fp32), 1 (bf16) or 2 (fp16)");
-    if (heads < 1 || M < 1 || n_slots < 1 || mp < 1 || n_pages < 1) throw std::runtime_error("debug_attn_decode: empty problem");
-    // the kernels' contract: distinct active slots, the new token's page inside the block table, page ids inside the pool
-    std::vector<char> used(n_slots, 0);
-    for (int i = 0; i < M; ++i) {
-        const int s = active[i];
-        if (s < 0 || s >= n_slots || used[s]) throw std::runtime_error("debug_attn_decode: active slots must be distinct and < n_slots");
-        used[s] = 1;
-        if (ctx_len[s] < 0 || ctx_len[s] / kPageTokens >= mp) throw std::runtime_error("debug_attn_decode: ctx_len outside the block table");
-        for (int p = 0; p <= ctx_len[s] / kPageTokens; ++p) {
-            const int id = block_tables[(size_t)s * mp + p];
-            if (id < 0 || id >= n_pages) throw std::runtime_error("debug_attn_decode: page id outside the pool");
-        }
-    }
-    CUDA_CHECK(cudaSetDevice(cfg.device));
-    const size_t esz = kv_type == 0 ? 4 : 2;
-    const size_t pool = (size_t)n_pages * heads * kPageTokens * kHeadDim, Hq = (size_t)heads * kHeadDim;
-    DBuf<int> dact, dctx, dbt;
-    DBuf<float> dqkv;
-    DBuf<uint8_t> dk, dv, dout;
-    dact.alloc(M); dctx.alloc(n_slots); dbt.alloc((size_t)n_slots * mp); dqkv.alloc((size_t)M * 3 * Hq);
-    dk.alloc(pool * esz); dv.alloc(pool * esz); dout.alloc((size_t)M * Hq * esz);
-    dact.upload(active, M, st); dctx.upload(ctx_len, n_slots, st); dbt.upload(block_tables, (size_t)n_slots * mp, st);
-    dqkv.upload(qkv, (size_t)M * 3 * Hq, st);
-    dk.upload(static_cast<const uint8_t*>(kpool), pool * esz, st); dv.upload(static_cast<const uint8_t*>(vpool), pool * esz, st);
-    double ctx_sum = 0;
-    for (int i = 0; i < M; ++i) ctx_sum += ctx_len[active[i]];
-    if (kv_type == 0)
-        launch_attn_decode<float, float>(dqkv.p, dact.p, M, dctx.p, dbt.p, mp, reinterpret_cast<float*>(dk.p),
-                                         reinterpret_cast<float*>(dv.p), reinterpret_cast<float*>(dout.p), heads, st, ctx_sum);
-    else if (kv_type == 1)
-        launch_attn_decode<__nv_bfloat16, __nv_bfloat16>(dqkv.p, dact.p, M, dctx.p, dbt.p, mp, reinterpret_cast<__nv_bfloat16*>(dk.p),
-                                                         reinterpret_cast<__nv_bfloat16*>(dv.p),
-                                                         reinterpret_cast<__nv_bfloat16*>(dout.p), heads, st, ctx_sum);
-    else
-        launch_attn_decode<__half, __half>(dqkv.p, dact.p, M, dctx.p, dbt.p, mp, reinterpret_cast<__half*>(dk.p),
-                                           reinterpret_cast<__half*>(dv.p), reinterpret_cast<__half*>(dout.p), heads, st, ctx_sum);
-    dk.download(static_cast<uint8_t*>(kpool), pool * esz, st); dv.download(static_cast<uint8_t*>(vpool), pool * esz, st);
-    if (kv_type == 0) {
-        dout.download(reinterpret_cast<uint8_t*>(out), (size_t)M * Hq * 4, st);
-        CUDA_CHECK(cudaStreamSynchronize(st));
-    } else {
-        std::vector<uint16_t> o((size_t)M * Hq);
-        dout.download(reinterpret_cast<uint8_t*>(o.data()), o.size() * 2, st);
-        CUDA_CHECK(cudaStreamSynchronize(st));
-        widen16(o, kv_type == 2, out);
-    }
-}
-
-// One beam step on caller arrays for one group of nb beams in slots 0..nb-1: logprob, select, reorder and the partial-page
-// copy (launch_beam_step without the gather), every input and output on the host (include/xtts_b200.h)
-void Engine::debug_beam_step(int kv_type, int heads, int layers, int Vn, const xtts_sampling& sp, const xtts_beam& bm, int first,
-                             int advance, const float* logits, int32_t* n_gen, int32_t* ctx_len, int32_t* last_tok,
-                             uint32_t* seen, int mp, int32_t* block_tables, int n_pages, int32_t* pool, int cap, int32_t* hist,
-                             xtts_beam_state* state, void* kpool, void* vpool, float* scores) {
-    static_assert(sizeof(xtts_beam_state) == sizeof(BeamState), "xtts_beam_state mirrors BeamState");
-    ApiLock lk(this);
-    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
-    const int nb = bm.num_beams;
-    auto bad = [](const char* m) { throw std::runtime_error(std::string("debug_beam_step: ") + m); };
-    if (kv_type < 0 || kv_type > 2) bad("kv_type 0 (fp32), 1 (bf16) or 2 (fp16)");
-    if (nb < 2 || nb > kMaxBeams) bad("num_beams 2..8");
-    if (heads < 1 || layers < 1 || Vn < 2 * nb || n_pages < 1 || cap < 1 || mp < 1) bad("empty problem");
-    if (!beam_supported(Vn, mp, cap)) bad("geometry outside the beam kernels' limits");
-    const int W = ceil_div(Vn, 32), pool_cap = nb * mp;
-    BeamState bs;
-    std::memcpy(&bs, state, sizeof(bs));
-    if (bs.n_free < nb || bs.n_free > pool_cap) bad("the pool must hold nb .. nb * max_pages pages");
-    for (int i = 0; i < bs.n_free; ++i) if (pool[i] < 0 || pool[i] >= n_pages) bad("pool page outside the pool");
-    // every beam that owns pages holds exactly those of its KV positions [0, L), L = ctx_len + advance; the pool and the
-    // tables together never exceed nb * max_pages entries
-    const int L = ctx_len[0] + advance;
-    if (L < 1 || L / kPageTokens >= mp) bad("the next position must lie inside the block table");
-    int held = 0;
-    for (int j = 0; j < nb; ++j) {
-        if (n_gen[j] != n_gen[0] || ctx_len[j] != ctx_len[0]) bad("the beams of a group share n_gen and ctx_len");
-        const int np = first && j > 0 ? 0 : bs.n_pages[j];
-        if (np != (first && j > 0 ? 0 : ceil_div(L, kPageTokens))) bad("n_pages must cover the KV positions [0, ctx_len + advance)");
-        for (int k = 0; k < np; ++k)
-            if (block_tables[(size_t)j * mp + k] < 0 || block_tables[(size_t)j * mp + k] >= n_pages) bad("page id outside the pool");
-        held += np;
-    }
-    if (held + bs.n_free > pool_cap) bad("pool and tables exceed nb * max_pages pages");
-    if (n_gen[0] < 0 || n_gen[0] >= cap) bad("n_gen outside the history");
-    CUDA_CHECK(cudaSetDevice(cfg.device));
-    const size_t esz = kv_type == 0 ? 4 : 2;
-    const size_t page_bytes = (size_t)heads * kPageTokens * kHeadDim * esz, pool_bytes = (size_t)layers * n_pages * page_bytes;
-    DBuf<int> dng, dctx, dlast, dfin, dtok, dtk, dmt, dstop, dss, dbt, dpool;
-    DBuf<float> dT, dtp, dpen, dlog, dsc;
-    DBuf<unsigned long long> dseed;
-    DBuf<unsigned> dseen;
-    DBuf<BeamState> dstate;
-    DBuf<BeamDesc> ddesc;
-    DBuf<int2> dhist;
-    DBuf<uint8_t> dk, dv;
-    DBuf<void*> dptr;
-    dng.alloc(nb); dctx.alloc(nb); dlast.alloc(nb); dfin.alloc(nb); dtok.alloc((size_t)nb * cap); dtk.alloc(nb); dmt.alloc(nb);
-    dstop.alloc(nb); dss.alloc(nb); dbt.alloc((size_t)nb * mp); dpool.alloc(pool_cap); dT.alloc(nb); dtp.alloc(nb); dpen.alloc(nb);
-    dlog.alloc((size_t)nb * Vn); dsc.alloc((size_t)nb * Vn); dseed.alloc(nb); dseen.alloc((size_t)nb * W); dstate.alloc(1);
-    ddesc.alloc(1); dhist.alloc((size_t)cap * kMaxBeams); dk.alloc(pool_bytes); dv.alloc(pool_bytes); dptr.alloc(2 * layers);
-    std::vector<int> v_tk(nb, sp.top_k), v_mt(nb, sp.max_tokens), v_stop(nb, sp.stop_token), v_ss(nb, sp.seq_seed);
-    std::vector<float> v_T(nb, sp.temperature), v_tp(nb, sp.top_p), v_pen(nb, sp.repetition_penalty);
-    std::vector<unsigned long long> v_seed(nb, sp.seed);
-    std::vector<void*> ptr(2 * layers);
-    for (int l = 0; l < layers; ++l) { ptr[l] = dk.p + l * n_pages * page_bytes; ptr[layers + l] = dv.p + l * n_pages * page_bytes; }
-    BeamDesc d{};
-    d.primary = 0; d.nb = nb; d.first = first != 0; d.advance = advance; d.do_sample = bm.do_sample != 0;
-    d.length_penalty = bm.length_penalty;
-    for (int j = 0; j < kMaxBeams; ++j) { d.slot[j] = j < nb ? j : -1; d.row[j] = j < nb ? (first ? 0 : j) : 0; }
-    dng.upload(n_gen, nb, st); dctx.upload(ctx_len, nb, st); dfin.zero(st); dtok.zero(st);
-    dtk.upload(v_tk.data(), nb, st); dmt.upload(v_mt.data(), nb, st); dstop.upload(v_stop.data(), nb, st); dss.upload(v_ss.data(), nb, st);
-    dT.upload(v_T.data(), nb, st); dtp.upload(v_tp.data(), nb, st); dpen.upload(v_pen.data(), nb, st); dseed.upload(v_seed.data(), nb, st);
-    dseen.upload(seen, (size_t)nb * W, st); dbt.upload(block_tables, (size_t)nb * mp, st); dpool.upload(pool, pool_cap, st);
-    dlog.upload(logits, (size_t)(first ? 1 : nb) * Vn, st); dstate.upload(&bs, 1, st); ddesc.upload(&d, 1, st);
-    dhist.upload(reinterpret_cast<const int2*>(hist), (size_t)cap * kMaxBeams, st);
-    dk.upload(static_cast<const uint8_t*>(kpool), pool_bytes, st); dv.upload(static_cast<const uint8_t*>(vpool), pool_bytes, st);
-    dptr.upload(ptr.data(), 2 * layers, st);
-    SampleState S{};
-    S.last_tok = dlast.p; S.n_gen = dng.p; S.ctx_len = dctx.p; S.finished = dfin.p; S.tokens = dtok.p; S.sampled = nullptr;
-    S.forced = nullptr; S.seen = dseen.p; S.temperature = dT.p; S.top_p = dtp.p; S.top_k = dtk.p; S.penalty = dpen.p;
-    S.max_tokens = dmt.p; S.stop_token = dstop.p; S.seed = dseed.p; S.seq_seed = dss.p; S.beam = nullptr;
-    S.tokens_cap = cap; S.seen_words = W;
-    BeamArgs a{};
-    a.desc = ddesc.p; a.n_groups = 1; a.state = dstate.p; a.hist = dhist.p; a.pool = dpool.p; a.pool_cap = pool_cap;
-    a.scores = dsc.p; a.block_tables = dbt.p; a.max_pages = mp; a.latents = nullptr; a.H = 0;
-    launch_beam_step(dlog.p, Vn, Vn, S, a, dptr.p, dptr.p + layers, layers, heads, (int)esz, st, false);
-    dng.download(n_gen, nb, st); dctx.download(ctx_len, nb, st); dlast.download(last_tok, nb, st);
-    dseen.download(seen, (size_t)nb * W, st); dbt.download(block_tables, (size_t)nb * mp, st); dpool.download(pool, pool_cap, st);
-    dstate.download(&bs, 1, st); dhist.download(reinterpret_cast<int2*>(hist), (size_t)cap * kMaxBeams, st);
-    dk.download(static_cast<uint8_t*>(kpool), pool_bytes, st); dv.download(static_cast<uint8_t*>(vpool), pool_bytes, st);
-    dsc.download(scores, (size_t)nb * Vn, st);
-    CUDA_CHECK(cudaStreamSynchronize(st));
-    std::memcpy(state, &bs, sizeof(bs));
-}
-
-// One launch of the prefill / encoder attention (launch_attn_generic).  q rows and k / v rows are addressed with the given
-// strides (k at kv + k_off, v at kv + v_off); out is [out_rows][heads * 64], rows no sequence covers keep their NaN fill.
-void Engine::debug_attn_prefill(int out_type, int heads, const int32_t* seqs, int nseq, int causal, float scale,
-                                const float* q, int64_t q_len, int q_row_stride, int q_head_stride,
-                                const float* kv, int64_t kv_len, int kv_row_stride, int kv_head_stride, int64_t k_off,
-                                int64_t v_off, float* out, int out_rows) {
-    ApiLock lk(this);
-    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
-    if (out_type < 0 || out_type > 2) throw std::runtime_error("debug_attn_prefill: out_type 0 (fp32), 1 (bf16) or 2 (fp16)");
-    if (heads < 1 || nseq < 1 || out_rows < 1 || q_len < 1 || kv_len < 1) throw std::runtime_error("debug_attn_prefill: empty problem");
-    const int Hq = heads * kHeadDim;
-    int max_nq = 0;
-    auto last = [&](int64_t row, int64_t rs, int64_t hs) { return row * rs + (int64_t)(heads - 1) * hs + kHeadDim - 1; };
-    for (int i = 0; i < nseq; ++i) {
-        const int32_t* s = seqs + 4 * i;        // q_start, nq, kv_start, nk
-        if (s[0] < 0 || s[1] < 1 || s[2] < 0 || s[3] < 1 || s[0] + s[1] > out_rows)
-            throw std::runtime_error("debug_attn_prefill: sequence outside the output rows");
-        if (causal && s[3] < s[1]) throw std::runtime_error("debug_attn_prefill: causal attention needs nk >= nq");
-        if (last(s[0] + s[1] - 1, q_row_stride, q_head_stride) >= q_len ||
-            std::max(k_off, v_off) + last(s[2] + s[3] - 1, kv_row_stride, kv_head_stride) >= kv_len || std::min(k_off, v_off) < 0)
-            throw std::runtime_error("debug_attn_prefill: sequence outside the q / kv buffers");
-        max_nq = std::max(max_nq, (int)s[1]);
-    }
-    CUDA_CHECK(cudaSetDevice(cfg.device));
-    const size_t esz = out_type == 0 ? 4 : 2, n_out = (size_t)out_rows * Hq;
-    DBuf<float> dq, dkv;
-    DBuf<AttnSeq> dseq;
-    DBuf<uint8_t> dout;
-    dq.alloc(q_len); dkv.alloc(kv_len); dseq.alloc(nseq); dout.alloc(n_out * esz);
-    dq.upload(q, q_len, st); dkv.upload(kv, kv_len, st);
-    dseq.upload(reinterpret_cast<const AttnSeq*>(seqs), nseq, st);
-    CUDA_CHECK(cudaMemsetAsync(dout.p, 0xFF, n_out * esz, st));        // NaN in every output type
-    AttnLayout A;
-    A.q = dq.p; A.k = dkv.p + k_off; A.v = dkv.p + v_off;
-    A.q_row_stride = q_row_stride; A.kv_row_stride = kv_row_stride; A.q_head_stride = q_head_stride; A.kv_head_stride = kv_head_stride;
-    A.heads = heads; A.scale = scale; A.causal = causal ? 1 : 0;
-    if (out_type == 0) launch_attn_generic<float>(A, dseq.p, nseq, max_nq, reinterpret_cast<float*>(dout.p), Hq, st);
-    else if (out_type == 1) launch_attn_generic<__nv_bfloat16>(A, dseq.p, nseq, max_nq, reinterpret_cast<__nv_bfloat16*>(dout.p), Hq, st);
-    else launch_attn_generic<__half>(A, dseq.p, nseq, max_nq, reinterpret_cast<__half*>(dout.p), Hq, st);
-    if (out_type == 0) {
-        dout.download(reinterpret_cast<uint8_t*>(out), n_out * 4, st);
-        CUDA_CHECK(cudaStreamSynchronize(st));
-    } else {
-        std::vector<uint16_t> o(n_out);
-        dout.download(reinterpret_cast<uint8_t*>(o.data()), n_out * 2, st);
-        CUDA_CHECK(cudaStreamSynchronize(st));
-        widen16(o, out_type == 2, out);
-    }
-}
-
-// The decode step's split-K projection + residual / LayerNorm pair, as layers_forward runs it: the 16-bit GEMM into fp32
-// partials, then X += bias + sum of the partials and Y = LN(X) (Y skipped without ln_w / ln_b: the last layer's form).
-void Engine::debug_splitk_ln(int mode, int M, int N, int K, int splits, const float* A, const float* W, const float* bias,
-                             float* X, const float* ln_w, const float* ln_b, float* Y) {
-    ApiLock lk(this);
-    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
-    if (mode != 1 && mode != 2) throw std::runtime_error("debug_splitk_ln: mode 1 (bf16) or 2 (fp16)");
-    if (M < 1 || N < 32 || N % 32 != 0 || N > 8192 || K < 64 || K % 64 != 0 || splits < 1 || splits > 8 || (K / 64) % splits != 0)
-        throw std::runtime_error("debug_splitk_ln: need N % 32 == 0 (<= 8192), K % 64 == 0, 1 <= splits <= 8 dividing K / 64");
-    if (!bias || (ln_w == nullptr) != (ln_b == nullptr) || (ln_w && !Y)) throw std::runtime_error("debug_splitk_ln: bias, and ln_w / ln_b / Y together");
-    CUDA_CHECK(cudaSetDevice(cfg.device));
-    std::string err;
-    if (!gemm_tc_init(&err)) throw std::runtime_error(err);
-    DBuf<float> dA, dW, db, dX, dlw, dlb, dpart;
-    DBuf<__nv_bfloat16> hA, hW, dY;                 // 16-bit operands / output (IEEE fp16 bits in mode 2)
-    dA.alloc((size_t)M * K); dW.alloc((size_t)N * K); db.alloc(N); dX.alloc((size_t)M * N); dpart.alloc((size_t)splits * M * N);
-    hA.alloc((size_t)M * K); hW.alloc((size_t)N * K);
-    dA.upload(A, (size_t)M * K, st); dW.upload(W, (size_t)N * K, st); db.upload(bias, N, st); dX.upload(X, (size_t)M * N, st);
-    if (ln_w) {
-        dlw.alloc(N); dlb.alloc(N); dY.alloc((size_t)M * N);
-        dlw.upload(ln_w, N, st); dlb.upload(ln_b, N, st);
-    }
-    if (mode == 1) {
-        launch_f32_to_bf16(dA.p, hA.p, (size_t)M * K, st); launch_f32_to_bf16(dW.p, hW.p, (size_t)N * K, st);
-    } else {
-        launch_f32_to_f16(dA.p, reinterpret_cast<__half*>(hA.p), (size_t)M * K, st);
-        launch_f32_to_f16(dW.p, reinterpret_cast<__half*>(hW.p), (size_t)N * K, st);
-    }
-    launch_gemm_bf16_tc_splitk(hA.p, hW.p, dpart.p, M, N, K, splits, st, false, mode == 2 ? GEMM_F16 : 0);
-    if (mode == 2)
-        launch_residual_reduce_layernorm<__half>(dX.p, dpart.p, splits, db.p, dlw.p, dlb.p, reinterpret_cast<__half*>(dY.p), M, N,
-                                                 cfg.ln_eps, st);
-    else
-        launch_residual_reduce_layernorm<__nv_bfloat16>(dX.p, dpart.p, splits, db.p, dlw.p, dlb.p, dY.p, M, N, cfg.ln_eps, st);
-    dX.download(X, (size_t)M * N, st);
-    std::vector<uint16_t> y(ln_w ? (size_t)M * N : 0);
-    if (ln_w) dY.download(reinterpret_cast<__nv_bfloat16*>(y.data()), y.size(), st);
-    CUDA_CHECK(cudaStreamSynchronize(st));
-    if (ln_w) widen16(y, mode == 2, Y);
-}
-
-// The decode step's LayerNorm -> GEMM pair as decode_layers_rows launches it: the 16-bit LayerNorm into the operand buffer,
-// then the one-tile GEMM on it.  launch 0: plain launches; 1: both with PDL.
-void Engine::debug_ln_gemm(int mode, int launch, int M, int N, int K, const float* X, const float* ln_w, const float* ln_b,
-                           const float* W, const float* bias, const float* resid, int dflags, float* Y, float* out) {
-    ApiLock lk(this);
-    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
-    if (mode != 1 && mode != 2) throw std::runtime_error("debug_ln_gemm: mode 1 (bf16) or 2 (fp16)");
-    if (launch < 0 || launch > 1) throw std::runtime_error("debug_ln_gemm: launch 0 (plain) or 1 (PDL)");
-    if (M < 1 || N < 32 || N % 32 != 0 || K < 64 || K % 64 != 0 || K > 8192) throw std::runtime_error("debug_ln_gemm: need M >= 1, N % 32 == 0, K % 64 == 0 (<= 8192)");
-    if (dflags & ~(XTTS_DEBUG_GEMM_GELU | XTTS_DEBUG_GEMM_OUT16)) throw std::runtime_error("debug_ln_gemm: flags GELU / OUT16 only");
-    if (!X || !ln_w || !ln_b || !W || !Y || !out) throw std::runtime_error("debug_ln_gemm: only bias and resid may be NULL");
-    if (resid && (dflags & XTTS_DEBUG_GEMM_OUT16)) throw std::runtime_error("debug_ln_gemm: a residual needs fp32 output");
-    CUDA_CHECK(cudaSetDevice(cfg.device));
-    std::string err;
-    if (!gemm_tc_init(&err)) throw std::runtime_error(err);
-    const bool out16 = dflags & XTTS_DEBUG_GEMM_OUT16;
-    DBuf<float> dX, dlw, dlb, dW, db, dr, dout;
-    DBuf<__nv_bfloat16> hW, dY, dout16;
-    dX.alloc((size_t)M * K); dlw.alloc(K); dlb.alloc(K); dW.alloc((size_t)N * K); hW.alloc((size_t)N * K); dY.alloc((size_t)M * K);
-    if (out16) dout16.alloc((size_t)M * N); else dout.alloc((size_t)M * N);
-    dX.upload(X, (size_t)M * K, st); dlw.upload(ln_w, K, st); dlb.upload(ln_b, K, st); dW.upload(W, (size_t)N * K, st);
-    if (bias) { db.alloc(N); db.upload(bias, N, st); }
-    if (resid) { dr.alloc((size_t)M * N); dr.upload(resid, (size_t)M * N, st); }
-    to16(mode, dW.p, hW.p, (size_t)N * K, st);
-    CUDA_CHECK(cudaStreamSynchronize(st));
-    const bool pdl = launch == 1;
-    if (mode == 2) launch_layernorm<__half>(dX.p, dlw.p, dlb.p, reinterpret_cast<__half*>(dY.p), M, K, cfg.ln_eps, st, pdl);
-    else launch_layernorm<__nv_bfloat16>(dX.p, dlw.p, dlb.p, dY.p, M, K, cfg.ln_eps, st, pdl);
-    const int flags = ((dflags & XTTS_DEBUG_GEMM_GELU) ? GEMM_GELU : 0) | (out16 ? GEMM_OUT_BF16 : 0) | (resid ? GEMM_RESID : 0) |
-                      (mode == 2 ? GEMM_F16 : 0);
-    launch_gemm_bf16_tc(dY.p, hW.p, db.p, dr.p, out16 ? (void*)dout16.p : (void*)dout.p, M, N, K, flags, st, pdl);
-    std::vector<uint16_t> y((size_t)M * K), o16(out16 ? (size_t)M * N : 0);
-    dY.download(reinterpret_cast<__nv_bfloat16*>(y.data()), y.size(), st);
-    if (out16) dout16.download(reinterpret_cast<__nv_bfloat16*>(o16.data()), o16.size(), st);
-    else dout.download(out, (size_t)M * N, st);
-    CUDA_CHECK(cudaStreamSynchronize(st));
-    widen16(y, mode == 2, Y);
-    if (out16) widen16(o16, mode == 2, out);
-}
-
-// launch_layernorm (w2 == NULL) or launch_head_norms (w2 != NULL) in the output type `out_type` on private buffers
-void Engine::debug_norms(int out_type, int M, int H, const float* X, int x_rows, const int32_t* row_index, const float* w1,
-                         const float* b1, const float* w2, const float* b2, float* Y, float* latents, int n_slots,
-                         int lat_rows, const int32_t* slots, const int32_t* lat_pos, const int32_t* n_gen) {
-    ApiLock lk(this);
-    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
-    if (out_type < 0 || out_type > 2) throw std::runtime_error("debug_norms: out_type 0 (fp32), 1 (bf16) or 2 (fp16)");
-    if (M < 1 || H < 1 || H > 8192 || x_rows < 1) throw std::runtime_error("debug_norms: need M >= 1, 1 <= H <= 8192, x_rows >= 1");
-    if (!X || !w1 || !b1 || !Y || (w2 == nullptr) != (b2 == nullptr)) throw std::runtime_error("debug_norms: X, w1, b1, Y, and w2 / b2 together");
-    const bool head = w2 != nullptr;
-    if (!head && (row_index || latents || x_rows < M)) throw std::runtime_error("debug_norms: a plain LayerNorm reads rows 0 .. M-1 and has no latents");
-    if (row_index)
-        for (int i = 0; i < M; ++i)
-            if (row_index[i] < 0 || row_index[i] >= x_rows) throw std::runtime_error("debug_norms: row_index outside X");
-    if (!row_index && x_rows < M) throw std::runtime_error("debug_norms: X has fewer than M rows");
-    if (latents) {
-        if (!slots || n_slots < 1 || lat_rows < 1 || (!lat_pos && !n_gen)) throw std::runtime_error("debug_norms: latents need slots, n_slots, lat_rows and lat_pos or n_gen");
-        for (int i = 0; i < M; ++i)
-            if (slots[i] < 0 || slots[i] >= n_slots) throw std::runtime_error("debug_norms: slot outside n_slots");
-    }
-    CUDA_CHECK(cudaSetDevice(cfg.device));
-    const size_t esz = out_type == 0 ? 4 : 2, nlat = latents ? (size_t)n_slots * lat_rows * H : 0;
-    DBuf<float> dX, dw1, db1, dw2, db2, dlat;
-    DBuf<int> dri, dsl, dlp, dng;
-    DBuf<uint8_t> dY;
-    dX.alloc((size_t)x_rows * H); dw1.alloc(H); db1.alloc(H); dY.alloc((size_t)M * H * esz);
-    dX.upload(X, (size_t)x_rows * H, st); dw1.upload(w1, H, st); db1.upload(b1, H, st);
-    if (head) { dw2.alloc(H); db2.alloc(H); dw2.upload(w2, H, st); db2.upload(b2, H, st); }
-    if (row_index) { dri.alloc(M); dri.upload(row_index, M, st); }
-    if (latents) {
-        dlat.alloc(nlat); dlat.upload(latents, nlat, st);
-        dsl.alloc(M); dsl.upload(slots, M, st);
-        if (lat_pos) { dlp.alloc(M); dlp.upload(lat_pos, M, st); }
-        if (n_gen) { dng.alloc(n_slots); dng.upload(n_gen, n_slots, st); }
-    }
-    const float eps = cfg.ln_eps;
-    auto run = [&](auto* y) {
-        using T = std::remove_pointer_t<decltype(y)>;
-        if (!head) launch_layernorm<T>(dX.p, dw1.p, db1.p, y, M, H, eps, st);
-        else launch_head_norms<T>(dX.p, dri.p, dw1.p, db1.p, dw2.p, db2.p, y, latents ? dlat.p : nullptr, dsl.p, dlp.p, dng.p,
-                                  lat_rows, M, H, eps, st);
-    };
-    if (out_type == 0) run(reinterpret_cast<float*>(dY.p));
-    else if (out_type == 1) run(reinterpret_cast<__nv_bfloat16*>(dY.p));
-    else run(reinterpret_cast<__half*>(dY.p));
-    if (latents) dlat.download(latents, nlat, st);
-    if (out_type == 0) {
-        dY.download(reinterpret_cast<uint8_t*>(Y), (size_t)M * H * 4, st);
-        CUDA_CHECK(cudaStreamSynchronize(st));
-    } else {
-        std::vector<uint16_t> y((size_t)M * H);
-        dY.download(reinterpret_cast<uint8_t*>(y.data()), y.size() * 2, st);
-        CUDA_CHECK(cudaStreamSynchronize(st));
-        widen16(y, out_type == 2, Y);
-    }
-}
-
-// launch_kv_write (the prefill's paged-cache write) over raw pools in the device layout, updated in place
-void Engine::debug_kv_write(int kv_type, int heads, int M, const float* qkv, const int32_t* row_slot, const int32_t* row_pos,
-                            int n_slots, const int32_t* ctx_len, const int32_t* block_tables, int mp, int n_pages, void* kpool,
-                            void* vpool) {
-    ApiLock lk(this);
-    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
-    if (kv_type < 0 || kv_type > 2) throw std::runtime_error("debug_kv_write: kv_type 0 (fp32), 1 (bf16) or 2 (fp16)");
-    if (heads < 1 || M < 1 || n_slots < 1 || mp < 1 || n_pages < 1) throw std::runtime_error("debug_kv_write: empty problem");
-    if (!qkv || !row_slot || !block_tables || !kpool || !vpool || (!row_pos && !ctx_len)) throw std::runtime_error("debug_kv_write: row_pos or ctx_len, and every other pointer");
-    for (int r = 0; r < M; ++r) {
-        const int s = row_slot[r];
-        if (s < 0 || s >= n_slots) throw std::runtime_error("debug_kv_write: row slot outside n_slots");
-        const int pos = row_pos ? row_pos[r] : ctx_len[s];
-        if (pos < 0 || pos / kPageTokens >= mp) throw std::runtime_error("debug_kv_write: position outside the block table");
-        const int id = block_tables[(size_t)s * mp + pos / kPageTokens];
-        if (id < 0 || id >= n_pages) throw std::runtime_error("debug_kv_write: page id outside the pool");
-    }
-    CUDA_CHECK(cudaSetDevice(cfg.device));
-    const size_t esz = kv_type == 0 ? 4 : 2;
-    const size_t pool = (size_t)n_pages * heads * kPageTokens * kHeadDim, Hq = (size_t)heads * kHeadDim;
-    DBuf<int> dslot, dpos, dctx, dbt;
-    DBuf<float> dqkv;
-    DBuf<uint8_t> dk, dv;
-    dslot.alloc(M); dbt.alloc((size_t)n_slots * mp); dqkv.alloc((size_t)M * 3 * Hq); dk.alloc(pool * esz); dv.alloc(pool * esz);
-    dslot.upload(row_slot, M, st); dbt.upload(block_tables, (size_t)n_slots * mp, st); dqkv.upload(qkv, (size_t)M * 3 * Hq, st);
-    if (row_pos) { dpos.alloc(M); dpos.upload(row_pos, M, st); }
-    if (ctx_len) { dctx.alloc(n_slots); dctx.upload(ctx_len, n_slots, st); }
-    dk.upload(static_cast<const uint8_t*>(kpool), pool * esz, st); dv.upload(static_cast<const uint8_t*>(vpool), pool * esz, st);
-    if (kv_type == 0)
-        launch_kv_write<float>(dqkv.p, M, dslot.p, dpos.p, dctx.p, dbt.p, mp, reinterpret_cast<float*>(dk.p), reinterpret_cast<float*>(dv.p), heads, st);
-    else if (kv_type == 1)
-        launch_kv_write<__nv_bfloat16>(dqkv.p, M, dslot.p, dpos.p, dctx.p, dbt.p, mp, reinterpret_cast<__nv_bfloat16*>(dk.p),
-                                       reinterpret_cast<__nv_bfloat16*>(dv.p), heads, st);
-    else
-        launch_kv_write<__half>(dqkv.p, M, dslot.p, dpos.p, dctx.p, dbt.p, mp, reinterpret_cast<__half*>(dk.p), reinterpret_cast<__half*>(dv.p), heads, st);
-    dk.download(static_cast<uint8_t*>(kpool), pool * esz, st); dv.download(static_cast<uint8_t*>(vpool), pool * esz, st);
-    CUDA_CHECK(cudaStreamSynchronize(st));
-}
-
-// launch_build_rows over private embedding tables: rows [n_rows][4] = RowDesc (kind, a, b, c)
-void Engine::debug_build_rows(int Hd, int n_cond, const float* text_emb, int n_text, const float* text_pos, int n_tpos,
-                              const float* wte_h, int n_audio, const float* wpe_h, int n_wpe, const float* spk, int n_spk,
-                              const int32_t* rows, int n_rows, float* X) {
-    ApiLock lk(this);
-    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
-    if (Hd < 4 || Hd % 4 != 0 || n_rows < 1 || n_cond < 1 || n_text < 1 || n_tpos < 1 || n_audio < 1 || n_wpe < 1 || n_spk < 1)
-        throw std::runtime_error("debug_build_rows: need H % 4 == 0 and non-empty tables and rows");
-    if (!text_emb || !text_pos || !wte_h || !wpe_h || !spk || !rows || !X) throw std::runtime_error("debug_build_rows: NULL argument");
-    for (int i = 0; i < n_rows; ++i) {
-        const int32_t* r = rows + 4 * i;
-        const bool ok = r[0] == 0 ? (r[1] >= 0 && r[1] < n_cond && r[3] >= 0 && r[3] < n_spk)
-                      : r[0] == 1 ? (r[1] >= 0 && r[1] < n_text && r[2] >= 0 && r[2] < n_tpos)
-                      : r[0] == 2 ? (r[1] >= 0 && r[1] < n_audio && r[2] >= 0 && r[2] < n_wpe) : false;
-        if (!ok) throw std::runtime_error("debug_build_rows: row kind outside 0..2 or index outside its table");
-    }
-    CUDA_CHECK(cudaSetDevice(cfg.device));
-    DBuf<float> dte, dtp, dwte, dwpe, dspk, dX;
-    DBuf<RowDesc> drows;
-    dte.alloc((size_t)n_text * Hd); dtp.alloc((size_t)n_tpos * Hd); dwte.alloc((size_t)n_audio * Hd); dwpe.alloc((size_t)n_wpe * Hd);
-    dspk.alloc((size_t)n_spk * n_cond * Hd); dX.alloc((size_t)n_rows * Hd); drows.alloc(n_rows);
-    dte.upload(text_emb, (size_t)n_text * Hd, st); dtp.upload(text_pos, (size_t)n_tpos * Hd, st);
-    dwte.upload(wte_h, (size_t)n_audio * Hd, st); dwpe.upload(wpe_h, (size_t)n_wpe * Hd, st);
-    dspk.upload(spk, (size_t)n_spk * n_cond * Hd, st);
-    static_assert(sizeof(RowDesc) == 4 * sizeof(int32_t), "RowDesc crosses the ABI as four int32");
-    drows.upload(reinterpret_cast<const RowDesc*>(rows), n_rows, st);
-    GptTables t; t.text_emb = dte.p; t.text_pos = dtp.p; t.wte = dwte.p; t.wpe = dwpe.p; t.spk_cond = dspk.p; t.H = Hd; t.n_cond = n_cond;
-    launch_build_rows(drows.p, n_rows, t, dX.p, st);
-    dX.download(X, (size_t)n_rows * Hd, st);
-    CUDA_CHECK(cudaStreamSynchronize(st));
-}
-
-// launch_build_decode_rows over private tables and slot arrays
-void Engine::debug_build_decode_rows(int Hd, const float* wte_h, int n_audio, const float* wpe_h, int n_wpe, int M,
-                                     const int32_t* active, int n_slots, const int32_t* last_tok, const int32_t* n_gen, float* X) {
-    ApiLock lk(this);
-    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
-    if (Hd < 4 || Hd % 4 != 0 || M < 1 || n_slots < 1 || n_audio < 1 || n_wpe < 1) throw std::runtime_error("debug_build_decode_rows: need H % 4 == 0, M >= 1 and non-empty tables");
-    if (!wte_h || !wpe_h || !active || !last_tok || !n_gen || !X) throw std::runtime_error("debug_build_decode_rows: NULL argument");
-    for (int i = 0; i < M; ++i) {
-        const int s = active[i];
-        if (s < 0 || s >= n_slots) throw std::runtime_error("debug_build_decode_rows: active slot outside n_slots");
-        if (last_tok[s] < 0 || last_tok[s] >= n_audio || n_gen[s] < 0 || n_gen[s] >= n_wpe)
-            throw std::runtime_error("debug_build_decode_rows: last_tok / n_gen outside the tables");
-    }
-    CUDA_CHECK(cudaSetDevice(cfg.device));
-    DBuf<float> dwte, dwpe, dX;
-    DBuf<int> dact, dlast, dng;
-    dwte.alloc((size_t)n_audio * Hd); dwpe.alloc((size_t)n_wpe * Hd); dX.alloc((size_t)M * Hd);
-    dact.alloc(M); dlast.alloc(n_slots); dng.alloc(n_slots);
-    dwte.upload(wte_h, (size_t)n_audio * Hd, st); dwpe.upload(wpe_h, (size_t)n_wpe * Hd, st);
-    dact.upload(active, M, st); dlast.upload(last_tok, n_slots, st); dng.upload(n_gen, n_slots, st);
-    GptTables t{}; t.wte = dwte.p; t.wpe = dwpe.p; t.H = Hd;
-    launch_build_decode_rows(dact.p, M, dlast.p, dng.p, t, dX.p, st, use_pdl);
-    dX.download(X, (size_t)M * Hd, st);
-    CUDA_CHECK(cudaStreamSynchronize(st));
-}
-
-// One launch of the fast-mode vocoder convolution (launch_conv1d_tc, or launch_convT_tc for up > 0) with the weights
-// packed and planned as make_conv does.  The input atom image is NaN except each item's signal rows; the production pad
-// routine then clears what it claims the kernel reads, so any other read reaches a stored output as NaN.  out32 / out16
-// are in/out: their incoming contents are the accumulate base and the sentinels of every row the kernel must not write.
-void Engine::debug_conv_tc(int up, int Cin, int Cout, int K, int dil, int batch, int L, const int32_t* item_len,
-                           const float* w, const float* bias, const float* cbias, int cbias_stride, const float* x,
-                           const float* resid, int mode, float slope_out, float scale16, int max_ctas, float* out32,
-                           float* out16) {
-    ApiLock lk(this);
-    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
-    if (up != 0 && up != 2 && up != 4 && up != 8) throw std::runtime_error("debug_conv_tc: up 0 (Conv1d) or 2, 4, 8 (ConvTranspose1d)");
-    if (up == 0 && (K < 1 || K % 2 == 0 || dil < 1)) throw std::runtime_error("debug_conv_tc: Conv1d needs an odd K and dil >= 1");
-    if (up > 0 && (K != 2 * up || dil != 1)) throw std::runtime_error("debug_conv_tc: ConvTranspose1d needs K = 2 * up and dil = 1");
-    if (up > 0 && (resid || mode != CONV_STORE || scale16 != 1.0f))
-        throw std::runtime_error("debug_conv_tc: ConvTranspose1d takes no resid, mode STORE and scale16 1");
-    if (mode != CONV_STORE && mode != CONV_ACCUM) throw std::runtime_error("debug_conv_tc: mode 0 (store) or 1 (accumulate)");
-    if (mode == CONV_ACCUM && !out32) throw std::runtime_error("debug_conv_tc: accumulate mode needs out32");
-    if (up == 0 && (K - 1) / 2 * dil > kAtomPadL) throw std::runtime_error("debug_conv_tc: halo (K-1)/2*dil exceeds the atom head pad");
-    if (batch < 1 || batch > kVocMaxItems) throw std::runtime_error("debug_conv_tc: batch must be 1..32");
-    if (L < 1) throw std::runtime_error("debug_conv_tc: L must be >= 1");
-    if (!w) throw std::runtime_error("debug_conv_tc: w is required");
-    if (!x) throw std::runtime_error("debug_conv_tc: x is required");
-    std::vector<int> lens(batch, L);
-    for (int i = 0; i < batch && item_len; ++i) {
-        if (item_len[i] < 0 || item_len[i] > L) throw std::runtime_error("debug_conv_tc: item_len must lie in [0, L]");
-        lens[i] = item_len[i];
-    }
-    if (Cin < 1 || Cout < 1) throw std::runtime_error("debug_conv_tc: empty channel count");
-    const ConvTcPlan pl = up ? conv1d_tc_plan(Cin, up * Cout, 2) : conv1d_tc_plan(Cin, Cout, K);
-    if (!pl.ok) throw std::runtime_error("debug_conv_tc: no tensor-core plan for these channel counts");
-    if (up > 0 && Cout % 32 != 0) throw std::runtime_error("debug_conv_tc: ConvTranspose1d needs Cout % 32 == 0");
-    if (out16 && Cout % 8 != 0) throw std::runtime_error("debug_conv_tc: out16 needs Cout % 8 == 0");
-    if (cbias && cbias_stride < Cout) throw std::runtime_error("debug_conv_tc: cbias_stride < Cout");
-    if (max_ctas < 0) throw std::runtime_error("debug_conv_tc: max_ctas must be >= 0");
-    CUDA_CHECK(cudaSetDevice(cfg.device));
-    const int Lout = up ? L * up : L, lpad = atoms_lpad(L), lpad_out = atoms_lpad(Lout);
-    std::vector<__half> blob(pl.blob_halves);
-    if (up) convT_tc_pack(w, Cin, Cout, up, pl, blob.data());
-    else conv1d_tc_pack(w, Cin, Cout, K, pl, blob.data());
-    __half_raw nan_raw; nan_raw.x = 0x7e00;
-    const size_t n_in = (size_t)batch * Cin * lpad, n32 = (size_t)batch * Cout * Lout, n16 = (size_t)batch * Cout * lpad_out;
-    std::vector<__half> a(n_in, __half(nan_raw));
-    for (int b = 0; b < batch; ++b)
-        for (int c = 0; c < Cin; ++c)
-            for (int t = 0; t < lens[b]; ++t)
-                a[(((size_t)b * (Cin / 8) + c / 8) * lpad + kAtomPadL + t) * 8 + c % 8] = __float2half_rn(x[((size_t)b * Cin + c) * L + t]);
-    DBuf<__half> da, dblob, do16;
-    DBuf<float> dbias, dcb, dres, do32;
-    da.alloc(n_in); dblob.alloc(blob.size());
-    da.upload(a.data(), n_in, st); dblob.upload(blob.data(), blob.size(), st);
-    if (bias) { dbias.alloc(Cout); dbias.upload(bias, Cout, st); }
-    if (cbias) { dcb.alloc((size_t)batch * cbias_stride); dcb.upload(cbias, (size_t)batch * cbias_stride, st); }
-    if (resid) { dres.alloc(n32); dres.upload(resid, n32, st); }
-    if (out32) { do32.alloc(n32); do32.upload(out32, n32, st); }
-    std::vector<__half> o16(out16 ? n16 : 0);
-    if (out16) {
-        for (size_t i = 0; i < n16; ++i) o16[i] = __float2half_rn(out16[i]);
-        do16.alloc(n16); do16.upload(o16.data(), n16, st);
-    }
-    launch_atoms_zero_pads(da.p, batch * Cin / 8, lpad, L, st, batch, lens.data());
-    const int* il = item_len ? lens.data() : nullptr;
-    struct CapRestore { int& cap; int prev; ~CapRestore() { cap = prev; } } restore{g_voc_sm_cap, g_voc_sm_cap};
-    g_voc_sm_cap = max_ctas;
-    if (up)
-        launch_convT_tc(da.p, dblob.p, pl, dbias.p, dcb.p, do32.p, do16.p, Cin, Cout, L, lpad, lpad_out, up, slope_out, batch,
-                        cbias_stride, st, il);
-    else
-        launch_conv1d_tc(da.p, dblob.p, pl, dbias.p, dcb.p, dres.p, do32.p, do16.p, Cin, Cout, L, lpad, K, dil, slope_out,
-                         scale16, mode, batch, cbias_stride, st, il);
-    if (out32) do32.download(out32, n32, st);
-    std::vector<uint16_t> r16(out16 ? n16 : 0);
-    if (out16) do16.download(reinterpret_cast<__half*>(r16.data()), n16, st);
-    CUDA_CHECK(cudaStreamSynchronize(st));
-    if (out16) widen16(r16, true, out16);
-}
-
-// One conditioning kernel or front-end (cond_debug in cond.cu) on the engine's stream
-void Engine::debug_cond(int op, const int32_t* dims, int n_dims, const float* scal, int n_scal, const float* const* in,
-                        const int64_t* in_len, int n_in, float* out, int64_t out_len) {
-    ApiLock lk(this);
-    if (!running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty()) throw std::runtime_error("debug entry points need an idle engine");
-    CUDA_CHECK(cudaSetDevice(cfg.device));
-    cond_debug(conditioner.get(), op, dims, n_dims, scal, n_scal, in, in_len, n_in, out, out_len, st);
+    f(HarnessCtx{st, cfg.ln_eps, use_pdl, conditioner.get()});
 }
 
 }  // namespace xtts
@@ -3034,6 +2325,7 @@ void Engine::debug_cond(int op, const int32_t* dims, int n_dims, const float* sc
 // C ABI
 // ================================================================================================
 using xtts::Engine;
+using xtts::HarnessCtx;
 struct xtts_engine { Engine* impl; };
 
 #define XTTS_TRY(body)                                                  \
@@ -3125,8 +2417,10 @@ int xtts_debug_beam_step(xtts_engine* e, int32_t kv_type, int32_t heads, int32_t
                          void* vpool, float* scores) {
     if (!sp || !beam || !logits || !n_gen || !ctx_len || !last_tok || !seen || !block_tables || !pool || !hist || !state ||
         !kpool || !vpool || !scores) { xtts::set_error("null argument"); return XTTS_ERR_INVALID; }
-    XTTS_TRY(e->impl->debug_beam_step(kv_type, heads, layers, V, *sp, *beam, first, advance, logits, n_gen, ctx_len, last_tok,
-                                      seen, max_pages, block_tables, n_pages, pool, cap, hist, state, kpool, vpool, scores))
+    XTTS_TRY(e->impl->run_idle([&](const HarnessCtx& c) {
+        xtts::debug_beam_step(c, kv_type, heads, layers, V, *sp, *beam, first, advance, logits, n_gen, ctx_len, last_tok, seen,
+                              max_pages, block_tables, n_pages, pool, cap, hist, state, kpool, vpool, scores);
+    }))
 }
 int xtts_cancel(xtts_engine* e, uint64_t seq_id) { XTTS_TRY(e->impl->cancel(seq_id)) }
 int xtts_poll(xtts_engine* e, xtts_result* out, int32_t timeout_ms) {
@@ -3167,71 +2461,95 @@ int xtts_gpt_teacher_forced(xtts_engine* e, const int32_t* text_ids, int32_t n_t
 }
 int xtts_debug_gemm(xtts_engine* e, int32_t mode, const float* A, const float* W, const float* bias, const float* resid,
                     float* out, int32_t M, int32_t N, int32_t K, int32_t flags, int32_t iters, float* ms_per_iter) {
-    XTTS_TRY(e->impl->debug_gemm(mode, A, W, bias, resid, out, M, N, K, flags, iters, ms_per_iter))
+    XTTS_TRY(e->impl->run_idle([&](const HarnessCtx& c) {
+        xtts::debug_gemm(c, mode, A, W, bias, resid, out, M, N, K, flags, iters, ms_per_iter);
+    }))
 }
 int xtts_debug_ln_gemm(xtts_engine* e, int32_t mode, int32_t launch, int32_t M, int32_t N, int32_t K, const float* X,
                        const float* ln_w, const float* ln_b, const float* W, const float* bias, const float* resid, int32_t flags,
                        float* Y, float* out) {
-    XTTS_TRY(e->impl->debug_ln_gemm(mode, launch, M, N, K, X, ln_w, ln_b, W, bias, resid, flags, Y, out))
+    XTTS_TRY(e->impl->run_idle([&](const HarnessCtx& c) {
+        xtts::debug_ln_gemm(c, mode, launch, M, N, K, X, ln_w, ln_b, W, bias, resid, flags, Y, out);
+    }))
 }
 int xtts_debug_norms(xtts_engine* e, int32_t out_type, int32_t M, int32_t H, const float* X, int32_t x_rows,
                      const int32_t* row_index, const float* w1, const float* b1, const float* w2, const float* b2, float* Y,
                      float* latents, int32_t n_slots, int32_t lat_rows, const int32_t* slots, const int32_t* lat_pos,
                      const int32_t* n_gen) {
-    XTTS_TRY(e->impl->debug_norms(out_type, M, H, X, x_rows, row_index, w1, b1, w2, b2, Y, latents, n_slots, lat_rows, slots,
-                                  lat_pos, n_gen))
+    XTTS_TRY(e->impl->run_idle([&](const HarnessCtx& c) {
+        xtts::debug_norms(c, out_type, M, H, X, x_rows, row_index, w1, b1, w2, b2, Y, latents, n_slots, lat_rows, slots,
+                          lat_pos, n_gen);
+    }))
 }
 int xtts_debug_kv_write(xtts_engine* e, int32_t kv_type, int32_t heads, int32_t M, const float* qkv, const int32_t* row_slot,
                         const int32_t* row_pos, int32_t n_slots, const int32_t* ctx_len, const int32_t* block_tables,
                         int32_t max_pages, int32_t n_pages, void* kpool, void* vpool) {
-    XTTS_TRY(e->impl->debug_kv_write(kv_type, heads, M, qkv, row_slot, row_pos, n_slots, ctx_len, block_tables, max_pages, n_pages,
-                                     kpool, vpool))
+    XTTS_TRY(e->impl->run_idle([&](const HarnessCtx& c) {
+        xtts::debug_kv_write(c, kv_type, heads, M, qkv, row_slot, row_pos, n_slots, ctx_len, block_tables, max_pages, n_pages,
+                             kpool, vpool);
+    }))
 }
 int xtts_debug_build_rows(xtts_engine* e, int32_t H, int32_t n_cond, const float* text_emb, int32_t n_text, const float* text_pos,
                           int32_t n_text_pos, const float* wte, int32_t n_audio, const float* wpe, int32_t n_wpe,
                           const float* spk_cond, int32_t n_spk, const int32_t* rows, int32_t n_rows, float* X) {
-    XTTS_TRY(e->impl->debug_build_rows(H, n_cond, text_emb, n_text, text_pos, n_text_pos, wte, n_audio, wpe, n_wpe, spk_cond, n_spk,
-                                       rows, n_rows, X))
+    XTTS_TRY(e->impl->run_idle([&](const HarnessCtx& c) {
+        xtts::debug_build_rows(c, H, n_cond, text_emb, n_text, text_pos, n_text_pos, wte, n_audio, wpe, n_wpe, spk_cond, n_spk,
+                               rows, n_rows, X);
+    }))
 }
 int xtts_debug_build_decode_rows(xtts_engine* e, int32_t H, const float* wte, int32_t n_audio, const float* wpe, int32_t n_wpe,
                                  int32_t M, const int32_t* active, int32_t n_slots, const int32_t* last_tok, const int32_t* n_gen,
                                  float* X) {
-    XTTS_TRY(e->impl->debug_build_decode_rows(H, wte, n_audio, wpe, n_wpe, M, active, n_slots, last_tok, n_gen, X))
+    XTTS_TRY(e->impl->run_idle([&](const HarnessCtx& c) {
+        xtts::debug_build_decode_rows(c, H, wte, n_audio, wpe, n_wpe, M, active, n_slots, last_tok, n_gen, X);
+    }))
 }
 int xtts_debug_sample_slots(xtts_engine* e, int32_t V, int32_t M, const int32_t* active, int32_t n_slots, const float* logits,
                             int32_t ld, const xtts_sampling* sp, int32_t cap, int32_t advance_ctx, const int32_t* forced,
                             int32_t* n_gen, int32_t* ctx_len, int32_t* finished, int32_t* last_tok, uint8_t* seen,
                             int32_t* tokens, int32_t* sampled) {
-    XTTS_TRY(e->impl->debug_sample_slots(V, M, active, n_slots, logits, ld, sp, cap, advance_ctx, forced, n_gen, ctx_len,
-                                         finished, last_tok, seen, tokens, sampled))
+    XTTS_TRY(e->impl->run_idle([&](const HarnessCtx& c) {
+        xtts::debug_sample_slots(c, V, M, active, n_slots, logits, ld, sp, cap, advance_ctx, forced, n_gen, ctx_len, finished,
+                                 last_tok, seen, tokens, sampled);
+    }))
 }
 int xtts_debug_attn_decode(xtts_engine* e, int32_t kv_type, int32_t heads, int32_t M, const int32_t* active, int32_t n_slots,
                            const int32_t* ctx_len, const int32_t* block_tables, int32_t max_pages, int32_t n_pages,
                            void* kpool, void* vpool, const float* qkv, float* out) {
-    XTTS_TRY(e->impl->debug_attn_decode(kv_type, heads, M, active, n_slots, ctx_len, block_tables, max_pages, n_pages, kpool, vpool,
-                                        qkv, out))
+    XTTS_TRY(e->impl->run_idle([&](const HarnessCtx& c) {
+        xtts::debug_attn_decode(c, kv_type, heads, M, active, n_slots, ctx_len, block_tables, max_pages, n_pages, kpool, vpool,
+                                qkv, out);
+    }))
 }
 int xtts_debug_attn_prefill(xtts_engine* e, int32_t out_type, int32_t heads, const int32_t* seqs, int32_t nseq, int32_t causal,
                             float scale, const float* q, int64_t q_len, int32_t q_row_stride, int32_t q_head_stride,
                             const float* kv, int64_t kv_len, int32_t kv_row_stride, int32_t kv_head_stride, int64_t k_off,
                             int64_t v_off, float* out, int32_t out_rows) {
-    XTTS_TRY(e->impl->debug_attn_prefill(out_type, heads, seqs, nseq, causal, scale, q, q_len, q_row_stride, q_head_stride, kv,
-                                         kv_len, kv_row_stride, kv_head_stride, k_off, v_off, out, out_rows))
+    XTTS_TRY(e->impl->run_idle([&](const HarnessCtx& c) {
+        xtts::debug_attn_prefill(c, out_type, heads, seqs, nseq, causal, scale, q, q_len, q_row_stride, q_head_stride, kv,
+                                 kv_len, kv_row_stride, kv_head_stride, k_off, v_off, out, out_rows);
+    }))
 }
 int xtts_debug_splitk_ln(xtts_engine* e, int32_t mode, int32_t M, int32_t N, int32_t K, int32_t splits, const float* A,
                          const float* W, const float* bias, float* X, const float* ln_w, const float* ln_b, float* Y) {
-    XTTS_TRY(e->impl->debug_splitk_ln(mode, M, N, K, splits, A, W, bias, X, ln_w, ln_b, Y))
+    XTTS_TRY(e->impl->run_idle([&](const HarnessCtx& c) {
+        xtts::debug_splitk_ln(c, mode, M, N, K, splits, A, W, bias, X, ln_w, ln_b, Y);
+    }))
 }
 int xtts_debug_conv_tc(xtts_engine* e, int32_t up, int32_t Cin, int32_t Cout, int32_t K, int32_t dil, int32_t batch, int32_t L,
                        const int32_t* item_len, const float* w, const float* bias, const float* cbias, int32_t cbias_stride,
                        const float* x, const float* resid, int32_t mode, float slope_out, float scale16, int32_t max_ctas,
                        float* out32, float* out16) {
-    XTTS_TRY(e->impl->debug_conv_tc(up, Cin, Cout, K, dil, batch, L, item_len, w, bias, cbias, cbias_stride, x, resid, mode,
-                                    slope_out, scale16, max_ctas, out32, out16))
+    XTTS_TRY(e->impl->run_idle([&](const HarnessCtx& c) {
+        xtts::debug_conv_tc(c, up, Cin, Cout, K, dil, batch, L, item_len, w, bias, cbias, cbias_stride, x, resid, mode,
+                            slope_out, scale16, max_ctas, out32, out16);
+    }))
 }
 int xtts_debug_cond(xtts_engine* e, int32_t op, const int32_t* dims, int32_t n_dims, const float* scal, int32_t n_scal,
                     const float* const* in, const int64_t* in_len, int32_t n_in, float* out, int64_t out_len) {
-    XTTS_TRY(e->impl->debug_cond(op, dims, n_dims, scal, n_scal, in, in_len, n_in, out, out_len))
+    XTTS_TRY(e->impl->run_idle([&](const HarnessCtx& c) {
+        xtts::cond_debug(c.cnd, op, dims, n_dims, scal, n_scal, in, in_len, n_in, out, out_len, c.st);
+    }))
 }
 
 }  // extern "C"

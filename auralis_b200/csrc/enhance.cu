@@ -363,12 +363,12 @@ void stft_tables(std::vector<float>& hann, std::vector<float>& win2, std::vector
 
 struct Enhancer::Impl {
     cudaStream_t st;
-    Dev<float> hann, win2, basis, ibasis, gain, x, y, F, D, P, mel, magT, noise, energy, lsum;
-    std::map<int, Dev<float>> fb;                    // mel filterbank per sample rate
-    Dev<unsigned> ordmax;
-    Dev<double> kp, endst, init, csum, ctot, z, lres;
-    Dev<int64_t> blo, bhi;
-    Dev<int> bad;
+    DBuf<float> hann, win2, basis, ibasis, gain, x, y, F, D, P, mel, magT, noise, energy, lsum;
+    std::map<int, DBuf<float>> fb;                   // mel filterbank per sample rate
+    DBuf<unsigned> ordmax;
+    DBuf<double> kp, endst, init, csum, ctot, z, lres;
+    DBuf<int64_t> blo, bhi;
+    DBuf<int> bad;
 
     void lazy_init() {
         if (basis.p) return;

@@ -492,10 +492,10 @@ constexpr int64_t kMaxSamples = ((int64_t)1 << 36) - 1;   // STREAMINFO's 36-bit
 
 struct FlacEncoder::Impl {
     cudaStream_t st;
-    Dev<int16_t> pcm;
-    Dev<FrameDesc> desc;
-    Dev<int64_t> off, stats;
-    Dev<uint8_t> bytes;
+    DBuf<int16_t> pcm;
+    DBuf<FrameDesc> desc;
+    DBuf<int64_t> off, stats;
+    DBuf<uint8_t> bytes;
     bool attr_set = false;
 };
 
@@ -958,15 +958,15 @@ uint64_t be(const uint8_t* p, int n) {
 
 struct FlacDecoder::Impl {
     cudaStream_t st;
-    Dev<uint32_t> words;
-    Dev<uint16_t> mask;
-    Dev<int64_t> counts, total;
-    Dev<Cand> cands;
-    Dev<DFrame> frames;
-    Dev<DSub> subs;
-    Dev<DRes> res;
-    Dev<int32_t> w32;
-    Dev<int64_t> w64;
+    DBuf<uint32_t> words;
+    DBuf<uint16_t> mask;
+    DBuf<int64_t> counts, total;
+    DBuf<Cand> cands;
+    DBuf<DFrame> frames;
+    DBuf<DSub> subs;
+    DBuf<DRes> res;
+    DBuf<int32_t> w32;
+    DBuf<int64_t> w64;
 };
 
 FlacDecoder::FlacDecoder(cudaStream_t st) : impl(new Impl()) { impl->st = st; }

@@ -128,10 +128,10 @@ int64_t out_frames(int64_t n, double rate) {
 
 struct PhaseVocoder::Impl {
     cudaStream_t st;
-    Dev<float> hann, win2, basis, ibasis, x, y, F, D, mag, ang, phase, Y, acc;
-    Dev<double> phi, dph;
-    Dev<unsigned> peak;
-    Dev<int> bad;
+    DBuf<float> hann, win2, basis, ibasis, x, y, F, D, mag, ang, phase, Y, acc;
+    DBuf<double> phi, dph;
+    DBuf<unsigned> peak;
+    DBuf<int> bad;
 
     void lazy_init() {
         if (basis.p) return;

@@ -154,8 +154,8 @@ Geo geometry(int orig, int new_sr) {
 struct Resampler::Impl {
     cudaStream_t st;
     int L = 0, M = 0;                        // the geometry `tab` / `kstart` hold
-    Dev<float> tab, x, y;
-    Dev<int> kstart, bad;
+    DBuf<float> tab, x, y;
+    DBuf<int> kstart, bad;
 };
 
 Resampler::Resampler(cudaStream_t st) : impl(new Impl()) {
