@@ -72,7 +72,7 @@ inline KernelCtx& kctx() { return t_kctx ? *t_kctx : kctx_default(); }
 // Off by default; when on, every launcher records an event pair and its algorithmic FLOPs / bytes.
 enum KernelFamily : int {
     KF_GEMM_TC = 0, KF_GEMM_F32, KF_ATTN_DECODE, KF_ATTN_PREFILL, KF_NORM, KF_SAMPLE, KF_KV_WRITE, KF_EMBED,
-    KF_CONV1D, KF_CONVT, KF_CONV_POST, KF_INTERP, KF_COND, KF_MISC, KF_CONV1D_TC, KF_COUNT
+    KF_CONV1D, KF_CONVT, KF_CONV_POST, KF_INTERP, KF_COND, KF_MISC, KF_CONV1D_TC, KF_RESBLOCK_TC, KF_COUNT
 };
 struct KernelProfiler {
     bool enabled = false;
@@ -185,7 +185,8 @@ struct ProfScope {
 inline const char* kernel_family_name(int f) {
     static const char* n[KF_COUNT] = {"gemm_bf16_wgmma", "gemm_f32", "attn_decode_paged", "attn_prefill", "layernorm",
                                       "sample", "kv_write", "embed", "conv1d", "conv_transpose1d", "conv_post_tanh",
-                                      "interp", "conditioning", "misc", "conv1d_tc_f16_wgmma"};
+                                      "interp", "conditioning", "misc", "conv1d_tc_f16_wgmma",
+                                      "resblock_tc_f16_wgmma"};
     return (f >= 0 && f < KF_COUNT) ? n[f] : "?";
 }
 

@@ -418,7 +418,6 @@ void conv1d_tc_pack(const float* w, int Cin, int Cout, int K, const ConvTcPlan& 
 
 int atoms_lpad(int L) { return kAtomPadL + ceil_div(L + 1, 512) * 512 + kAtomPadR; }
 
-constexpr int kMaxDynTc = 227 * 1024 - 4096;      // opt-in limit minus the kernel's static shared memory
 template <int N, int MB, bool STAGED>
 static void launch_inst(const ConvTcParams& P, dim3 grid, size_t smem, cudaStream_t st) {
     static bool attr[64] = {};

@@ -311,6 +311,7 @@ private:
     std::map<int, cudaGraphExec_t> decode_graphs;
     std::map<int, unsigned long long> graph_kernels;
     bool use_tc_vocoder = true;   // fast mode only; option "tc_vocoder" switches back to the fp32 CUDA-core convs
+    bool use_resblock_tc = true;  // test / A-B switch "tc_resblock": 0 runs every resblock as its six conv1d_tc launches (same bits)
     std::vector<std::pair<float*, size_t>> pinned_pool;
     // stats
     double decode_ctx_sum = 0;
@@ -1514,6 +1515,19 @@ void Engine::run_vocoder_tc(const VocItem* it, int nb, int Lz, float* wav_dev_ou
         if (more) launch_atoms_zero_pads(PA, nb * C / 8, lpad, len, sv, nb, lens);     // PA is re-shaped for the next stage's input
         for (int j = 0; j < nk; ++j) {
             const RB& rb = *rbs[i * nk + j];
+            const bool emit = more && (j == nk - 1);
+            const int mode = j == 0 ? CONV_STORE : CONV_ACCUM;
+            if (use_resblock_tc && resblock_tc_tile_rows(C, rb.c1[0]->K, c.voc_rb_dilations, len) > 0) {
+                // the whole resblock on chip: same bits as the six launches below
+                const __half* wb[6]; const float* bs[6];
+                for (int t = 0; t < 3; ++t) {
+                    wb[2 * t] = rb.c1[t]->blob.p; wb[2 * t + 1] = rb.c2[t]->blob.p;
+                    bs[2 * t] = rb.c1[t]->b.p; bs[2 * t + 1] = rb.c2[t]->b.p;
+                }
+                launch_resblock_tc(XA, X, wb, bs, ZS, emit ? PA : nullptr, C, len, lpad, rb.c1[0]->K, c.voc_rb_dilations, mode,
+                                   1.0f / (float)nk, nb, lens, sv);
+                continue;
+            }
             const __half* in16 = XA;
             const float* resid = X;
             for (int t = 0; t < 3; ++t) {
@@ -1523,9 +1537,7 @@ void Engine::run_vocoder_tc(const VocItem* it, int nb, int Lz, float* wav_dev_ou
                     in16 = RA[t]; resid = R[t];
                 } else {
                     // MRF sum; the last resblock also emits lrelu(sum / nk) as the next transposed conv's operand
-                    const bool emit = more && (j == nk - 1);
-                    conv_tc(*rb.c2[t], TA, nullptr, resid, ZS, emit ? PA : nullptr, len, lpad, 1,
-                            j == 0 ? CONV_STORE : CONV_ACCUM, 1.0f / (float)nk);
+                    conv_tc(*rb.c2[t], TA, nullptr, resid, ZS, emit ? PA : nullptr, len, lpad, 1, mode, 1.0f / (float)nk);
                 }
             }
         }
@@ -2060,6 +2072,7 @@ void Engine::set_option(const std::string& k, int64_t v) {
     else if (k == "voc_segment") voc_segment = (int)std::max<int64_t>(0, v);
     else if (k == "voc_sms") voc_sms = (int)std::max<int64_t>(0, v);
     else if (k == "tc_epilogue") g_conv_tc_epilogue = v ? 1 : 0;
+    else if (k == "tc_resblock") use_resblock_tc = v != 0;
     else if (k == "pvoc_block_frames") {
         if (v < 1 || v > (1 << 20)) throw std::runtime_error("pvoc_block_frames: 1 .. 2^20 output frames");
         pvoc_block_frames = (int)v;
@@ -2543,6 +2556,13 @@ int xtts_debug_conv_tc(xtts_engine* e, int32_t up, int32_t Cin, int32_t Cout, in
     XTTS_TRY(e->impl->run_idle([&](const HarnessCtx& c) {
         xtts::debug_conv_tc(c, up, Cin, Cout, K, dil, batch, L, item_len, w, bias, cbias, cbias_stride, x, resid, mode,
                             slope_out, scale16, max_ctas, out32, out16);
+    }))
+}
+int xtts_debug_resblock_tc(xtts_engine* e, int32_t C, int32_t K, const int32_t* dil, int32_t batch, int32_t L,
+                           const int32_t* item_len, const float* w, const float* bias, const float* x, int32_t mode,
+                           float scale16, int32_t max_ctas, int32_t fused, float* zs, float* pa) {
+    XTTS_TRY(e->impl->run_idle([&](const HarnessCtx& c) {
+        xtts::debug_resblock_tc(c, C, K, dil, batch, L, item_len, w, bias, x, mode, scale16, max_ctas, fused, zs, pa);
     }))
 }
 int xtts_debug_cond(xtts_engine* e, int32_t op, const int32_t* dims, int32_t n_dims, const float* scal, int32_t n_scal,

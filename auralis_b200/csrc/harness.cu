@@ -5,6 +5,7 @@
 
 #include <algorithm>
 #include <cstring>
+#include <limits>
 #include <type_traits>
 #include <vector>
 
@@ -568,6 +569,87 @@ void debug_conv_tc(const HarnessCtx& c, int up, int Cin, int Cout, int K, int di
                          scale16, mode, batch, cbias_stride, st, il);
     if (out32) do32.download(out32, n32, st);
     if (out16) download_f32(do16.p, 2, out16, n16, st);
+    CUDA_CHECK(cudaStreamSynchronize(st));
+}
+
+// One vocoder ResBlock1 of C channels on host data, through the fused kernel (launch_resblock_tc) or through the six
+// launch_conv1d_tc calls it replaces, issued as Engine::run_vocoder_tc issues them.  Weights w [6][C][C][K] and biases
+// [6][C] in the order c1_0, c2_0, c1_1, c2_1, c1_2, c2_2.  The input atoms are lrelu(x, 0.1) as fp16, NaN outside each
+// item's signal until the production pad routine clears its pads (the six-launch workspaces too), and the fp32 rows past
+// an item's length are NaN: a read of anything else reaches a stored output as NaN.  zs / pa are in/out as in
+// debug_conv_tc.
+void debug_resblock_tc(const HarnessCtx& c, int C, int K, const int32_t* dil, int batch, int L, const int32_t* item_len,
+                       const float* w, const float* bias, const float* x, int mode, float scale16, int max_ctas, int fused,
+                       float* zs, float* pa) {
+    if (!dil || !w || !bias || !x || !zs) throw std::runtime_error("debug_resblock_tc: dil, w, bias, x and zs are required");
+    if (fused && resblock_tc_tile_rows(C, K, dil, L) == 0)
+        throw std::runtime_error("debug_resblock_tc: fused needs C 32 or 64, K odd, dilations >= 1 and a halo that is a multiple of 4 and fits the tile");
+    if (!fused && (C % 8 != 0 || K % 2 == 0 || dil[0] < 1 || dil[1] < 1 || dil[2] < 1 || !conv1d_tc_plan(C, C, K).ok))
+        throw std::runtime_error("debug_resblock_tc: no tensor-core plan for these channel counts, an even K or a dilation < 1");
+    if (mode != CONV_STORE && mode != CONV_ACCUM) throw std::runtime_error("debug_resblock_tc: mode 0 (store) or 1 (accumulate)");
+    if (batch < 1 || batch > kVocMaxItems) throw std::runtime_error("debug_resblock_tc: batch must be 1..32");
+    if (L < 4 || L % 4 != 0) throw std::runtime_error("debug_resblock_tc: L must be a positive multiple of 4");
+    if (max_ctas < 0) throw std::runtime_error("debug_resblock_tc: max_ctas must be >= 0");
+    for (int t = 0; t < 3; ++t)
+        if ((K - 1) / 2 * dil[t] > kAtomPadL) throw std::runtime_error("debug_resblock_tc: halo (K-1)/2*dil exceeds the atom head pad");
+    std::vector<int> lens(batch, L);
+    for (int i = 0; i < batch && item_len; ++i) {
+        if (item_len[i] < 0 || item_len[i] > L) throw std::runtime_error("debug_resblock_tc: item_len must lie in [0, L]");
+        lens[i] = item_len[i];
+    }
+    const cudaStream_t st = c.st;
+    const int lpad = atoms_lpad(L), PL = C / 8;
+    const ConvTcPlan pl = conv1d_tc_plan(C, C, K);
+    std::vector<__half> blob(6 * pl.blob_halves);
+    for (int i = 0; i < 6; ++i) conv1d_tc_pack(w + (size_t)i * C * C * K, C, C, K, pl, blob.data() + i * pl.blob_halves);
+    __half_raw nan_raw; nan_raw.x = 0x7e00;
+    const size_t n32 = (size_t)batch * C * L, n16 = (size_t)batch * C * lpad;
+    std::vector<__half> a(n16, __half(nan_raw));
+    std::vector<float> x32(n32, std::numeric_limits<float>::quiet_NaN());
+    for (int b = 0; b < batch; ++b)
+        for (int ch = 0; ch < C; ++ch)
+            for (int t = 0; t < lens[b]; ++t) {
+                const float v = x[((size_t)b * C + ch) * L + t];
+                x32[((size_t)b * C + ch) * L + t] = v;
+                a[(((size_t)b * PL + ch / 8) * lpad + kAtomPadL + t) * 8 + ch % 8] = __float2half_rn(v > 0.f ? v : v * 0.1f);
+            }
+    std::vector<__half> o16(pa ? n16 : 0);
+    for (size_t i = 0; i < o16.size(); ++i) o16[i] = __float2half_rn(pa[i]);
+    DBuf<__half> dxa = to_dev(a.data(), n16, st), dblob = to_dev(blob.data(), blob.size(), st),
+                 dpa = to_dev(pa ? o16.data() : nullptr, n16, st);
+    DBuf<float> dx = to_dev(x32.data(), n32, st), dzs = to_dev(zs, n32, st), dbias = to_dev(bias, (size_t)6 * C, st);
+    const int* il = item_len ? lens.data() : nullptr;
+    launch_atoms_zero_pads(dxa.p, batch * PL, lpad, L, st, batch, lens.data());
+    struct CapRestore { int& cap; int prev; ~CapRestore() { cap = prev; } } restore{g_voc_sm_cap, g_voc_sm_cap};
+    g_voc_sm_cap = max_ctas;
+    const __half* wb[6]; const float* bs[6];
+    for (int i = 0; i < 6; ++i) { wb[i] = dblob.p + i * pl.blob_halves; bs[i] = dbias.p + (size_t)i * C; }
+    if (fused) {
+        launch_resblock_tc(dxa.p, dx.p, wb, bs, dzs.p, dpa.p, C, L, lpad, K, dil, mode, scale16, batch, il, st);
+    } else {
+        DBuf<__half> ta = to_dev(a.data(), n16, st), ra0 = to_dev(a.data(), n16, st), ra1 = to_dev(a.data(), n16, st);
+        DBuf<float> r[2];
+        for (auto& rr : r) rr = to_dev(x32.data(), n32, st);
+        for (__half* b : {ta.p, ra0.p, ra1.p}) launch_atoms_zero_pads(b, batch * PL, lpad, L, st, batch, lens.data());
+        const __half* in16 = dxa.p;
+        const float* resid = dx.p;
+        __half* ra[2] = {ra0.p, ra1.p};
+        for (int t = 0; t < 3; ++t) {
+            launch_conv1d_tc(in16, wb[2 * t], pl, bs[2 * t], nullptr, nullptr, nullptr, ta.p, C, C, L, lpad, K, dil[t], 0.1f,
+                             1.0f, CONV_STORE, batch, 0, st, il);
+            if (t < 2) {
+                launch_conv1d_tc(ta.p, wb[2 * t + 1], pl, bs[2 * t + 1], nullptr, resid, r[t].p, ra[t], C, C, L, lpad, K, 1, 0.1f,
+                                 1.0f, CONV_STORE, batch, 0, st, il);
+                in16 = ra[t]; resid = r[t].p;
+            } else {
+                launch_conv1d_tc(ta.p, wb[2 * t + 1], pl, bs[2 * t + 1], nullptr, resid, dzs.p, dpa.p, C, C, L, lpad, K, 1, 0.1f,
+                                 scale16, mode, batch, 0, st, il);
+            }
+        }
+        CUDA_CHECK(cudaStreamSynchronize(st));
+    }
+    dzs.download(zs, n32, st);
+    if (pa) download_f32(dpa.p, 2, pa, n16, st);
     CUDA_CHECK(cudaStreamSynchronize(st));
 }
 

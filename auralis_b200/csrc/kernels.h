@@ -201,6 +201,8 @@ void launch_conv1d(const float* x, const float* w_t, const float* bias, const fl
 //   [C/8 plane][kAtomPadL + L + tail][8 channels], zero pads — the wgmma no-swizzle K-major operand image.
 constexpr int kAtomPadL = 64, kAtomPadR = 64;
 int atoms_lpad(int L);                                   // padded rows per plane for a signal of L steps
+// dynamic shared memory a tensor-core conv kernel may take: the opt-in limit minus the kernels' static shared memory
+constexpr int kMaxDynTc = 227 * 1024 - 4096;
 struct ConvTcPlan { int N, CK, n_tiles, nacc; bool ok; size_t tile_halves, blob_halves; };
 ConvTcPlan conv1d_tc_plan(int Cin, int Cout, int K);
 void conv1d_tc_pack(const float* w /*[Cout][Cin][K]*/, int Cin, int Cout, int K, const ConvTcPlan& pl, __half* blob);
@@ -216,6 +218,15 @@ void launch_conv1d_tc(const __half* a16, const __half* wblob, const ConvTcPlan& 
                       const float* resid, float* out32, __half* out16, int Cin, int Cout, int L, int lpad, int K, int dil,
                       float slope_out, float scale16, int mode, int batch, int cbias_batch_stride, cudaStream_t st,
                       const int* item_len = nullptr);
+// One whole ResBlock1 (for t = 0..2: x += c2_t(lrelu(c1_t(lrelu(x), dil[t])), 1); then zs (=|+=) x) as one launch, bit-identical
+// to its six launch_conv1d_tc calls.  xa: lrelu(x) atoms, x: fp32 [batch][C][L] (L % 4 == 0); wblob / bias: the six convs
+// c1_0, c2_0, c1_1, c2_1, c1_2, c2_2 (conv1d_tc_pack blobs); pa (optional): lrelu(sum * scale16, 0.1) atoms.
+// resblock_tc_tile_rows: output rows per CTA tile, 0 when the fused kernel does not take this geometry (C must be 32 or 64,
+// the chain's halo (K-1)/2 * (dil[0] + dil[1] + dil[2] + 3) and the row stride L multiples of 4).
+int resblock_tc_tile_rows(int C, int K, const int* dil, int L);
+void launch_resblock_tc(const __half* xa, const float* x, const __half* const* wblob, const float* const* bias, float* zs,
+                        __half* pa, int C, int L, int lpad, int K, const int* dil, int mode, float scale16, int batch,
+                        const int* item_len, cudaStream_t st);
 // ConvTranspose1d(kernel 2u, stride u, padding u/2) on the same kernel (u phases x 2 taps); plan = conv1d_tc_plan(Cin, u*Cr, 2)
 void convT_tc_pack(const float* w /*[Cin][Cr][2u]*/, int Cin, int Cr, int u, const ConvTcPlan& pl, __half* blob);
 void launch_convT_tc(const __half* a16, const __half* wblob, const ConvTcPlan& pl, const float* bias, const float* cbias,

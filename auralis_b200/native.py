@@ -126,7 +126,7 @@ ABI_SYMBOLS = [
     "xtts_fetch", "xtts_set_option", "xtts_get_stats", "xtts_sync", "xtts_get_kernel_profile", "xtts_device_timer", "xtts_vocode",
     "xtts_vocode_window", "xtts_vocode_speed", "xtts_gpt_prefill", "xtts_gpt_teacher_forced",
     "xtts_debug_gemm", "xtts_debug_sample_slots", "xtts_debug_trace",
-    "xtts_debug_attn_decode", "xtts_debug_attn_prefill", "xtts_debug_splitk_ln", "xtts_debug_conv_tc",
+    "xtts_debug_attn_decode", "xtts_debug_attn_prefill", "xtts_debug_splitk_ln", "xtts_debug_conv_tc", "xtts_debug_resblock_tc",
     "xtts_debug_ln_gemm", "xtts_debug_norms", "xtts_debug_kv_write", "xtts_debug_build_rows", "xtts_debug_build_decode_rows",
     "xtts_debug_cond",
 ]
@@ -191,6 +191,8 @@ def load_library(path: Optional[str] = None):
     lib.xtts_debug_attn_prefill.argtypes = [vp, i32, i32, i32p, i32, i32, C.c_float, f32p, i64, i32, i32, f32p, i64, i32, i32,
                                             i64, i64, f32p, i32]
     lib.xtts_debug_splitk_ln.argtypes = [vp, i32, i32, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, f32p, f32p]
+    lib.xtts_debug_resblock_tc.argtypes = [vp, i32, i32, i32p, i32, i32, i32p, f32p, f32p, f32p, i32, C.c_float, i32, i32, f32p,
+                                           f32p]
     lib.xtts_debug_conv_tc.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, i32p, f32p, f32p, f32p, i32, f32p, f32p, i32,
                                        C.c_float, C.c_float, i32, f32p, f32p]
     u32p = C.POINTER(C.c_uint32)
@@ -828,6 +830,33 @@ class NativeEngine:
         self._chk(self.lib.xtts_debug_conv_tc(self.h, up, Cin, Cout, K, dil, B, L, _ip(il), _fp(w), _fp(b), _fp(cb),
                                               cb.shape[1] if cb is not None else 0, _fp(x), _fp(r), mode, slope_out,
                                               scale16, max_ctas, _fp(o32), _fp(o16)), "debug_conv_tc")
+        return o32, o16
+
+    def debug_resblock_tc(self, x, ws, bs, dil=(1, 3, 5), item_len=None, zs=None, mode: int = 0, pa=None,
+                          scale16: float = 1.0, max_ctas: int = 0, fused: bool = True):
+        """One vocoder ResBlock1 (include/xtts_b200.h): fused kernel (fused=True) or its six tensor-core conv launches.
+        x [batch, C, L] (L % 4 == 0); ws: six [C, C, K] weights and bs: six [C] biases, c1_0, c2_0, c1_1, c2_1, c1_2, c2_2.
+        zs [batch, C, L] and pa [batch, C / 8, atoms_lpad(L), 8] are the incoming contents (accumulate base, sentinels);
+        zs None = NaN, pa None = not produced.  -> (zs, pa) after the launch."""
+        x = _f32(x)
+        B, Cc, L = x.shape
+        w = np.ascontiguousarray(np.stack([_f32(a) for a in ws]))
+        b = np.ascontiguousarray(np.stack([_f32(a) for a in bs]))
+        if w.ndim != 4 or w.shape[:3] != (6, Cc, Cc) or b.shape != (6, Cc):
+            raise ValueError(f"six [C, C, K] weights and six [C] biases expected, got {w.shape} and {b.shape}")
+        d = _i32(dil)
+        if d.size != 3:
+            raise ValueError("dil must hold three dilations")
+        il = _i32(item_len) if item_len is not None else None
+        if il is not None and il.size != B:
+            raise ValueError(f"item_len has {il.size} elements, expected {B}")
+        o32 = _f32(zs).copy() if zs is not None else np.full((B, Cc, L), np.nan, np.float32)
+        o16 = _f32(pa).copy() if pa is not None else None
+        if o32.size != B * Cc * L or (o16 is not None and o16.size != B * Cc * atoms_lpad(L)):
+            raise ValueError("zs / pa do not match x")
+        self._chk(self.lib.xtts_debug_resblock_tc(self.h, Cc, w.shape[3], _ip(d), B, L, _ip(il), _fp(w), _fp(b), _fp(x),
+                                                  mode, scale16, max_ctas, int(bool(fused)), _fp(o32), _fp(o16)),
+                  "debug_resblock_tc")
         return o32, o16
 
     def debug_cond(self, op, dims, inputs=(), out=None, out_len: Optional[int] = None, scal=()):

@@ -308,6 +308,10 @@ int xtts_fetch(xtts_engine* e, uint64_t seq_id, int32_t* tokens, float* wav, flo
  *   "tc_epilogue"         epilogue of the fast-mode vocoder's tensor-core Conv1d: 1 (default) = staged through shared
  *                         memory (residual prefetched by a loader warp, outputs drained by bulk copies while the next
  *                         tile's MMAs run), 0 = straight from the accumulators.  Bit-identical results either way.
+ *   "tc_resblock"         test / measurement switch, not a tuning knob (the path follows from the channel count): 1
+ *                         (default) = the fast-mode vocoder's resblocks of 32 or 64 channels run as one fused kernel each
+ *                         (resblock_tc) wherever it takes their geometry, 0 = as six tensor-core Conv1d launches, for
+ *                         A/B timing and the bit-identity tests.  Bit-identical results.
  *   "attn_ctas_per_sm"    > 0 caps the decode-attention grid (each CTA walks several items); < 0: absolute grid size (tests)
  *   "profile"             1 = CUDA events around every launch (xtts_get_kernel_profile), "reset_stats" = zero the counters */
 int xtts_set_option(xtts_engine* e, const char* key, int64_t value);
@@ -450,6 +454,18 @@ int xtts_debug_conv_tc(xtts_engine* e, int32_t up, int32_t Cin, int32_t Cout, in
                        const int32_t* item_len, const float* w, const float* bias, const float* cbias, int32_t cbias_stride,
                        const float* x, const float* resid, int32_t mode, float slope_out, float scale16, int32_t max_ctas,
                        float* out32, float* out16);
+/* one ResBlock1 of the fast-mode vocoder on caller data: for t = 0..2 x <- x + c2_t(lrelu(c1_t(
+ * lrelu(x), dil[t]))) with c2_t of dilation 1, then zs = x (mode 0) or zs + x (mode 1), and (pa != NULL) pa = fp16(lrelu(
+ * zs * scale16, 0.1)) as atoms.  fused 1: one resblock_tc launch; 0: the six tensor-core Conv1d launches it replaces.  Both
+ * give the same bits.  w [6][C][C][K] and bias [6][C] in the order c1_0, c2_0, c1_1, c2_1, c1_2, c2_2; x [batch][C][L]
+ * with L % 4 == 0 and item_len (NULL = all L) as in xtts_debug_conv_tc; zs [batch][C][L] and pa [batch][C/8][lpad(L)][8]
+ * are in/out as there.  max_ctas > 0 caps the persistent grid.  Rejected before any launch: an even K, a dilation < 1,
+ * fused with C other than 32 / 64 or a halo (K-1)/2*(dil[0]+dil[1]+dil[2]+3) that is not a multiple of 4 or too wide
+ * for the fused tile, six launches with a C that has no tensor-core
+ * plan, batch outside 1..32, L_i > L. */
+int xtts_debug_resblock_tc(xtts_engine* e, int32_t C, int32_t K, const int32_t* dil, int32_t batch, int32_t L,
+                           const int32_t* item_len, const float* w, const float* bias, const float* x, int32_t mode,
+                           float scale16, int32_t max_ctas, int32_t fused, float* zs, float* pa);
 /* one speaker-conditioning kernel (csrc/cond.cu) on caller data, launched with the grid, block size and shared memory
  * xtts_condition uses.  dims [n_dims] and scal [n_scal] are the op's parameters; in [n_in] its fp32 inputs of in_len[i]
  * floats each; out [out_len] is in/out: uploaded before the launch (the base of the in-place ops, and what an element the
