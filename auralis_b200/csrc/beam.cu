@@ -332,23 +332,32 @@ beam_reorder_kernel(SampleState S, BeamArgs A) {
 }
 
 // grid (groups * kMaxBeams, layers, 2): the valid tokens of one partial page of one layer's K (z = 0) or V (z = 1) pool
-// K page: [head][64 / X][32 tok][X], V page: [head][32 tok][64], X * elem = 16 bytes
+// (page, head) block: K [64 / X][32 tok][X], V [32 tok][64], X * elem = 16 bytes; fp8 (elem 1): then 32 exponent bytes
 __global__ void __launch_bounds__(256)
 kv_page_copy_kernel(BeamArgs A, void* const* kpool, void* const* vpool, int heads, int elem) {
     const BeamDesc& d = A.desc[blockIdx.x / kMaxBeams];
     const BeamState& bs = A.state[d.primary];
     const int c = blockIdx.x % kMaxBeams;
     if (bs.done || c >= bs.n_copy) return;
-    const size_t page_vec = (size_t)heads * kPageTokens * kHeadDim * elem / 16;
-    uint4* base = reinterpret_cast<uint4*>(blockIdx.z == 0 ? kpool[blockIdx.y] : vpool[blockIdx.y]);
-    const uint4* src = base + (size_t)bs.copy_src[c] * page_vec;
-    uint4* dst = base + (size_t)bs.copy_dst[c] * page_vec;
+    const size_t blk = kv_block_bytes(elem), page_bytes = heads * blk;
+    uint8_t* base = reinterpret_cast<uint8_t*>(blockIdx.z == 0 ? kpool[blockIdx.y] : vpool[blockIdx.y]);
+    const uint8_t* src = base + (size_t)bs.copy_src[c] * page_bytes;
+    uint8_t* dst = base + (size_t)bs.copy_dst[c] * page_bytes;
     const int ntok = bs.copy_ntok[c];
+    const int data_vec = kPageTokens * kHeadDim * elem / 16;    // 16-byte vectors of element data per block
     const int vpr = kHeadDim * elem / 16;              // 16-byte vectors per V token row
+    const size_t page_vec = (size_t)heads * data_vec;
     for (size_t q = threadIdx.x; q < page_vec; q += blockDim.x) {
-        const int tk = blockIdx.z == 0 ? (int)(q % kPageTokens) : (int)((q / vpr) % kPageTokens);
-        if (tk < ntok) dst[q] = src[q];
+        const int v = (int)(q % data_vec);
+        const int tk = blockIdx.z == 0 ? v % kPageTokens : v / vpr;
+        const size_t off = (q / data_vec) * blk + (size_t)v * 16;
+        if (tk < ntok) *reinterpret_cast<uint4*>(dst + off) = *reinterpret_cast<const uint4*>(src + off);
     }
+    if (elem == 1)
+        for (int q = threadIdx.x; q < heads * kPageTokens; q += blockDim.x) {
+            const size_t off = (size_t)(q / kPageTokens) * blk + kv8_e_off(q % kPageTokens);
+            if (q % kPageTokens < ntok) dst[off] = src[off];
+        }
 }
 
 // one CTA per group that ended this step: backtrack the best finished hypothesis through the history and write its

@@ -34,6 +34,11 @@ static void set_error(const std::string& s) {
     g_last_error = s;
 }
 
+// a request the engine cannot take in its current state (XTTS_ERR_STATE), e.g. a KV format switch with work in flight
+struct StateError : std::runtime_error {
+    using std::runtime_error::runtime_error;
+};
+
 static double now_s() {
     using namespace std::chrono;
     return duration<double>(steady_clock::now().time_since_epoch()).count();
@@ -241,10 +246,15 @@ private:
     DBuf<RowDesc> d_rows;
     DBuf<AttnSeq> d_attnseq;
     bool use_forced = false;
-    // KV pools, one pair per layer
+    // KV pools, one pair per layer, in one format: fp32 (parity mode), 16-bit, or fp8 (option "kv_fp8", kv_fp8.cuh)
     std::vector<std::unique_ptr<DBuf<float>>> k32, v32;
     std::vector<std::unique_ptr<DBuf<__nv_bfloat16>>> k16, v16;
+    std::vector<std::unique_ptr<DBuf<uint8_t>>> k8, v8;
+    bool kv_fp8 = false;
     std::vector<int> free_pages;
+    void alloc_kv();              // the pools in the current format, d_kv_ptrs, every page free
+    __nv_fp8_e4m3* k8p(int l) const { return reinterpret_cast<__nv_fp8_e4m3*>(k8[l]->p); }
+    __nv_fp8_e4m3* v8p(int l) const { return reinterpret_cast<__nv_fp8_e4m3*>(v8[l]->p); }
     // GPT workspace
     DBuf<float> wX, wQKV, wLOG, wPART;
     DBuf<float> wXn32, wATT32, wFF32, wY32;
@@ -489,28 +499,7 @@ Engine::Engine(const xtts_config& c) : cfg(c) {
     if (bf16) { wXn16.alloc(Mmax * H); wATT16.alloc(Mmax * H); wFF16.alloc(Mmax * FF); wY16.alloc((size_t)std::max(NSLOT, CAP + 1) * H); }
     else { wXn32.alloc(Mmax * H); wATT32.alloc(Mmax * H); wFF32.alloc(Mmax * FF); wY32.alloc((size_t)std::max(NSLOT, CAP + 1) * H); }
 
-    // KV pools
-    const int total_pages = NSLOT * max_pages;
-    const size_t page_elems = (size_t)NH * kPageTokens * kHeadDim;
-    for (int l = 0; l < L; ++l) {
-        if (bf16) {
-            k16.emplace_back(new DBuf<__nv_bfloat16>()); v16.emplace_back(new DBuf<__nv_bfloat16>());
-            k16.back()->alloc(total_pages * page_elems); v16.back()->alloc(total_pages * page_elems);
-        } else {
-            k32.emplace_back(new DBuf<float>()); v32.emplace_back(new DBuf<float>());
-            k32.back()->alloc(total_pages * page_elems); v32.back()->alloc(total_pages * page_elems);
-        }
-    }
-    {
-        std::vector<void*> kv(2 * L);
-        for (int l = 0; l < L; ++l) {
-            kv[l] = bf16 ? (void*)k16[l]->p : (void*)k32[l]->p;
-            kv[L + l] = bf16 ? (void*)v16[l]->p : (void*)v32[l]->p;
-        }
-        d_kv_ptrs.alloc(2 * L); d_kv_ptrs.upload(kv.data(), 2 * L, st);
-        CUDA_CHECK(cudaStreamSynchronize(st));
-    }
-    for (int p = total_pages - 1; p >= 0; --p) free_pages.push_back(p);
+    alloc_kv();
     for (int s = B - 1; s >= 0; --s) free_slots.push_back(s);
 
     // vocoder workspace: a batch is up to kVocMaxItems windows, nb x (longest window) <= voc_cap_z z-frames
@@ -534,6 +523,34 @@ Engine::Engine(const xtts_config& c) : cfg(c) {
     CUDA_CHECK(cudaStreamSynchronize(st));
     launch_base = g_launch_count;
     worker = std::thread([this] { this->loop(); });
+}
+
+// KV pools of every layer in the current format (the old ones are freed first, so a switch never holds both), their base
+// pointers for the beam kernels, and a free list of every page
+void Engine::alloc_kv() {
+    k32.clear(); v32.clear(); k16.clear(); v16.clear(); k8.clear(); v8.clear();
+    const int total_pages = NSLOT * max_pages;
+    const size_t page_elems = (size_t)NH * kPageTokens * kHeadDim;
+    std::vector<void*> kv(2 * L);
+    for (int l = 0; l < L; ++l) {
+        if (kv_fp8) {
+            k8.emplace_back(new DBuf<uint8_t>()); v8.emplace_back(new DBuf<uint8_t>());
+            k8.back()->alloc(total_pages * NH * kv_block_bytes(1)); v8.back()->alloc(total_pages * NH * kv_block_bytes(1));
+            kv[l] = k8[l]->p; kv[L + l] = v8[l]->p;
+        } else if (bf16) {
+            k16.emplace_back(new DBuf<__nv_bfloat16>()); v16.emplace_back(new DBuf<__nv_bfloat16>());
+            k16.back()->alloc(total_pages * page_elems); v16.back()->alloc(total_pages * page_elems);
+            kv[l] = k16[l]->p; kv[L + l] = v16[l]->p;
+        } else {
+            k32.emplace_back(new DBuf<float>()); v32.emplace_back(new DBuf<float>());
+            k32.back()->alloc(total_pages * page_elems); v32.back()->alloc(total_pages * page_elems);
+            kv[l] = k32[l]->p; kv[L + l] = v32[l]->p;
+        }
+    }
+    d_kv_ptrs.alloc(2 * L); d_kv_ptrs.upload(kv.data(), 2 * L, st);
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    free_pages.clear();
+    for (int p = total_pages - 1; p >= 0; --p) free_pages.push_back(p);
 }
 
 // receptive field of the generator in z-frames: conv_pre, per stage the transposed conv (1.5 input frames) and the widest
@@ -959,7 +976,8 @@ void Engine::layers_forward(int M, bool prefill, int nseq, int max_nq) {
         if (!splitk) ln(ly.ln1w.p, ly.ln1b.p);
         gemm(Xn, ly.qkv, nullptr, wQKV.p, M, 0, pdl);
         if (prefill) {
-            if (f16) launch_kv_write<__half>(wQKV.p, M, d_row_slot.p, d_row_pos.p, d_ctx_len.p, d_block_tables.p, max_pages, reinterpret_cast<__half*>(k16[l]->p), reinterpret_cast<__half*>(v16[l]->p), NH, st);
+            if (kv_fp8) launch_kv_write<__nv_fp8_e4m3>(wQKV.p, M, d_row_slot.p, d_row_pos.p, d_ctx_len.p, d_block_tables.p, max_pages, k8p(l), v8p(l), NH, st);
+            else if (f16) launch_kv_write<__half>(wQKV.p, M, d_row_slot.p, d_row_pos.p, d_ctx_len.p, d_block_tables.p, max_pages, reinterpret_cast<__half*>(k16[l]->p), reinterpret_cast<__half*>(v16[l]->p), NH, st);
             else if (bf16) launch_kv_write<__nv_bfloat16>(wQKV.p, M, d_row_slot.p, d_row_pos.p, d_ctx_len.p, d_block_tables.p, max_pages, k16[l]->p, v16[l]->p, NH, st);
             else launch_kv_write<float>(wQKV.p, M, d_row_slot.p, d_row_pos.p, d_ctx_len.p, d_block_tables.p, max_pages, k32[l]->p, v32[l]->p, NH, st);
             AttnLayout A;
@@ -971,7 +989,9 @@ void Engine::layers_forward(int M, bool prefill, int nseq, int max_nq) {
             else launch_attn_generic<float>(A, d_attnseq.p, nseq, max_nq, wATT32.p, H, st);
         } else {
             // (the attention kernel appends this step's K/V to the cache itself)
-            if (f16) launch_attn_decode<__half, __half>(wQKV.p, d_active.p, M, d_ctx_len.p, d_block_tables.p, max_pages, reinterpret_cast<__half*>(k16[l]->p), reinterpret_cast<__half*>(v16[l]->p), reinterpret_cast<__half*>(wATT16.p), NH, st, decode_ctx_sum, pdl);
+            if (kv_fp8 && f16) launch_attn_decode<__nv_fp8_e4m3, __half>(wQKV.p, d_active.p, M, d_ctx_len.p, d_block_tables.p, max_pages, k8p(l), v8p(l), reinterpret_cast<__half*>(wATT16.p), NH, st, decode_ctx_sum, pdl);
+            else if (kv_fp8) launch_attn_decode<__nv_fp8_e4m3, __nv_bfloat16>(wQKV.p, d_active.p, M, d_ctx_len.p, d_block_tables.p, max_pages, k8p(l), v8p(l), wATT16.p, NH, st, decode_ctx_sum, pdl);
+            else if (f16) launch_attn_decode<__half, __half>(wQKV.p, d_active.p, M, d_ctx_len.p, d_block_tables.p, max_pages, reinterpret_cast<__half*>(k16[l]->p), reinterpret_cast<__half*>(v16[l]->p), reinterpret_cast<__half*>(wATT16.p), NH, st, decode_ctx_sum, pdl);
             else if (bf16) launch_attn_decode<__nv_bfloat16, __nv_bfloat16>(wQKV.p, d_active.p, M, d_ctx_len.p, d_block_tables.p, max_pages, k16[l]->p, v16[l]->p, wATT16.p, NH, st, decode_ctx_sum, pdl);
             else launch_attn_decode<float, float>(wQKV.p, d_active.p, M, d_ctx_len.p, d_block_tables.p, max_pages, k32[l]->p, v32[l]->p, wATT32.p, NH, st, decode_ctx_sum, pdl);
         }
@@ -1098,7 +1118,7 @@ void Engine::beam_step(const std::vector<Sequence*>& groups, const std::vector<i
     a.desc = d_beam_desc.p; a.n_groups = (int)groups.size(); a.state = d_beam_state.p; a.hist = d_beam_hist.p;
     a.pool = d_beam_pool.p; a.pool_cap = beam_pool_cap; a.scores = d_beam_scores.p; a.block_tables = d_block_tables.p;
     a.max_pages = max_pages; a.latents = d_latents.p; a.H = H;
-    launch_beam_step(wLOG.p, Vpad, V, sample_state(), a, d_kv_ptrs.p, d_kv_ptrs.p + L, L, NH, bf16 ? 2 : 4, st);
+    launch_beam_step(wLOG.p, Vpad, V, sample_state(), a, d_kv_ptrs.p, d_kv_ptrs.p + L, L, NH, kv_fp8 ? 1 : bf16 ? 2 : 4, st);
 }
 
 // builds row descriptors for [prompt ; optional forced audio rows] of each sequence; returns total rows
@@ -1172,7 +1192,13 @@ void Engine::decode_layers_rows(int r0, int Mi, cudaStream_t s, bool pdl_first, 
     for (int l = 0; l < L; ++l) {
         Layer& ly = *layers[l];
         launch_gemm_bf16_tc(Xn, ly.qkv.w16.p, ly.qkv.b.p, nullptr, QKV, Mi, ly.qkv.N, ly.qkv.K, gflag, s, pdl);
-        if (f16)
+        if (kv_fp8 && f16)
+            launch_attn_decode<__nv_fp8_e4m3, __half>(QKV, act, Mi, d_ctx_len.p, d_block_tables.p, max_pages, k8p(l), v8p(l),
+                                                      reinterpret_cast<__half*>(ATT), NH, s, ctx_sum, pdl);
+        else if (kv_fp8)
+            launch_attn_decode<__nv_fp8_e4m3, __nv_bfloat16>(QKV, act, Mi, d_ctx_len.p, d_block_tables.p, max_pages, k8p(l), v8p(l),
+                                                             ATT, NH, s, ctx_sum, pdl);
+        else if (f16)
             launch_attn_decode<__half, __half>(QKV, act, Mi, d_ctx_len.p, d_block_tables.p, max_pages, reinterpret_cast<__half*>(k16[l]->p),
                                                reinterpret_cast<__half*>(v16[l]->p), reinterpret_cast<__half*>(ATT), NH, s, ctx_sum, pdl);
         else
@@ -2090,6 +2116,21 @@ void Engine::set_option(const std::string& k, int64_t v) {
         if (v != 0 && (v < 2 || v > 4)) throw std::runtime_error("gemm_wide: 0 (off) or a ring depth of 2, 3 or 4");
         g_gemm_wide = (int)v;
     }
+    else if (k == "kv_fp8") {
+        if (v != 0 && v != 1) throw std::runtime_error("kv_fp8: 0 (16-bit cache) or 1 (fp8 e4m3 cache)");
+        if (!bf16) throw std::runtime_error("kv_fp8: the fp8 KV cache needs precision bf16 or fp16");
+        if ((v != 0) == kv_fp8) return;
+        bool queued;
+        { std::lock_guard<std::mutex> q(q_mu); queued = !pending.empty(); }
+        if (queued || !running.empty() || !waiting.empty() || !voc_pending.empty() || !voc_inflight.empty() ||
+            (int)free_pages.size() != NSLOT * max_pages)
+            throw StateError("kv_fp8: the KV format can only change on an idle engine");
+        CUDA_CHECK(cudaSetDevice(cfg.device));
+        CUDA_CHECK(cudaStreamSynchronize(st));
+        drop_graphs();                                  // captured decode steps hold the old pools and kernels
+        kv_fp8 = v != 0;
+        alloc_kv();
+    }
     else if (k == "cuda_graphs") use_graphs = v != 0;
     else if (k == "pdl") { use_pdl = v != 0; drop_graphs(); }
     else if (k == "splitk") { use_splitk = v != 0; drop_graphs(); }
@@ -2344,6 +2385,7 @@ struct xtts_engine { Engine* impl; };
 #define XTTS_TRY(body)                                                  \
     try { Engine::Bind bind_ctx_(e->impl); body; return XTTS_OK; }      \
     catch (const xtts::CudaError& ex) { xtts::set_error(ex.what()); return XTTS_ERR_CUDA; } \
+    catch (const xtts::StateError& ex) { xtts::set_error(ex.what()); return XTTS_ERR_STATE; } \
     catch (const std::exception& ex) { xtts::set_error(ex.what()); return XTTS_ERR_INVALID; } \
     catch (...) { xtts::set_error("unknown error"); return XTTS_ERR_INVALID; }
 

@@ -9,6 +9,7 @@
 //   K10    hijack.py:49-88 LogitsRepetitionPenalizer                                    -> sample (penalty)
 //   K11    vLLM Sampler (SURVEY App. A.3)                                               -> sample
 #include <algorithm>
+#include <type_traits>
 #include "kernels.h"
 
 namespace xtts {
@@ -210,6 +211,22 @@ __global__ void kv_write_kernel(const float* __restrict__ QKV, const int* __rest
     }
 }
 
+// the fp8 cache (kv_fp8.cuh): same grid and thread roles, each (row, head) quantised with its own K and V exponents
+__global__ void __launch_bounds__(128)
+kv_write_fp8_kernel(const float* __restrict__ QKV, const int* __restrict__ row_slot, const int* __restrict__ row_pos,
+                    const int* __restrict__ ctx_len, const int* __restrict__ block_tables, int max_pages,
+                    uint8_t* __restrict__ kpool, uint8_t* __restrict__ vpool, int heads) {
+    __shared__ float red[4];
+    const int r = blockIdx.x, h = blockIdx.y;
+    const int H = heads * kHeadDim;
+    const int slot = row_slot[r];
+    const int pos = row_pos ? row_pos[r] : ctx_len[slot];
+    const size_t b = kv8_block(block_tables[(size_t)slot * max_pages + pos / kPageTokens], heads, h);
+    const int t = threadIdx.x;
+    const float x = QKV[(size_t)r * 3 * H + (t < 64 ? H : 2 * H) + h * kHeadDim + (t & 63)];
+    kv8_append(x, kpool + b, vpool + b, pos % kPageTokens, red);
+}
+
 // ------------------------------------------------------------------------------------------------
 // decode attention over the paged cache: one CTA per (sequence, head); 4 warps split the pages;
 // lane = token inside a page for QK^T (16-byte coalesced K reads), lane = 2 output dims for PV.
@@ -243,6 +260,56 @@ __device__ __forceinline__ uint4 ldg_stream(const void* p) {          // streami
     asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];"
                  : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
     return r;
+}
+
+// End of one fp8 decode-attention item, after each warp's pages: warp 0 adds the step's own token from shared memory, then
+// the token groups of each warp (lanes with equal dim chunk) and the NW warps are folded into head h of output row i.  X:
+// dims per lane, so 64 / X lanes cover a token row.  The same steps as the end of attn_decode_kernel, which keeps them
+// inline: calling this from there changes its instruction schedule.
+template <int X, int NW, typename TOut>
+__device__ __forceinline__ void attn_decode_tail(const float* qs, const float* ks, const float* vs, float* pm, float* pl,
+                                                 float (*pacc)[kHeadDim], float m, float l, float* acc, TOut* __restrict__ out,
+                                                 int i, int h, int H) {
+    constexpr int NCH = kHeadDim / X;
+    const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+    const int tg = lane / NCH, dc = lane % NCH;
+    if (w == 0) {
+        // ---- the step's own token, from shared memory
+        float s = qs[lane] * ks[lane] + qs[lane + 32] * ks[lane + 32];
+        s = warp_sum(s);
+        const float mnew = fmaxf(m, s);
+        const float p = expf(s - mnew);
+        const float corr = (m == -INFINITY) ? 0.f : expf(m - mnew);
+        l = l * corr + p;
+#pragma unroll
+        for (int e = 0; e < X; ++e) acc[e] = acc[e] * corr + ((tg == 0) ? p * vs[dc * X + e] : 0.f);
+        m = mnew;
+    }
+    // ---- fold the token groups of the warp (lanes with equal dc), then the 4 warps
+#pragma unroll
+    for (int o = NCH; o < 32; o <<= 1)
+#pragma unroll
+        for (int e = 0; e < X; ++e) acc[e] += __shfl_xor_sync(0xffffffffu, acc[e], o);
+    if (lane == 0) { pm[w] = m; pl[w] = l; }
+    if (lane < NCH) {
+#pragma unroll
+        for (int e = 0; e < X; ++e) pacc[w][dc * X + e] = acc[e];
+    }
+    __syncthreads();
+    for (int t = tid; t < kHeadDim; t += 32 * NW) {
+        float M = pm[0];
+#pragma unroll
+        for (int k = 1; k < NW; ++k) M = fmaxf(M, pm[k]);
+        float L = 0.f, o = 0.f;
+#pragma unroll
+        for (int k = 0; k < NW; ++k) {
+            const float e = (pm[k] == -INFINITY) ? 0.f : expf(pm[k] - M);
+            L = fmaf(pl[k], e, L);
+            o = fmaf(pacc[k][t], e, o);
+        }
+        out[(size_t)i * H + h * kHeadDim + t] = from_f32<TOut>(o / L);
+    }
+    __syncthreads();                                  // qs/ks/vs/pacc are reused by the next item
 }
 
 // One CTA per (sequence, head); the 4 warps take pages round-robin.  Per 32-token page a warp issues
@@ -383,6 +450,117 @@ attn_decode_kernel(const float* __restrict__ QKV, const int* __restrict__ active
         out[(size_t)i * H + h * kHeadDim + t] = from_f32<TOut>(o / L);
     }
     __syncthreads();                                  // qs/ks/vs/pacc are reused by the next item
+    }
+    trace_pt(TR_ATTN, 2);
+}
+
+// The fp8 cache (kv_fp8.cuh).  A page is half the bytes of a 16-bit page, and the kernel is bound by the bytes each warp
+// keeps in flight, so a warp takes two of its pages per iteration (pages pg and pg + NW: the same pages per warp as the
+// 16-bit kernel): 8 K + 8 V 16-byte loads up front, as there, plus each lane's K and V exponent byte.  The exponents are
+// applied to the score (2^ek) and to p_j before the PV broadcast (2^ev); l sums the unscaled p.  The step's own token is
+// appended in the fp8 format and attended to as its dequantised values.
+template <typename TOut>
+__global__ void __launch_bounds__(128)
+attn_decode_fp8_kernel(const float* __restrict__ QKV, const int* __restrict__ active, const int* __restrict__ ctx_len,
+                       const int* __restrict__ block_tables, int max_pages, uint8_t* __restrict__ kpool,
+                       uint8_t* __restrict__ vpool, TOut* __restrict__ out, int heads, int n_items) {
+    constexpr int NW = 4;                             // kv8_append: one thread per K / V element of the new token
+    constexpr int X = kKv8X;
+    constexpr int NCH = kHeadDim / X;                 // 4 atoms per token row
+    constexpr int TPI = 32 / NCH;                     // 8 tokens per warp-wide V load
+    constexpr int VIT = kPageTokens / TPI;            // 4 V loads per page
+    __shared__ __align__(16) float qs[kHeadDim], ks[kHeadDim], vs[kHeadDim];
+    __shared__ float pm[NW], pl[NW], red[NW];
+    __shared__ float pacc[NW][kHeadDim];
+    trace_pt(TR_ATTN, 0); pdl_trigger();
+    pdl_wait();
+    trace_pt(TR_ATTN, 1);
+    const int H = heads * kHeadDim;
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+    const int i = item / heads, h = item - i * heads;
+    const int slot = active[i];
+    const int past = ctx_len[slot];
+    const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+    const int* bt = block_tables + (size_t)slot * max_pages;
+    {
+        const float* row = QKV + (size_t)i * 3 * H + h * kHeadDim;
+        const size_t b = kv8_block(bt[past / kPageTokens], heads, h);
+        const int dd = tid & 63;
+        const float x = kv8_append(row[(tid < 64 ? H : 2 * H) + dd], kpool + b, vpool + b, past % kPageTokens, red);
+        if (tid < 64) { qs[dd] = row[dd] * 0.125f; ks[dd] = x; } else vs[dd] = x;
+    }
+    __syncthreads();
+    const int tg = lane / NCH, dc = lane % NCH;
+    float m = -INFINITY, l = 0.f;
+    float acc[X];
+#pragma unroll
+    for (int e = 0; e < X; ++e) acc[e] = 0.f;
+    const int npages = (past + kPageTokens - 1) / kPageTokens;
+    for (int pg = w; pg < npages; pg += 2 * NW) {
+        // ---- issue every load of both pages up front
+        uint4 kraw[2][NCH], vraw[2][VIT];
+        int ek[2] = {0, 0}, ev[2] = {0, 0}, nvalid[2] = {0, 0};
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+            const int p = pg + u * NW;
+            if (p < npages) {
+                const size_t b = kv8_block(bt[p], heads, h);
+                nvalid[u] = min(kPageTokens, past - p * kPageTokens);
+                const uint8_t* kb = kpool + b + (size_t)lane * X;
+#pragma unroll
+                for (int c = 0; c < NCH; ++c) kraw[u][c] = ldg_stream(kb + (size_t)c * kPageTokens * X);
+                const uint8_t* vb = vpool + b + (size_t)tg * kHeadDim + (size_t)dc * X;
+#pragma unroll
+                for (int it = 0; it < VIT; ++it) vraw[u][it] = ldg_stream(vb + (size_t)it * TPI * kHeadDim);
+                ek[u] = (int8_t)__ldg(kpool + b + kv8_e_off(lane));
+                ev[u] = (int8_t)__ldg(vpool + b + kv8_e_off(lane));
+            } else {
+#pragma unroll
+                for (int c = 0; c < NCH; ++c) kraw[u][c] = make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll
+                for (int it = 0; it < VIT; ++it) vraw[u][it] = make_uint4(0u, 0u, 0u, 0u);
+            }
+        }
+        // ---- scores of both pages, one softmax update
+        float s[2];
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+            float d = 0.f;
+#pragma unroll
+            for (int c = 0; c < NCH; ++c) {
+                float kf[X];
+                kv8_unpack16(kraw[u][c], kf);
+#pragma unroll
+                for (int e = 0; e < X; ++e) d = fmaf(kf[e], qs[c * X + e], d);
+            }
+            s[u] = lane < nvalid[u] ? d * kv8_pow2(ek[u]) : -INFINITY;
+        }
+        const float mnew = fmaxf(m, warp_max(fmaxf(s[0], s[1])));
+        const float p0 = lane < nvalid[0] ? expf(s[0] - mnew) : 0.f;
+        const float p1 = lane < nvalid[1] ? expf(s[1] - mnew) : 0.f;
+        const float corr = (m == -INFINITY) ? 0.f : expf(m - mnew);
+        l = l * corr + warp_sum(p0 + p1);
+#pragma unroll
+        for (int e = 0; e < X; ++e) acc[e] *= corr;
+        // ---- PV: lane j's weight carries its token's V scale
+        const float pv[2] = {p0 * kv8_pow2(ev[0]), p1 * kv8_pow2(ev[1])};
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+#pragma unroll
+            for (int it = 0; it < VIT; ++it) {
+                const int j = it * TPI + tg;
+                const float pj = __shfl_sync(0xffffffffu, pv[u], j);
+                if (j < nvalid[u]) {                    // stale page tails are never multiplied in
+                    float vf[X];
+                    kv8_unpack16(vraw[u][it], vf);
+#pragma unroll
+                    for (int e = 0; e < X; ++e) acc[e] = fmaf(pj, vf[e], acc[e]);
+                }
+            }
+        }
+        m = mnew;
+    }
+    attn_decode_tail<X, NW>(qs, ks, vs, pm, pl, pacc, m, l, acc, out, i, h, H);
     }
     trace_pt(TR_ATTN, 2);
 }
@@ -862,23 +1040,32 @@ template <typename TKV>
 void launch_kv_write(const float* QKV, int M, const int* row_slot, const int* row_pos, const int* ctx_len,
                      const int* block_tables, int max_pages, TKV* kpool, TKV* vpool, int heads, cudaStream_t st) {
     if (M <= 0) return;
-    ProfScope ps(KF_KV_WRITE, st, 0, (8.0 + 2.0 * sizeof(TKV)) * M * heads * kHeadDim);
-    kv_write_kernel<TKV><<<dim3(M, heads), 128, 0, st>>>(QKV, row_slot, row_pos, ctx_len, block_tables, max_pages,
-                                                         kpool, vpool, heads);
+    if constexpr (std::is_same_v<TKV, __nv_fp8_e4m3>) {
+        // fp32 QKV in, e4m3 bytes + one exponent byte per (row, head) for K and for V out
+        ProfScope ps(KF_KV_WRITE, st, 0, (8.0 * kHeadDim + 2.0 * (kHeadDim + 1)) * M * heads);
+        kv_write_fp8_kernel<<<dim3(M, heads), 128, 0, st>>>(QKV, row_slot, row_pos, ctx_len, block_tables, max_pages,
+                                                            reinterpret_cast<uint8_t*>(kpool), reinterpret_cast<uint8_t*>(vpool), heads);
+    } else {
+        ProfScope ps(KF_KV_WRITE, st, 0, (8.0 + 2.0 * sizeof(TKV)) * M * heads * kHeadDim);
+        kv_write_kernel<TKV><<<dim3(M, heads), 128, 0, st>>>(QKV, row_slot, row_pos, ctx_len, block_tables, max_pages,
+                                                             kpool, vpool, heads);
+    }
     COUNT_LAUNCH(); KERNEL_CHECK();
 }
 template void launch_kv_write<float>(const float*, int, const int*, const int*, const int*, const int*, int, float*, float*, int, cudaStream_t);
 template void launch_kv_write<__nv_bfloat16>(const float*, int, const int*, const int*, const int*, const int*, int, __nv_bfloat16*, __nv_bfloat16*, int, cudaStream_t);
 template void launch_kv_write<__half>(const float*, int, const int*, const int*, const int*, const int*, int, __half*, __half*, int, cudaStream_t);
+template void launch_kv_write<__nv_fp8_e4m3>(const float*, int, const int*, const int*, const int*, const int*, int, __nv_fp8_e4m3*, __nv_fp8_e4m3*, int, cudaStream_t);
 
 template <typename TKV, typename TOut>
 void launch_attn_decode(const float* QKV, const int* active, int M, const int* ctx_len, const int* block_tables,
                         int max_pages, TKV* kpool, TKV* vpool, TOut* out, int heads, cudaStream_t st,
                         double ctx_sum_hint, bool pdl) {
     if (M <= 0) return;
-    // algorithmic bytes: K and V of every cached token of every sequence, once
-    ProfScope ps(KF_ATTN_DECODE, st, 4.0 * ctx_sum_hint * heads * kHeadDim,
-                 2.0 * ctx_sum_hint * heads * kHeadDim * sizeof(TKV));
+    constexpr bool fp8 = std::is_same_v<TKV, __nv_fp8_e4m3>;
+    // algorithmic bytes: K and V of every cached token of every sequence, once (fp8: with the token's exponent byte)
+    const double tok_bytes = fp8 ? kHeadDim + 1.0 : (double)kHeadDim * sizeof(TKV);
+    ProfScope ps(KF_ATTN_DECODE, st, 4.0 * ctx_sum_hint * heads * kHeadDim, 2.0 * ctx_sum_hint * heads * tok_bytes);
     const int n_items = M * heads;
     int grid = n_items;
     if (g_attn_ctas_per_sm > 0) {
@@ -886,13 +1073,19 @@ void launch_attn_decode(const float* QKV, const int* active, int M, const int* c
     } else if (g_attn_ctas_per_sm < 0) {
         grid = std::min(n_items, -g_attn_ctas_per_sm);          // test hook: an absolute grid size
     }
-    launch_k(attn_decode_kernel<TKV, TOut, 4>, dim3(grid), dim3(128), 0, st, pdl, QKV, active, ctx_len, block_tables, max_pages,
-             kpool, vpool, out, heads, n_items);
+    if constexpr (fp8)
+        launch_k(attn_decode_fp8_kernel<TOut>, dim3(grid), dim3(128), 0, st, pdl, QKV, active, ctx_len, block_tables, max_pages,
+                 reinterpret_cast<uint8_t*>(kpool), reinterpret_cast<uint8_t*>(vpool), out, heads, n_items);
+    else
+        launch_k(attn_decode_kernel<TKV, TOut, 4>, dim3(grid), dim3(128), 0, st, pdl, QKV, active, ctx_len, block_tables, max_pages,
+                 kpool, vpool, out, heads, n_items);
     COUNT_LAUNCH(); KERNEL_CHECK();
 }
 template void launch_attn_decode<float, float>(const float*, const int*, int, const int*, const int*, int, float*, float*, float*, int, cudaStream_t, double, bool);
 template void launch_attn_decode<__nv_bfloat16, __nv_bfloat16>(const float*, const int*, int, const int*, const int*, int, __nv_bfloat16*, __nv_bfloat16*, __nv_bfloat16*, int, cudaStream_t, double, bool);
 template void launch_attn_decode<__half, __half>(const float*, const int*, int, const int*, const int*, int, __half*, __half*, __half*, int, cudaStream_t, double, bool);
+template void launch_attn_decode<__nv_fp8_e4m3, __nv_bfloat16>(const float*, const int*, int, const int*, const int*, int, __nv_fp8_e4m3*, __nv_fp8_e4m3*, __nv_bfloat16*, int, cudaStream_t, double, bool);
+template void launch_attn_decode<__nv_fp8_e4m3, __half>(const float*, const int*, int, const int*, const int*, int, __nv_fp8_e4m3*, __nv_fp8_e4m3*, __half*, int, cudaStream_t, double, bool);
 
 template <typename TOut>
 void launch_attn_generic(AttnLayout L, const AttnSeq* seqs, int nseq, int max_nq, TOut* out, int out_row_stride,

@@ -24,6 +24,22 @@ auto with_elem(int type, const char* what, F&& f) {
     throw std::runtime_error(std::string(what) + " 0 (fp32), 1 (bf16) or 2 (fp16)");
 }
 
+// Calls f with a null cache-element pointer and a null attention-output pointer for the KV type of the debug entry points:
+// 0..2 the cache in the output type (as with_elem), 3 / 4 the fp8 cache (kv_fp8.cuh) with fp16 / bf16 output.
+template <typename F>
+auto with_kv(int kv_type, const char* what, F&& f) {
+    switch (kv_type) {
+    case 3: return f(static_cast<__nv_fp8_e4m3*>(nullptr), static_cast<__half*>(nullptr));
+    case 4: return f(static_cast<__nv_fp8_e4m3*>(nullptr), static_cast<__nv_bfloat16*>(nullptr));
+    }
+    if (kv_type < 0 || kv_type > 2)
+        throw std::runtime_error(std::string(what) + " 0 (fp32), 1 (bf16), 2 (fp16), 3 (fp8, fp16 out) or 4 (fp8, bf16 out)");
+    return with_elem(kv_type, what, [&](auto* tag) { return f(tag, tag); });
+}
+
+// element type -> the type code of download_f32
+template <typename T> constexpr int type_code() { return std::is_same_v<T, float> ? 0 : std::is_same_v<T, __half> ? 2 : 1; }
+
 // host h[0 .. n) in a new device buffer; an empty buffer (p == NULL) for a NULL h
 template <typename T>
 DBuf<T> to_dev(const T* h, size_t n, cudaStream_t st) {
@@ -205,8 +221,9 @@ void debug_sample_slots(const HarnessCtx& c, int Vn, int M, const int32_t* activ
 void debug_attn_decode(const HarnessCtx& c, int kv_type, int heads, int M, const int32_t* active, int n_slots,
                        const int32_t* ctx_len, const int32_t* block_tables, int mp, int n_pages, void* kpool, void* vpool,
                        const float* qkv, float* out) {
-    with_elem(kv_type, "debug_attn_decode: kv_type", [&](auto* tag) {
+    with_kv(kv_type, "debug_attn_decode: kv_type", [&](auto* tag, auto* otag) {
         using T = std::remove_pointer_t<decltype(tag)>;
+        using TO = std::remove_pointer_t<decltype(otag)>;
         if (heads < 1 || M < 1 || n_slots < 1 || mp < 1 || n_pages < 1) throw std::runtime_error("debug_attn_decode: empty problem");
         // the kernels' contract: distinct active slots, the new token's page inside the block table, page ids inside the pool
         check_active(active, M, n_slots, "debug_attn_decode: active slots must be distinct and < n_slots");
@@ -216,16 +233,18 @@ void debug_attn_decode(const HarnessCtx& c, int kv_type, int heads, int M, const
             check_pages(block_tables + (size_t)s * mp, ctx_len[s] / kPageTokens + 1, n_pages, "debug_attn_decode: page id outside the pool");
         }
         const cudaStream_t st = c.st;
-        const size_t pool = (size_t)n_pages * heads * kPageTokens * kHeadDim, Hq = (size_t)heads * kHeadDim;
+        const size_t pool = (size_t)n_pages * heads * kv_block_bytes(sizeof(T)), Hq = (size_t)heads * kHeadDim;
         DBuf<int> dact = to_dev(active, M, st), dctx = to_dev(ctx_len, n_slots, st), dbt = to_dev(block_tables, (size_t)n_slots * mp, st);
         DBuf<float> dqkv = to_dev(qkv, (size_t)M * 3 * Hq, st);
-        DBuf<T> dk = to_dev(static_cast<const T*>(kpool), pool, st), dv = to_dev(static_cast<const T*>(vpool), pool, st), dout;
+        DBuf<uint8_t> dk = to_dev(static_cast<const uint8_t*>(kpool), pool, st), dv = to_dev(static_cast<const uint8_t*>(vpool), pool, st);
+        DBuf<TO> dout;
         dout.alloc((size_t)M * Hq);
         double ctx_sum = 0;
         for (int i = 0; i < M; ++i) ctx_sum += ctx_len[active[i]];
-        launch_attn_decode<T, T>(dqkv.p, dact.p, M, dctx.p, dbt.p, mp, dk.p, dv.p, dout.p, heads, st, ctx_sum);
-        dk.download(static_cast<T*>(kpool), pool, st); dv.download(static_cast<T*>(vpool), pool, st);
-        download_f32(dout.p, kv_type, out, (size_t)M * Hq, st);
+        launch_attn_decode<T, TO>(dqkv.p, dact.p, M, dctx.p, dbt.p, mp, reinterpret_cast<T*>(dk.p), reinterpret_cast<T*>(dv.p),
+                                  dout.p, heads, st, ctx_sum);
+        dk.download(static_cast<uint8_t*>(kpool), pool, st); dv.download(static_cast<uint8_t*>(vpool), pool, st);
+        download_f32(dout.p, type_code<TO>(), out, (size_t)M * Hq, st);
     });
 }
 
@@ -238,7 +257,7 @@ void debug_beam_step(const HarnessCtx& c, int kv_type, int heads, int layers, in
     static_assert(sizeof(xtts_beam_state) == sizeof(BeamState), "xtts_beam_state mirrors BeamState");
     const int nb = bm.num_beams;
     auto bad = [](const char* m) { throw std::runtime_error(std::string("debug_beam_step: ") + m); };
-    const size_t esz = with_elem(kv_type, "debug_beam_step: kv_type", [](auto* tag) { return sizeof(*tag); });
+    const size_t esz = with_kv(kv_type, "debug_beam_step: kv_type", [](auto* tag, auto*) { return sizeof(*tag); });
     if (nb < 2 || nb > kMaxBeams) bad("num_beams 2..8");
     if (heads < 1 || layers < 1 || Vn < 2 * nb || n_pages < 1 || cap < 1 || mp < 1) bad("empty problem");
     if (!beam_supported(Vn, mp, cap)) bad("geometry outside the beam kernels' limits");
@@ -262,7 +281,7 @@ void debug_beam_step(const HarnessCtx& c, int kv_type, int heads, int layers, in
     if (held + bs.n_free > pool_cap) bad("pool and tables exceed nb * max_pages pages");
     if (n_gen[0] < 0 || n_gen[0] >= cap) bad("n_gen outside the history");
     const cudaStream_t st = c.st;
-    const size_t page_bytes = (size_t)heads * kPageTokens * kHeadDim * esz, pool_bytes = (size_t)layers * n_pages * page_bytes;
+    const size_t page_bytes = (size_t)heads * kv_block_bytes((int)esz), pool_bytes = (size_t)layers * n_pages * page_bytes;
     BeamDesc d{};
     d.primary = 0; d.nb = nb; d.first = first != 0; d.advance = advance; d.do_sample = bm.do_sample != 0;
     d.length_penalty = bm.length_penalty;
@@ -437,7 +456,7 @@ void debug_norms(const HarnessCtx& c, int out_type, int M, int H, const float* X
 void debug_kv_write(const HarnessCtx& c, int kv_type, int heads, int M, const float* qkv, const int32_t* row_slot,
                     const int32_t* row_pos, int n_slots, const int32_t* ctx_len, const int32_t* block_tables, int mp,
                     int n_pages, void* kpool, void* vpool) {
-    with_elem(kv_type, "debug_kv_write: kv_type", [&](auto* tag) {
+    with_kv(kv_type, "debug_kv_write: kv_type", [&](auto* tag, auto*) {
         using T = std::remove_pointer_t<decltype(tag)>;
         if (heads < 1 || M < 1 || n_slots < 1 || mp < 1 || n_pages < 1) throw std::runtime_error("debug_kv_write: empty problem");
         if (!qkv || !row_slot || !block_tables || !kpool || !vpool || (!row_pos && !ctx_len)) throw std::runtime_error("debug_kv_write: row_pos or ctx_len, and every other pointer");
@@ -449,13 +468,13 @@ void debug_kv_write(const HarnessCtx& c, int kv_type, int heads, int M, const fl
             check_pages(block_tables + (size_t)s * mp + pos / kPageTokens, 1, n_pages, "debug_kv_write: page id outside the pool");
         }
         const cudaStream_t st = c.st;
-        const size_t pool = (size_t)n_pages * heads * kPageTokens * kHeadDim, Hq = (size_t)heads * kHeadDim;
+        const size_t pool = (size_t)n_pages * heads * kv_block_bytes(sizeof(T)), Hq = (size_t)heads * kHeadDim;
         DBuf<int> dslot = to_dev(row_slot, M, st), dpos = to_dev(row_pos, M, st), dctx = to_dev(ctx_len, n_slots, st),
                   dbt = to_dev(block_tables, (size_t)n_slots * mp, st);
         DBuf<float> dqkv = to_dev(qkv, (size_t)M * 3 * Hq, st);
-        DBuf<T> dk = to_dev(static_cast<const T*>(kpool), pool, st), dv = to_dev(static_cast<const T*>(vpool), pool, st);
-        launch_kv_write<T>(dqkv.p, M, dslot.p, dpos.p, dctx.p, dbt.p, mp, dk.p, dv.p, heads, st);
-        dk.download(static_cast<T*>(kpool), pool, st); dv.download(static_cast<T*>(vpool), pool, st);
+        DBuf<uint8_t> dk = to_dev(static_cast<const uint8_t*>(kpool), pool, st), dv = to_dev(static_cast<const uint8_t*>(vpool), pool, st);
+        launch_kv_write<T>(dqkv.p, M, dslot.p, dpos.p, dctx.p, dbt.p, mp, reinterpret_cast<T*>(dk.p), reinterpret_cast<T*>(dv.p), heads, st);
+        dk.download(static_cast<uint8_t*>(kpool), pool, st); dv.download(static_cast<uint8_t*>(vpool), pool, st);
         CUDA_CHECK(cudaStreamSynchronize(st));
     });
 }

@@ -3,6 +3,7 @@
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
+#include "kv_fp8.cuh"
 
 namespace xtts {
 
@@ -86,6 +87,7 @@ void launch_head_norms(const float* X, const int* row_index, const float* lnf_w,
 
 // KV page layout (per layer):  K: [page][head][D/X][32 tok][X]   V: [page][head][32 tok][D]
 //   X = 16 bytes / sizeof(TKV)  (so one lane = one token reads 16 B, coalesced across the warp)
+//   TKV = __nv_fp8_e4m3: the same per token, each (page, head) block followed by 32 exponent bytes (kv_fp8.cuh)
 template <typename TKV>
 void launch_kv_write(const float* QKV, int M, const int* row_slot, const int* row_pos, const int* ctx_len,
                      const int* block_tables, int max_pages, TKV* kpool, TKV* vpool, int heads,
@@ -93,6 +95,7 @@ void launch_kv_write(const float* QKV, int M, const int* row_slot, const int* ro
 
 // decode attention over the paged cache, ctx = ctx_len[slot] + 1.  The kernel also appends the new token's K/V
 // (read from the QKV row) to the cache — the reshape_and_cache step — so no separate kv_write launch is needed.
+// TKV: float / bf16 / fp16 with TOut = TKV, or __nv_fp8_e4m3 with TOut bf16 / fp16.
 template <typename TKV, typename TOut>
 void launch_attn_decode(const float* QKV, const int* active, int M, const int* ctx_len,
                         const int* block_tables, int max_pages, TKV* kpool, TKV* vpool,
@@ -165,7 +168,8 @@ struct BeamArgs {
     float* latents; int H;                       // latent ring [NSLOT][tokens_cap][H]
 };
 // logprob -> select -> reorder (block tables, slot state) -> partial-page copy -> gather of finished groups (`gather`)
-// kpool / vpool: device arrays of the `layers` per-layer pool base pointers; elem = bytes per KV element
+// kpool / vpool: device arrays of the `layers` per-layer pool base pointers; elem = bytes per KV element (1: the fp8
+// format, whose copied tokens take their exponent bytes along)
 void launch_beam_step(const float* logits, int ld_logits, int V, SampleState s, BeamArgs a, void* const* kpool,
                       void* const* vpool, int layers, int heads, int elem, cudaStream_t st, bool gather = true);
 // the geometry the beam kernels take: V <= 2048, <= 128 KV pages per sequence, the gather's token list in shared memory

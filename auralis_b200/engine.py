@@ -97,26 +97,36 @@ def load_audio(source: Union[str, Path, bytes], sampling_rate: int) -> np.ndarra
 
 class XTTSv2Engine(BaseAsyncTTSEngine):
     model_type = "xtts"
+    kv_cache_dtype = "auto"
 
     def __init__(self, dims: XTTSDims, gpt_state, core_state, *, device: int = 0, devices: Optional[List[int]] = None,
                  precision: str = "fp16", max_concurrency: int = 64, max_speakers: int = 32,
                  tokenizer_file: Optional[str] = None, early_emit_tokens: int = 0, voc_segment: Optional[int] = None,
-                 tune_malloc: bool = False, **_):
+                 tune_malloc: bool = False, kv_cache_dtype: str = "auto", **_):
         """`devices=[0, 1, ...]`: data parallelism inside the product (north_star: "requests shard data-parallel across the
         8-GPU box") — one native engine (full weight replica, own scheduler thread, own streams) per listed GPU in THIS
         process; every text chunk goes to the engine with the least work in flight, results are re-assembled in request
-        order by the façade as before.  `max_concurrency` is per GPU.  Default: the single GPU `device`."""
+        order by the façade as before.  `max_concurrency` is per GPU.  Default: the single GPU `device`.
+        `kv_cache_dtype`: "auto" keeps the KV cache in the precision's own type (fp16 / bf16, fp32 in parity mode); "fp8"
+        (vLLM's name for it) stores it as e4m3 with one power-of-two scale per token and head — half the KV bytes read per
+        decode step and held per slot, at an accuracy cost (DESIGN.md §5).  fp8 needs precision "fp16" or "bf16"."""
         prec = {"fp32": native.PRECISION_FP32, "bf16": native.PRECISION_BF16, "fp16": native.PRECISION_FP16}[precision]
+        if kv_cache_dtype not in ("auto", "fp8"):
+            raise ValueError(f"kv_cache_dtype must be 'auto' or 'fp8', not {kv_cache_dtype!r}")
+        if kv_cache_dtype == "fp8" and precision == "fp32":
+            raise ValueError("kv_cache_dtype='fp8' needs precision 'fp16' or 'bf16' (the fp32 parity mode keeps an fp32 cache)")
         if tune_malloc:
             tune_host_allocator()
         self.dims = dims
         self.precision = precision
+        self.kv_cache_dtype = kv_cache_dtype
         self.devices = [int(d) for d in devices] if devices else [int(device)]
         if len(set(self.devices)) != len(self.devices):
             raise ValueError("devices must be distinct CUDA ordinals")
         self.device_index = self.devices[0]
         self.max_concurrency = max_concurrency
-        self.natives = [native.NativeEngine(dims, device=d, precision=prec, max_batch=max_concurrency, max_speakers=max_speakers)
+        self.natives = [native.NativeEngine(dims, device=d, precision=prec, max_batch=max_concurrency, max_speakers=max_speakers,
+                                            kv_fp8=kv_cache_dtype == "fp8")
                         for d in self.devices]
         self.native = self.natives[0]
         if len(self.natives) == 1:
@@ -192,11 +202,12 @@ class XTTSv2Engine(BaseAsyncTTSEngine):
         geometry: weights + per-slot state (paged KV for a full-length sequence, latent ring, token rows) x max_concurrency
         + the vocoder workspace.  Sets (and returns) `max_gb_for_vllm_model`, the attribute the reference's engine exposes."""
         g, v = self.dims.gpt, self.dims.voc
-        kv_elem = 2 if self.precision in ("bf16", "fp16") else 4
+        # bytes per cached (token, head) row of 64 dims: fp8 stores 64 e4m3 bytes + 1 exponent byte
+        kv_row = 65 if self.kv_cache_dtype == "fp8" else 64 * (2 if self.precision in ("bf16", "fp16") else 4)
         w_elem = 2 if self.precision in ("bf16", "fp16") else 4
         gpt_w = g.layers * (4 * g.hidden * g.hidden + 2 * g.hidden * g.ff) * w_elem
         pages = -(-(g.max_prompt_rows + g.max_audio_tokens) // 32)
-        per_slot = pages * 32 * 2 * g.layers * g.hidden * kv_elem + g.max_audio_tokens * g.hidden * 4 + 3 * g.max_audio_tokens * 4
+        per_slot = pages * 32 * 2 * g.layers * g.heads * kv_row + g.max_audio_tokens * g.hidden * 4 + 3 * g.max_audio_tokens * 4
         tz = v.z_frames(g.max_audio_tokens)
         widest = max((v.init_ch >> (i + 1)) * int(np.prod(v.up_rates[: i + 1])) for i in range(len(v.up_rates)))
         voc_ws = 8 * tz * (5 * widest * 4 + (5 * widest * 2 if self.precision in ("bf16", "fp16") else 0) + v.hop * 4)

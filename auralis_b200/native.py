@@ -296,7 +296,8 @@ class NativeEngine:
     """One engine = one GPU.  Thin, allocation-free wrapper over the C ABI."""
 
     def __init__(self, dims: XTTSDims, device: int = 0, precision: int = PRECISION_FP32, max_batch: int = 64,
-                 max_speakers: int = 16):
+                 max_speakers: int = 16, kv_fp8: bool = False):
+        """kv_fp8: the KV cache in fp8 e4m3 with per-token power-of-two scales (engine option "kv_fp8"; bf16 / fp16 only)."""
         self.lib = load_library()
         self.dims = dims
         self.cfg = make_config(dims, device, precision, max_batch, max_speakers)
@@ -307,6 +308,8 @@ class NativeEngine:
         if rc != 0:
             raise NativeError(f"xtts_create failed ({rc}): {self.lib.xtts_last_error().decode()}")
         self.h = h
+        if kv_fp8:
+            self.set_option("kv_fp8", 1)
 
     def _chk(self, rc: int, what: str):
         if rc != 0:
@@ -457,7 +460,7 @@ class NativeEngine:
             assert a.dtype == dt and a.flags.c_contiguous
         last = np.zeros(nb, np.int32)
         scores = np.zeros((nb, V), np.float32)
-        page = heads * 32 * 64 * (4 if kv_type == 0 else 2)
+        page = heads * self.KV_BLOCK_BYTES[kv_type]
         n_pages = kpool.nbytes // (layers * page)
         bm = XttsBeam(nb, float(sp.length_penalty), 1 if sp.do_sample else 0)
         cs = sp.c()
@@ -755,8 +758,10 @@ class NativeEngine:
                                                    _ip(st["tokens"]), _ip(st["sampled"])), "debug_sample_slots")
         return st
 
-    # KV type code of xtts_debug_attn_decode -> numpy dtype of the raw pool elements (bf16 as its uint16 bit pattern)
-    KV_DTYPES = {0: np.float32, 1: np.uint16, 2: np.float16}
+    # KV type code of xtts_debug_attn_decode -> numpy dtype of the raw pool elements (bf16 as its uint16 bit pattern; 3 / 4:
+    # the fp8 cache as raw bytes, e4m3 data then exponents per (page, head) block) and the bytes of one such block
+    KV_DTYPES = {0: np.float32, 1: np.uint16, 2: np.float16, 3: np.uint8, 4: np.uint8}
+    KV_BLOCK_BYTES = {0: 32 * 64 * 4, 1: 32 * 64 * 2, 2: 32 * 64 * 2, 3: 32 * 64 + 32, 4: 32 * 64 + 32}
 
     def debug_attn_decode(self, kv_type: int, heads: int, qkv, active, ctx_len, block_tables, kpool, vpool):
         """One decode-attention launch under the current options.  kpool / vpool: [n_pages, heads, 32 * 64] raw cache

@@ -254,7 +254,8 @@ int xtts_submit_beams(xtts_engine* e, uint64_t seq_id, const int32_t* text_ids, 
  * (equal across beams), seen [nb][ceil(V / 32)] bitmaps, block_tables [nb][max_pages] (max_pages <= 128), pool [nb *
  * max_pages] (the first state->n_free entries are free page ids, n_free >= nb), hist [cap][8][2] (parent, token) rows,
  * *state (the group state, transformers' beam-search tensors; sel_* / copy_* are this step's outputs), kpool / vpool
- * [layers][n_pages pages] in the layout of xtts_debug_attn_decode, kv_type 0 fp32, 1 bf16, 2 fp16.  Out: last_tok [nb],
+ * [layers][n_pages pages] in the layout of xtts_debug_attn_decode, kv_type 0 fp32, 1 bf16, 2 fp16, 3 fp8 (a copied token
+ * takes its exponent bytes along).  Out: last_tok [nb],
  * scores [nb][V] (the processed, accumulated scores the selection ranked).  logits: [1][V] when first, else [nb][V]. */
 typedef struct xtts_beam_state {
     float run_score[8], fin_score[8];
@@ -312,6 +313,12 @@ int xtts_fetch(xtts_engine* e, uint64_t seq_id, int32_t* tokens, float* wav, flo
  *                         (default) = the fast-mode vocoder's resblocks of 32 or 64 channels run as one fused kernel each
  *                         (resblock_tc) wherever it takes their geometry, 0 = as six tensor-core Conv1d launches, for
  *                         A/B timing and the bit-identity tests.  Bit-identical results.
+ *   "kv_fp8"              1 = the KV cache in fp8 e4m3 with one power-of-two scale per (token, head) for K and for V
+ *                         (layout at xtts_debug_attn_decode): half the KV bytes per slot and per decode step; 0 (default) =
+ *                         the cache in the precision's 16-bit type.  bf16 / fp16 precision only (fp32: XTTS_ERR_INVALID),
+ *                         on an idle engine only (a queued or running chunk: XTTS_ERR_STATE).  Switching reallocates the KV
+ *                         pools in the chosen format and drops the captured decode graphs; 0 again gives the bits of an
+ *                         engine that never switched.
  *   "attn_ctas_per_sm"    > 0 caps the decode-attention grid (each CTA walks several items); < 0: absolute grid size (tests)
  *   "profile"             1 = CUDA events around every launch (xtts_get_kernel_profile), "reset_stats" = zero the counters */
 int xtts_set_option(xtts_engine* e, const char* key, int64_t value);
@@ -382,9 +389,14 @@ int xtts_debug_sample_slots(xtts_engine* e, int32_t V, int32_t M, const int32_t*
                             int32_t* n_gen, int32_t* ctx_len, int32_t* finished, int32_t* last_tok, uint8_t* seen,
                             int32_t* tokens, int32_t* sampled);
 /* paged decode attention (one launch, appends each row's k / v): kv_type 0 fp32, 1 bf16, 2 fp16 (the output has the cache
- * type, returned as fp32).  active [M] (distinct slots < n_slots), ctx_len [n_slots], block_tables [n_slots][max_pages];
- * kpool / vpool: n_pages pages of raw cache-typed elements in the device layout (K [page][head][64/X][32 tok][X], X = 16 bytes
- * per element group; V [page][head][32 tok][64]), updated in place; qkv [M][3 * heads * 64]; out [M][heads * 64] */
+ * type, returned as fp32), 3 fp8 cache with fp16 output, 4 fp8 cache with bf16 output.  active [M] (distinct slots <
+ * n_slots), ctx_len [n_slots], block_tables [n_slots][max_pages]; kpool / vpool: n_pages pages of raw cache-typed elements in
+ * the device layout (K [page][head][64/X][32 tok][X], X = 16 bytes per element group; V [page][head][32 tok][64]), updated
+ * in place; qkv [M][3 * heads * 64]; out [M][heads * 64].
+ * fp8 (kv_type 3 / 4): each (page, head) block is 2080 bytes, the e4m3 data in the layout above (X = 16) followed by 32 int8
+ * exponents, one per token: value = e4m3 * 2^e.  Per (token, head), for K and V separately, e is the smallest integer with
+ * max |x| * 2^-e <= 448, clamped to [-128, 127] (-128 for an all-zero row), and the byte is e4m3(x * 2^-e) rounded to
+ * nearest even. */
 int xtts_debug_attn_decode(xtts_engine* e, int32_t kv_type, int32_t heads, int32_t M, const int32_t* active, int32_t n_slots,
                            const int32_t* ctx_len, const int32_t* block_tables, int32_t max_pages, int32_t n_pages,
                            void* kpool, void* vpool, const float* qkv, float* out);
@@ -421,7 +433,7 @@ int xtts_debug_norms(xtts_engine* e, int32_t out_type, int32_t M, int32_t H, con
                      const int32_t* n_gen);
 /* the prefill's paged-cache write: k / v of QKV row r (qkv [M][3 * heads * 64]) go to slot row_slot[r] at token position
  * p = row_pos ? row_pos[r] : ctx_len[row_slot[r]], page block_tables[slot][p / 32], rounded to kv_type (0 fp32, 1 bf16,
- * 2 fp16).  kpool / vpool: raw pools in the layout of xtts_debug_attn_decode, updated in place.  Rejected before any
+ * 2 fp16, 3 / 4 fp8 with its exponents).  kpool / vpool: raw pools in the layout of xtts_debug_attn_decode, updated in place.  Rejected before any
  * launch: a slot outside n_slots, a position outside the block table, a page id outside the pool. */
 int xtts_debug_kv_write(xtts_engine* e, int32_t kv_type, int32_t heads, int32_t M, const float* qkv, const int32_t* row_slot,
                         const int32_t* row_pos, int32_t n_slots, const int32_t* ctx_len, const int32_t* block_tables,
