@@ -691,12 +691,7 @@ void Engine::make_conv(ConvW& c, const std::string& prefix, bool transposed, boo
     const int d0 = (int)ref.shape[0], d1 = (int)ref.shape[1], K = (int)ref.shape[2];
     const int Cin = transposed ? d0 : d1, Cout = transposed ? d1 : d0;
     std::vector<float> t((size_t)Cin * K * Cout);
-    for (int ci = 0; ci < Cin; ++ci)
-        for (int co = 0; co < Cout; ++co)
-            for (int j = 0; j < K; ++j) {
-                const float x = transposed ? w[((size_t)ci * Cout + co) * K + j] : w[((size_t)co * Cin + ci) * K + j];
-                t[((size_t)ci * K + j) * Cout + co] = x;
-            }
+    conv_weight_ckc(w.data(), Cin, Cout, K, transposed, t.data());
     c.Cin = Cin; c.Cout = Cout; c.K = K;
     up(c.wt, t);
     if (has_bias) up(c.b, need(prefix + ".bias").data);
@@ -1418,9 +1413,8 @@ void Engine::run_vocoder_f32(const VocItem* it, int nb, int Lz, float* wav_dev_o
                              int64_t stage_cap) {
     const auto& c = cfg;
     cudaStream_t sv = st_voc;
-    const double s1 = (double)c.code_stride / (double)c.output_hop_length;
-    const double s2 = (double)c.output_sample_rate / (double)c.input_sample_rate;
-    const bool resample = c.output_sample_rate != c.input_sample_rate;
+    const double s1 = interp_scale1(c.code_stride, c.output_hop_length);
+    const double s2 = interp_scale2(c.input_sample_rate, c.output_sample_rate);
     const int nk = c.voc_n_rb;
     const size_t wav_stride = (size_t)Lz * voc_hop;
     for (int i0 = 0; i0 < nb;) {
@@ -1437,7 +1431,7 @@ void Engine::run_vocoder_f32(const VocItem* it, int nb, int Lz, float* wav_dev_o
         };
         InterpItem ii[kVocMaxItems];
         for (int k = 0; k < rn; ++k) ii[k] = interp_item(it[i0 + k]);
-        launch_interp(ii, rn, vz.p, nullptr, 0, c.voc_in_dim, Tz, s1, resample ? s2 : 1.0, sv);
+        launch_interp(ii, rn, vz.p, nullptr, 0, c.voc_in_dim, Tz, s1, s2, sv);
         dump("z", vz.p, (size_t)c.voc_in_dim * Tz);
         launch_conv1d(vz.p, conv_pre.wt.p, conv_pre.b.p, cb + cbias_off[0], nullptr, vpre.p, conv_pre.Cin, conv_pre.Cout, Tz,
                       conv_pre.K, 1, 1.0f, 1.0f, CONV_STORE, rn, cbias_stride, sv);
@@ -1451,8 +1445,8 @@ void Engine::run_vocoder_f32(const VocItem* it, int nb, int Lz, float* wav_dev_o
         };
         for (int i = 0; i < c.voc_n_up; ++i) {
             const ConvW& u = *ups[i];
-            launch_conv_transpose1d(cur, u.wt.p, u.b.p, cb + cbias_off[i + 1], X, nullptr, 0, 0.f, u.Cin, u.Cout, len, u.K,
-                                    c.voc_up_rates[i], in_scale, 0.1f, rn, cbias_stride, sv);
+            launch_conv_transpose1d(cur, u.wt.p, u.b.p, cb + cbias_off[i + 1], X, u.Cin, u.Cout, len, u.K, c.voc_up_rates[i],
+                                    in_scale, 0.1f, rn, cbias_stride, sv);
             len *= c.voc_up_rates[i];
             const int C = u.Cout;
             { char nm[16]; snprintf(nm, sizeof(nm), "up%d", i); dump(nm, X, (size_t)C * len); }
@@ -1489,9 +1483,8 @@ void Engine::run_vocoder_tc(const VocItem* it, int nb, int Lz, float* wav_dev_ou
                             int64_t stage_cap) {
     const auto& c = cfg;
     cudaStream_t sv = st_voc;
-    const double s1 = (double)c.code_stride / (double)c.output_hop_length;
-    const double s2 = (double)c.output_sample_rate / (double)c.input_sample_rate;
-    const bool resample = c.output_sample_rate != c.input_sample_rate;
+    const double s1 = interp_scale1(c.code_stride, c.output_hop_length);
+    const double s2 = interp_scale2(c.input_sample_rate, c.output_sample_rate);
     const float* cb = vcb.p;
     auto dump = [&](const char* name, const float* p, size_t n) {
         if (stage && stage_out && std::strcmp(stage, name) == 0) {
@@ -1514,7 +1507,7 @@ void Engine::run_vocoder_tc(const VocItem* it, int nb, int Lz, float* wav_dev_ou
     __half* XA = va16[0].p; __half* TA = va16[1].p; __half* RA[2] = {va16[2].p, va16[3].p}; __half* PA = va16[4].p;
     launch_atoms_zero_pads(vz16.p, nb * c.voc_in_dim / 8, lpad, Lz, sv, nb, lens);
     launch_atoms_zero_pads(PA, nb * c.voc_init_ch / 8, lpad, Lz, sv, nb, lens);
-    launch_interp(ii, nb, stage ? vz.p : nullptr, vz16.p, lpad, c.voc_in_dim, Lz, s1, resample ? s2 : 1.0, sv);
+    launch_interp(ii, nb, stage ? vz.p : nullptr, vz16.p, lpad, c.voc_in_dim, Lz, s1, s2, sv);
     if (stage) dump("z", vz.p, (size_t)c.voc_in_dim * Lz);
     // conv_pre: fp32 copy only for the stage tap; its activated fp16 atoms feed the first transposed conv
     conv_tc(conv_pre, vz16.p, cb + cbias_off[0], nullptr, stage ? vpre.p : nullptr, PA, Lz, lpad, 1, CONV_STORE, 1.0f);
@@ -2611,6 +2604,12 @@ int xtts_debug_cond(xtts_engine* e, int32_t op, const int32_t* dims, int32_t n_d
                     const float* const* in, const int64_t* in_len, int32_t n_in, float* out, int64_t out_len) {
     XTTS_TRY(e->impl->run_idle([&](const HarnessCtx& c) {
         xtts::cond_debug(c.cnd, op, dims, n_dims, scal, n_scal, in, in_len, n_in, out, out_len, c.st);
+    }))
+}
+int xtts_debug_vocoder(xtts_engine* e, int32_t op, const int32_t* dims, int32_t n_dims, const float* scal, int32_t n_scal,
+                       const float* const* in, const int64_t* in_len, int32_t n_in, float* out, int64_t out_len) {
+    XTTS_TRY(e->impl->run_idle([&](const HarnessCtx& c) {
+        xtts::debug_vocoder(c, op, dims, n_dims, scal, n_scal, in, in_len, n_in, out, out_len);
     }))
 }
 

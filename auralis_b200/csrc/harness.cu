@@ -112,6 +112,30 @@ void check_pages(const int32_t* ids, int n, int n_pages, const char* msg) {
         if (ids[i] < 0 || ids[i] >= n_pages) throw std::runtime_error(msg);
 }
 
+// A device copy of a host array of raw fp32 (U = uint32_t) or fp16 (uint16_t) bits with kGuardWords sentinels on each side;
+// fetch() brings the array back and throws if the kernel wrote a sentinel.
+constexpr int kGuardWords = 256;
+template <typename U>
+struct Guarded {
+    static constexpr U kBits = sizeof(U) == 4 ? (U)0x7fc5a5a5u : (U)0x7e5au;    // quiet-NaN payloads no kernel here produces
+    std::vector<U> h;
+    DBuf<U> d;
+    Guarded(const U* src, size_t n, cudaStream_t st) : h(n + 2 * kGuardWords, kBits) {
+        std::copy(src, src + n, h.begin() + kGuardWords);
+        d.alloc(h.size());
+        d.upload(h.data(), h.size(), st);
+    }
+    U* p() const { return d.p + kGuardWords; }
+    void fetch(U* dst, cudaStream_t st, const std::string& what) {
+        d.download(h.data(), h.size(), st);
+        CUDA_CHECK(cudaStreamSynchronize(st));
+        const size_t n = h.size() - 2 * kGuardWords;
+        for (int i = 0; i < kGuardWords; ++i)
+            if (h[i] != kBits || h[kGuardWords + n + i] != kBits) throw std::runtime_error("debug_vocoder: " + what + " wrote outside its output");
+        std::memcpy(dst, h.data() + kGuardWords, n * sizeof(U));
+    }
+};
+
 }  // namespace
 
 // One GEMM launch on private buffers.  The weights are converted and synchronised first; the activation conversion is the
@@ -670,6 +694,146 @@ void debug_resblock_tc(const HarnessCtx& c, int C, int K, const int32_t* dil, in
     dzs.download(zs, n32, st);
     if (pa) download_f32(dpa.p, 2, pa, n16, st);
     CUDA_CHECK(cudaStreamSynchronize(st));
+}
+
+// One launch of a CUDA-core vocoder kernel (launch_interp, launch_conv1d, launch_conv_transpose1d, launch_conv_post) on
+// private buffers, as the engine's vocoder passes.  Op layouts: include/xtts_b200.h.
+void debug_vocoder(const HarnessCtx& c, int op, const int32_t* dims, int n_dims, const float* scal, int n_scal,
+                   const float* const* in, const int64_t* in_len, int n_in, float* out, int64_t out_len) {
+    auto bad = [](const std::string& s) { return std::runtime_error("debug_vocoder: " + s); };
+    static const int kBaseDims[XTTS_VOC_N_OPS] = {9, 11, 9, 6};
+    if (op < 0 || op >= XTTS_VOC_N_OPS) throw bad("unknown op " + std::to_string(op));
+    if (n_dims < kBaseDims[op] || !dims) throw bad("op " + std::to_string(op) + " takes at least " + std::to_string(kBaseDims[op]) + " dims");
+    if ((n_scal && !scal) || (n_in > 0 && (!in || !in_len)) || !out) throw bad("NULL argument");
+    const int batch = dims[op == XTTS_VOC_INTERP ? 1 : op == XTTS_VOC_CONV_POST ? 3 : 5];
+    if (batch < 1 || batch > kVocMaxItems) throw bad("batch must be 1..32");
+    const int want_dims = op == XTTS_VOC_INTERP ? 9 + 5 * batch : op == XTTS_VOC_CONV_POST && dims[5] ? 6 + batch : kBaseDims[op];
+    const int want_scal = op == XTTS_VOC_INTERP ? batch : 2;
+    if (n_dims != want_dims || n_scal != want_scal)
+        throw bad("op " + std::to_string(op) + " takes " + std::to_string(want_dims) + " dims and " + std::to_string(want_scal) + " scalars");
+    for (int i = 0; i < n_dims; ++i)
+        if (dims[i] < 0) throw bad("negative dim");
+    auto d = [&](int i) { return (int64_t)dims[i]; };
+    auto pos = [&](std::initializer_list<int> idx) {
+        for (int i : idx) if (dims[i] < 1) throw bad("dim " + std::to_string(i) + " must be >= 1");
+    };
+    auto flag = [&](std::initializer_list<int> idx) {
+        for (int i : idx) if (dims[i] > 1) throw bad("dim " + std::to_string(i) + " is a flag: 0 or 1");
+    };
+    std::vector<int64_t> need;       // in_len each input must have
+    int64_t need_out = 0, n16 = 0;   // n16: floats of the INTERP atom image at the end of out
+    std::vector<InterpItem> items;
+    switch (op) {
+    case XTTS_VOC_INTERP: {          // C, batch, Lz, atoms, lpad, code_stride, hop, in_sr, out_sr, [T, T0, T1, z0, nz] x batch
+        pos({0, 2, 5, 6, 7, 8});
+        flag({3});
+        if (d(3) && (d(0) % 8 != 0 || d(4) < kAtomPadL + d(2))) throw bad("the atom image needs C % 8 == 0 and lpad >= 64 + Lz");
+        for (int i = 0; i < batch; ++i) {
+            const int32_t* it = dims + 9 + 5 * i;
+            const float r0 = scal[i];
+            if (it[0] < 1 || it[2] < 1) throw bad("item " + std::to_string(i) + ": T and T1 must be >= 1");
+            if (!(r0 >= 0.f) || r0 > 1e4f || (r0 > 0.f && it[1] < 1)) throw bad("item " + std::to_string(i) + ": r0 must be 0, or > 0 with T0 >= 1");
+            if (it[4] > d(2)) throw bad("item " + std::to_string(i) + ": nz > Lz");
+            InterpItem ii{nullptr, it[0], it[2], it[3], it[4]};
+            ii.T0 = it[1]; ii.r0 = r0;
+            items.push_back(ii);
+            need.push_back(d(0) * it[0]);
+        }
+        n16 = d(3) ? batch * d(0) * d(4) : 0;
+        need_out = batch * d(0) * d(2) + n16;
+        break;
+    }
+    case XTTS_VOC_CONV1D:            // Cin, Cout, K, dil, L, batch, mode, has_bias, has_cbias, cbias_stride, has_resid
+        pos({0, 1, 3, 4});
+        flag({6, 7, 8, 10});
+        if (d(2) != 3 && d(2) != 7 && d(2) != 11) throw bad("conv1d takes K 3, 7 or 11");
+        if ((d(2) - 1) / 2 * d(3) > 64) throw bad("conv1d halo (K-1)/2*dil above 64");
+        if (d(8) && d(9) < d(1)) throw bad("cbias_stride < Cout");
+        need = {batch * d(0) * d(4), d(1) * d(0) * d(2)};
+        if (d(7)) need.push_back(d(1));
+        if (d(8)) need.push_back(batch * d(9));
+        if (d(10)) need.push_back(batch * d(1) * d(4));
+        need_out = batch * d(1) * d(4);
+        break;
+    case XTTS_VOC_CONV_T:            // Cin, Cout, u, K, Lin, batch, has_bias, has_cbias, cbias_stride
+        pos({0, 1, 2, 4});
+        flag({6, 7});
+        if (d(3) != 2 * d(2) || d(2) % 2 != 0 || 128 % d(2) != 0 || d(2) > 32)
+            throw bad("conv_transpose1d takes K = 2u with u even, dividing 128 and <= 32");
+        if (d(7) && d(8) < d(1)) throw bad("cbias_stride < Cout");
+        need = {batch * d(0) * d(4), d(0) * d(1) * d(3)};
+        if (d(6)) need.push_back(d(1));
+        if (d(7)) need.push_back(batch * d(8));
+        need_out = batch * d(1) * d(4) * d(2);
+        break;
+    case XTTS_VOC_CONV_POST:         // Cin, K, L, batch, wav_stride, has_lens, [L_i] x batch
+        pos({0, 1, 2});
+        flag({5});
+        if (d(1) % 2 == 0 || d(0) * d(1) > 12288) throw bad("conv_post takes an odd K with Cin * K <= 12288");
+        if (d(4) < d(2)) throw bad("wav_stride < L");
+        for (int i = 0; i < batch && d(5); ++i)
+            if (d(6 + i) > d(2)) throw bad("item " + std::to_string(i) + ": length > L");
+        need = {batch * d(0) * d(2), d(0) * d(1)};
+        need_out = batch * d(4);
+        break;
+    }
+    if (n_in != (int)need.size()) throw bad("op " + std::to_string(op) + " takes " + std::to_string(need.size()) + " inputs");
+    for (int i = 0; i < n_in; ++i) {
+        if (in_len[i] != need[i])
+            throw bad("input " + std::to_string(i) + " has " + std::to_string(in_len[i]) + " floats, expected " + std::to_string(need[i]));
+        if (!in[i]) throw bad("input " + std::to_string(i) + " is NULL");
+    }
+    if (out_len < 1 || out_len != need_out) throw bad("out has " + std::to_string(out_len) + " floats, expected " + std::to_string(need_out));
+
+    const cudaStream_t st = c.st;
+    std::vector<DBuf<float>> din(n_in);
+    for (int i = 0; i < n_in; ++i) din[i] = to_dev(in[i], (size_t)in_len[i], st);
+    auto I = [&](int i) -> const float* { return din[i].p; };
+    const size_t n32 = (size_t)(out_len - n16);
+    Guarded<uint32_t> o32(reinterpret_cast<const uint32_t*>(out), n32, st);
+    float* o = reinterpret_cast<float*>(o32.p());
+    const int* D = dims;
+    DBuf<float> dw;                  // conv weights as the engine packs them
+    switch (op) {
+    case XTTS_VOC_INTERP: {
+        std::vector<uint16_t> h16(n16);
+        for (int64_t i = 0; i < n16; ++i) { const __half_raw r = __float2half_rn(out[n32 + i]); h16[i] = r.x; }
+        Guarded<uint16_t> o16(h16.data(), h16.size(), st);
+        for (int i = 0; i < batch; ++i) items[i].lat = I(i);
+        launch_interp(items.data(), batch, o, D[3] ? reinterpret_cast<__half*>(o16.p()) : nullptr, D[4], D[0], D[2],
+                      interp_scale1(D[5], D[6]), interp_scale2(D[7], D[8]), st);
+        if (n16) {
+            o16.fetch(h16.data(), st, "interp (atoms)");
+            for (int64_t i = 0; i < n16; ++i) { __half_raw r; r.x = h16[i]; out[n32 + i] = __half2float(__half(r)); }
+        }
+        break;
+    }
+    case XTTS_VOC_CONV1D: {
+        std::vector<float> wt(d(1) * d(0) * d(2));
+        conv_weight_ckc(in[1], D[0], D[1], D[2], false, wt.data());
+        dw = to_dev(wt.data(), wt.size(), st);
+        int k = 2;
+        const float* bias = D[7] ? I(k++) : nullptr;
+        const float* cbias = D[8] ? I(k++) : nullptr;
+        const float* resid = D[10] ? I(k++) : nullptr;
+        launch_conv1d(I(0), dw.p, bias, cbias, resid, o, D[0], D[1], D[4], D[2], D[3], scal[0], scal[1], D[6], batch, D[9], st);
+        break;
+    }
+    case XTTS_VOC_CONV_T: {
+        std::vector<float> wt(d(0) * d(1) * d(3));
+        conv_weight_ckc(in[1], D[0], D[1], D[3], true, wt.data());
+        dw = to_dev(wt.data(), wt.size(), st);
+        int k = 2;
+        const float* bias = D[6] ? I(k++) : nullptr;
+        const float* cbias = D[7] ? I(k++) : nullptr;
+        launch_conv_transpose1d(I(0), dw.p, bias, cbias, o, D[0], D[1], D[4], D[3], D[2], scal[0], scal[1], batch, D[8], st);
+        break;
+    }
+    case XTTS_VOC_CONV_POST:
+        launch_conv_post(I(0), I(1), o, D[0], D[2], D[1], scal[0], scal[1], batch, st, D[5] ? D + 6 : nullptr, D[4]);
+        break;
+    }
+    o32.fetch(reinterpret_cast<uint32_t*>(out), st, "op " + std::to_string(op));
 }
 
 }  // namespace xtts

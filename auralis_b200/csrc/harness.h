@@ -47,6 +47,8 @@ void debug_conv_tc(const HarnessCtx& c, int up, int Cin, int Cout, int K, int di
 void debug_resblock_tc(const HarnessCtx& c, int C, int K, const int32_t* dil, int batch, int L, const int32_t* item_len,
                        const float* w, const float* bias, const float* x, int mode, float scale16, int max_ctas, int fused,
                        float* zs, float* pa);
+void debug_vocoder(const HarnessCtx& c, int op, const int32_t* dims, int n_dims, const float* scal, int n_scal,
+                   const float* const* in, const int64_t* in_len, int n_in, float* out, int64_t out_len);
 void debug_beam_step(const HarnessCtx& c, int kv_type, int heads, int layers, int V, const xtts_sampling& sp,
                      const xtts_beam& bm, int first, int advance, const float* logits, int32_t* n_gen, int32_t* ctx_len,
                      int32_t* last_tok, uint32_t* seen, int max_pages, int32_t* block_tables, int n_pages, int32_t* pool,

@@ -195,7 +195,14 @@ struct InterpItem { const float* lat; int T, T1, z0, nz; int T0 = 0; float r0 = 
 void launch_interp(const InterpItem* items, int batch, float* z32, __half* z16, int lpad, int C, int Lz, double scale1,
                    double scale2, cudaStream_t st);
 
+// the scale factors of the two interpolations (HifiDecoder.forward): code_stride / hop, then out_sr / in_sr (1: no resampling)
+inline double interp_scale1(int code_stride, int hop) { return (double)code_stride / (double)hop; }
+inline double interp_scale2(int in_sr, int out_sr) { return in_sr != out_sr ? (double)out_sr / (double)in_sr : 1.0; }
+
 enum : int { CONV_STORE = 0, CONV_ACCUM = 1 };
+// Conv1d weight [Cout][Cin][K] (transposed = false) or ConvTranspose1d weight [Cin][Cout][K] (true), torch's layouts ->
+// w_t [Cin][K][Cout], the layout launch_conv1d and launch_conv_transpose1d read
+void conv_weight_ckc(const float* w, int Cin, int Cout, int K, bool transposed, float* w_t);
 // out[co][t] (=|+=) bias[co] + cbias[co] + resid[co][t] + sum_{ci,j} w[ci][j][co] * act(in_scale*x[ci][t+(j-(K-1)/2)*dil])
 //   act = leaky_relu(slope) (slope==1 -> identity).  w is pre-transposed to [Cin][K][Cout].
 void launch_conv1d(const float* x, const float* w_t, const float* bias, const float* cbias, const float* resid,
@@ -240,10 +247,9 @@ void launch_convT_tc(const __half* a16, const __half* wblob, const ConvTcPlan& p
 void launch_atoms_zero_pads(__half* buf, int planes_total, int lpad, int L, cudaStream_t st, int batch = 1,
                             const int* item_len = nullptr);
 // transposed conv, stride u, kernel K = 2u, padding (K-u)/2;  w pre-transposed to [Cin][K][Cout]
-// out16 (optional): lrelu(out, slope16) as fp16 atoms with lpad16 rows per plane
-void launch_conv_transpose1d(const float* x, const float* w_t, const float* bias, const float* cbias, float* out,
-                             __half* out16, int lpad16, float slope16, int Cin, int Cout, int Lin, int K, int u,
-                             float in_scale, float slope, int batch, int cbias_batch_stride, cudaStream_t st);
+void launch_conv_transpose1d(const float* x, const float* w_t, const float* bias, const float* cbias, float* out, int Cin,
+                             int Cout, int Lin, int K, int u, float in_scale, float slope, int batch, int cbias_batch_stride,
+                             cudaStream_t st);
 // wav[t] = tanh(sum w[ci][j] * lrelu(in_scale*x[ci][t+j-3], slope));  x [batch][Cin][L], wav [batch][wav_stride (0 = L)];
 // item_len as above
 void launch_conv_post(const float* x, const float* w, float* wav, int Cin, int L, int K, float in_scale, float slope,

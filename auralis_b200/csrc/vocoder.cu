@@ -23,8 +23,9 @@ __device__ __forceinline__ float lrelu(float v, float slope) { return v > 0.f ? 
 // ------------------------------------------------------------------------------------------------
 // fused double (triple, with a speaking rate) linear interpolation + transpose:  latents [T][C]  ->  z [C][Tz]
 // ------------------------------------------------------------------------------------------------
-// The roundings of this stage are spelled out with intrinsics (no contraction left to the compiler), so that the two-level
-// code keeps its exact arithmetic whatever code surrounds it: chunks without a speaking rate get the same bits as before it.
+// The roundings of this stage are spelled out with intrinsics (no contraction left to the compiler): every level rounds
+// l0 * x0 + l1 * x1 as ATen's CPU kernel does, so z equals the chained F.interpolate calls bit for bit, with or without a
+// speaking rate (tests/test_gpu_vocoder_f32.py), whatever code surrounds it.
 __device__ __forceinline__ void lin_src(int dst, float rscale, int in_len, int& i0, int& i1, float& l0, float& l1) {
     float src = __fmaf_rn(rscale, (float)dst + 0.5f, -0.5f);
     if (src < 0.f) src = 0.f;
@@ -35,9 +36,9 @@ __device__ __forceinline__ void lin_src(int dst, float rscale, int in_len, int& 
     l0 = 1.0f - l1;
 }
 
-// speed stage, channel c: frame b of the time-scaled latents, then frame a of the first chunk-level interpolation on them;
 // l0 * x0 + l1 * x1 rounded as ATen's CPU kernel does, fma(l0, x0, l1 * x1)
 __device__ __forceinline__ float lerp_aten(float l0, float x0, float l1, float x1) { return __fmaf_rn(l0, x0, __fmul_rn(l1, x1)); }
+// speed stage, channel c: frame b of the time-scaled latents, then frame a of the first chunk-level interpolation on them
 __device__ __forceinline__ float speed_frame(const float* __restrict__ lat, int b, float r0, int T, int C, int c) {
     int i0, i1; float l0, l1;
     lin_src(b, r0, T, i0, i1, l0, l1);
@@ -73,13 +74,13 @@ interp_kernel(const InterpBatch B, float* __restrict__ z_, uint4* __restrict__ z
                 const float za = speed_level1(lat, a0, r1, it.T0, it.r0, T, C, c);
                 const float zb = speed_level1(lat, a1, r1, it.T0, it.r0, T, C, c);
                 v = lerp_aten(m0, za, m1, zb);
-            } else {                                    // n0 x0 + n1 x1 = fma(n1, x1, n0 x0);  m0 za + m1 zb = fma(m0, za, m1 zb)
+            } else {                                    // two levels, the latents read directly
                 int b0, b1; float n0, n1;
                 lin_src(a0, r1, T, b0, b1, n0, n1);
-                const float za = __fmaf_rn(n1, lat[(size_t)b1 * C + c], __fmul_rn(n0, lat[(size_t)b0 * C + c]));
+                const float za = lerp_aten(n0, lat[(size_t)b0 * C + c], n1, lat[(size_t)b1 * C + c]);
                 lin_src(a1, r1, T, b0, b1, n0, n1);
-                const float zb = __fmaf_rn(n1, lat[(size_t)b1 * C + c], __fmul_rn(n0, lat[(size_t)b0 * C + c]));
-                v = __fmaf_rn(m0, za, __fmul_rn(m1, zb));
+                const float zb = lerp_aten(n0, lat[(size_t)b0 * C + c], n1, lat[(size_t)b1 * C + c]);
+                v = lerp_aten(m0, za, m1, zb);
             }
         }
         tile[ty + 8 * k][tx] = v;                       // tile[j][c]
@@ -203,8 +204,8 @@ constexpr int UP_T = 128, UP_CI = 8, UP_CO = 16;
 
 __global__ void __launch_bounds__(UP_T)
 conv_transpose1d_kernel(const float* __restrict__ x_, const float* __restrict__ w_t, const float* __restrict__ bias,
-                        const float* __restrict__ cbias_, float* __restrict__ out_, uint4* __restrict__ out16_, int lpad16,
-                        float slope16, int Cin, int Cout, int Lin, int K, int u, float in_scale, float slope, int cbias_bs) {
+                        const float* __restrict__ cbias_, float* __restrict__ out_, int Cin, int Cout, int Lin, int K, int u,
+                        float in_scale, float slope, int cbias_bs) {
     extern __shared__ __align__(16) float smem[];
     const float* x = x_ + (size_t)blockIdx.z * Cin * Lin;
     float* out = out_ + (size_t)blockIdx.z * Cout * Lin * u;
@@ -268,22 +269,6 @@ conv_transpose1d_kernel(const float* __restrict__ x_, const float* __restrict__ 
                 out[(size_t)co * Lout + t] = acc[c];
             }
         }
-        if (out16_) {                                   // activated fp16 copy for the tensor-core resblocks
-#pragma unroll
-            for (int g = 0; g < UP_CO / 8; ++g) {
-                if (co0 + 8 * g < Cout) {
-                    const float* a = acc + 8 * g;
-                    __half2 h0 = __floats2half2_rn(lrelu(a[0], slope16), lrelu(a[1], slope16));
-                    __half2 h1 = __floats2half2_rn(lrelu(a[2], slope16), lrelu(a[3], slope16));
-                    __half2 h2 = __floats2half2_rn(lrelu(a[4], slope16), lrelu(a[5], slope16));
-                    __half2 h3 = __floats2half2_rn(lrelu(a[6], slope16), lrelu(a[7], slope16));
-                    uint4 pk;
-                    pk.x = *reinterpret_cast<uint32_t*>(&h0); pk.y = *reinterpret_cast<uint32_t*>(&h1);
-                    pk.z = *reinterpret_cast<uint32_t*>(&h2); pk.w = *reinterpret_cast<uint32_t*>(&h3);
-                    out16_[((size_t)blockIdx.z * (Cout / 8) + (co0 / 8 + g)) * lpad16 + kAtomPadL + t] = pk;
-                }
-            }
-        }
     }
 }
 
@@ -342,6 +327,13 @@ void conv1d_dispatch(const float* x, const float* w_t, const float* bias, const 
 
 }  // namespace
 
+void conv_weight_ckc(const float* w, int Cin, int Cout, int K, bool transposed, float* w_t) {
+    for (int ci = 0; ci < Cin; ++ci)
+        for (int co = 0; co < Cout; ++co)
+            for (int j = 0; j < K; ++j)
+                w_t[((size_t)ci * K + j) * Cout + co] = transposed ? w[((size_t)ci * Cout + co) * K + j] : w[((size_t)co * Cin + ci) * K + j];
+}
+
 void launch_interp(const InterpItem* items, int batch, float* z32, __half* z16, int lpad, int C, int Lz, double scale1,
                    double scale2, cudaStream_t st) {
     if (batch < 1 || batch > kVocMaxItems) throw CudaError("interp: batch out of range");
@@ -372,17 +364,16 @@ void launch_conv1d(const float* x, const float* w_t, const float* bias, const fl
     }
 }
 
-void launch_conv_transpose1d(const float* x, const float* w_t, const float* bias, const float* cbias, float* out,
-                             __half* out16, int lpad16, float slope16, int Cin, int Cout, int Lin, int K, int u,
-                             float in_scale, float slope, int batch, int cbias_bs, cudaStream_t st) {
+void launch_conv_transpose1d(const float* x, const float* w_t, const float* bias, const float* cbias, float* out, int Cin,
+                             int Cout, int Lin, int K, int u, float in_scale, float slope, int batch, int cbias_bs,
+                             cudaStream_t st) {
     if (K != 2 * u || (u & 1)) throw CudaError("conv_transpose1d: only kernel == 2*stride with even stride is supported");
     if (UP_T % u != 0) throw CudaError("conv_transpose1d: stride must divide 128");
     const int XS = UP_T / u + 3;
     const size_t smem = (size_t)(((UP_CI * XS + 3) / 4) * 4 + UP_CI * K * (UP_CO + 4)) * sizeof(float);
     dim3 grid(ceil_div(Lin * u, UP_T), ceil_div(Cout, UP_CO), batch);
     ProfScope ps(KF_CONVT, st, 4.0 * Cin * Cout * (double)Lin * u * batch, 4.0 * (batch * ((double)Lin * Cin + (double)Lin * u * Cout) + (double)Cin * Cout * K));
-    if (out16 && (Cout % 8 != 0)) throw CudaError("conv_transpose1d: atoms output needs Cout % 8 == 0");
-    conv_transpose1d_kernel<<<grid, UP_T, smem, st>>>(x, w_t, bias, cbias, out, reinterpret_cast<uint4*>(out16), lpad16, slope16, Cin, Cout, Lin, K, u, in_scale, slope, cbias_bs);
+    conv_transpose1d_kernel<<<grid, UP_T, smem, st>>>(x, w_t, bias, cbias, out, Cin, Cout, Lin, K, u, in_scale, slope, cbias_bs);
     COUNT_LAUNCH(); KERNEL_CHECK();
 }
 

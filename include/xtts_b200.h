@@ -537,6 +537,41 @@ int xtts_debug_resblock_tc(xtts_engine* e, int32_t C, int32_t K, const int32_t* 
 int xtts_debug_cond(xtts_engine* e, int32_t op, const int32_t* dims, int32_t n_dims, const float* scal, int32_t n_scal,
                     const float* const* in, const int64_t* in_len, int32_t n_in, float* out, int64_t out_len);
 
+/* one CUDA-core vocoder kernel (csrc/vocoder.cu: the fp32 parity-mode convolutions, and the interpolation and conv_post of
+ * every precision) on caller data, through its launcher with the arguments the engine passes.  As in xtts_debug_cond:
+ * dims [n_dims] and scal [n_scal] are the op's parameters, in [n_in] its fp32 inputs of in_len[i] floats each, and out
+ * [out_len] is in/out: uploaded before the launch (the accumulate base, and what every element the kernel does not write
+ * comes back as) and downloaded after it, with 256 sentinel words on each side of its device copy (the fp16 atom image
+ * too); a kernel that writes one of them is an error.  Conv weights come in torch's layout and are packed as the engine
+ * packs them at weight load.  Rejected before any launch: an unknown op, a wrong n_dims / n_scal / n_in, batch outside
+ * 1..32, a dim out of range, any in_len or out_len other than the one the dims imply, a NULL pointer.  Layouts are
+ * row-major; per op, "dims; scal; inputs -> out":
+ *   INTERP     C, batch, Lz, atoms (0 / 1), lpad, code_stride, hop, in_sr, out_sr, then per item T, T0, T1, z0, nz;
+ *              per item r0; per item its latents [T][C] -> z [batch][C][Lz], then with atoms the fp16 atom image
+ *              [batch][C/8][lpad][8] (as fp32).  Item i writes z-frames z0 .. z0 + nz - 1 of its chunk to columns
+ *              0 .. nz - 1 (atom rows 64 .. 64 + nz - 1): linear interpolations with scale1 = code_stride / hop, clamp
+ *              length T1, then scale2 = out_sr / in_sr (1 when equal), after a speed stage to T0 frames at source step r0
+ *              when r0 > 0 (InterpItem, csrc/kernels.h).  T, T1 >= 1, T0 >= 1 with r0 > 0, z0 >= 0, 0 <= nz <= Lz;
+ *              atoms need C % 8 == 0 and lpad >= 64 + Lz.
+ *   CONV1D     Cin, Cout, K (3, 7, 11), dil, L, batch, mode (0 store, 1 accumulate), has_bias, has_cbias, cbias_stride,
+ *              has_resid; in_scale, slope; x [batch][Cin][L], w [Cout][Cin][K], then bias [Cout], cbias
+ *              [batch][cbias_stride] (>= Cout), resid [batch][Cout][L] as flagged -> out [batch][Cout][L] (=|+=)
+ *              conv(lrelu(in_scale * x, slope), dilation dil, "same" padding) + bias + cbias + resid; (K-1)/2*dil <= 64
+ *   CONV_T     Cin, Cout, u, K, Lin, batch, has_bias, has_cbias, cbias_stride; in_scale, slope; x [batch][Cin][Lin],
+ *              w [Cin][Cout][K], then bias, cbias as flagged -> out [batch][Cout][Lin*u] = ConvTranspose1d(lrelu(in_scale
+ *              * x, slope), stride u, padding u/2) + bias + cbias; K = 2u, u even, dividing 128 and <= 32
+ *   CONV_POST  Cin, K (odd, Cin * K <= 12288), L, batch, wav_stride (>= L), has_lens, then L_i per item if has_lens;
+ *              in_scale, slope; x [batch][Cin][L], w [Cin][K] -> wav [batch][wav_stride], wav[i][t] = tanh(conv(lrelu(
+ *              in_scale * x_i, slope), "same" padding)) for t < L_i, item i's signal ending at L_i (0 <= L_i <= L, all L
+ *              without lens) */
+#define XTTS_VOC_INTERP 0
+#define XTTS_VOC_CONV1D 1
+#define XTTS_VOC_CONV_T 2
+#define XTTS_VOC_CONV_POST 3
+#define XTTS_VOC_N_OPS 4
+int xtts_debug_vocoder(xtts_engine* e, int32_t op, const int32_t* dims, int32_t n_dims, const float* scal, int32_t n_scal,
+                       const float* const* in, const int64_t* in_len, int32_t n_in, float* out, int64_t out_len);
+
 #ifdef __cplusplus
 }
 #endif
